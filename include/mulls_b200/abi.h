@@ -470,7 +470,12 @@ int mulls_pose_write(const char *path, const double pose[16], int overwrite);
 void *mulls_host_alloc(size_t bytes);
 void mulls_host_free(void *p);
 
-/* Runtime tunables (integers), e.g. "start_level", "pairs_in_flight". Returns MULLS_E_ARG if unknown. */
+/* Runtime tunables (integers). Returns MULLS_E_ARG for any other name.
+ *   "use_graph"     1 (default): the iteration loop as one CUDA graph launch, or as one cooperative kernel for batches
+ *                   whose chunks all find a co-resident block; 0: the host launch loop (per-kernel timing events)
+ *   "host_pack"     repack host clouds to the packed wire format on the host cores before the copy:
+ *                   0 never, 1 always, 2 (default) when a call ships at least 2^18 points
+ *   "pack_threads"  the process-wide packing pool has at least n workers (n <= 0: MULLS_PACK_THREADS or cores/16, 2..8) */
 int mulls_set_tunable(mulls_ctx *ctx, const char *name, int value);
 
 #ifdef __cplusplus

@@ -123,7 +123,8 @@ __global__ void __launch_bounds__(kIngestBlock, kUndistort ? 4 : 6) k_ingest_tra
 
 // ---- k_pair_setup: one thread per pair. Intersection bbox (utility.hpp:858-866, pad 1.0,
 //      cregistration.hpp:2907-2916), grid geometry, initial state (:1144-1164).
-__global__ void k_pair_setup(DeviceArrays A, int n_pairs, float h0_min) {
+constexpr float kH0Min = 0.125f; // smallest level-0 cell (m); doubled until the grid spans the pair
+__global__ void k_pair_setup(DeviceArrays A, int n_pairs) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= n_pairs) return;
     const PairConst &pc = A.pc[p];
@@ -166,10 +167,10 @@ __global__ void k_pair_setup(DeviceArrays A, int n_pairs, float h0_min) {
         ext = fmax(ext, gmax[d] - gmin[d]);
     }
     const int ncell = 1 << kCoordBits;
-    float h0 = h0_min;
+    float h0 = kH0Min;
     while ((ext + 8.0 * h0) * 1.001 > (double)h0 * (ncell - 4)) h0 *= 2.0f;
     ps.h0 = h0;
-    ps.inv_h0 = 1.0f / h0; // power of two times h0_min: exact when h0_min is a power of two
+    ps.inv_h0 = 1.0f / h0; // a power of two: exact
     for (int d = 0; d < 3; ++d) ps.origin[d] = (float)gmin[d] - 2.0f * h0;
     // number of levels: the top level's guaranteed coverage 0.999*h must reach the largest search
     // radius 2.5*dis_thre_unit (filter_dis_times, cregistration.hpp:1707)
@@ -206,7 +207,7 @@ __global__ void k_pair_setup(DeviceArrays A, int n_pairs, float h0_min) {
 
 // ---- k_make_keys: intersection filter (cfilter.hpp:950-981: strictly inside) + 64-bit sort key
 //      [pair*12+seg | morton36(cell)]; filtered-out points sort to the very end.
-__global__ void __launch_bounds__(kIngestBlock) k_make_keys(DeviceArrays A, int sort_sources) {
+__global__ void __launch_bounds__(kIngestBlock) k_make_keys(DeviceArrays A) {
     const ChunkDesc cd = A.in_chunks[blockIdx.x];
     const PairConst &pc = A.pc[cd.pair];
     PairState &ps = A.ps[cd.pair];
@@ -232,8 +233,6 @@ __global__ void __launch_bounds__(kIngestBlock) k_make_keys(DeviceArrays A, int 
             cy = min(max(cy, 0), hi);
             cz = min(max(cz, 0), hi);
             key = ((uint64_t)(cd.pair * kNumSegs + seg) << 36) | morton36((uint32_t)cx, (uint32_t)cy, (uint32_t)cz);
-            // (study switch: sources left in the caller's order — nothing but the search's locality depends on it)
-            if (!sort_sources && seg >= kNumClasses) key = ((uint64_t)(cd.pair * kNumSegs + seg) << 36) | (uint64_t)local;
         }
         A.keys_a[gi] = key;
         A.vals_a[gi] = (uint32_t)gi;
@@ -531,9 +530,10 @@ __global__ void __launch_bounds__(256) k_hash_build(DeviceArrays A, const uint64
 
 // k_hash_layout: single block. Power-of-two table per (pair, class) with load factor <= 0.5, carved out
 // of the pool in order; flags overflow instead of writing out of bounds.
-__global__ void k_hash_layout(DeviceArrays A, int n_pairs, int slack) {
+constexpr uint64_t kHashSlack = 4; // first choice: table capacity >= kHashSlack x cells
+__global__ void k_hash_layout(DeviceArrays A, int n_pairs) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    // load factor <= 1/slack if the pool allows it (slack 4: a miss costs ~1.4 probes instead of 2.5 at 1/2), else
+    // load factor <= 1/kHashSlack if the pool allows it (a miss costs ~1.4 probes instead of 2.5 at 1/2), else
     // <= 0.5, else <= 0.8 (longer probe chains, same results), else give up
     for (int attempt = 0; attempt < 3; ++attempt) {
         uint64_t used = 0;
@@ -541,7 +541,7 @@ __global__ void k_hash_layout(DeviceArrays A, int n_pairs, int slack) {
         for (int p = 0; p < n_pairs && !overflow; ++p) {
             PairState &ps = A.ps[p];
             for (int c = 0; c < kNumClasses; ++c) {
-                const uint64_t want = (attempt == 0) ? (uint64_t)slack * ps.hash_entries[c] : (attempt == 1) ? 2ull * ps.hash_entries[c] : (5ull * ps.hash_entries[c]) / 4 + 1;
+                const uint64_t want = (attempt == 0) ? kHashSlack * ps.hash_entries[c] : (attempt == 1) ? 2ull * ps.hash_entries[c] : (5ull * ps.hash_entries[c]) / 4 + 1;
                 uint32_t cap = 16;
                 while (cap < want) cap <<= 1;
                 if (used + cap > A.hash_pool_entries) {

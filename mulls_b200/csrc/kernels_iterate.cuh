@@ -72,9 +72,15 @@ __global__ void __launch_bounds__(256) k_live_init(DeviceArrays A) {
 
 // ------------------------------------------------------------------------------------------------
 // exact 1-NN within radius on the multi-level hashed grid of one target class: search_core.cuh
-// (__host__ __device__; the CPU suite runs the same functions against a brute-force scan)
+// (__host__ __device__; the CPU suite runs the same functions against a brute-force scan). The core takes its search
+// parameters as arguments; every kernel here passes these values.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ GridView grid_of(const DeviceArrays &A, const PairConst &pc, const PairState &ps, int c, int leaf_count) {
+constexpr int kStartLevel0 = 5;      // level the walk starts from (clamped to the grid's levels)
+constexpr int kLeafCount = 32;       // a cell with more points is split into its children
+constexpr int kDeferFromIter = 3;    // k_search queues the small cells of a block (one scan loop per block) from here on
+constexpr float kReseedCells = 4.0f; // a previous match farther than this many level-0 cells is challenged by a greedy descent
+
+__device__ __forceinline__ GridView grid_of(const DeviceArrays &A, const PairConst &pc, const PairState &ps, int c) {
     GridView g;
     g.table = A.hash + ps.hash_base[c];
     g.mask = ps.hash_mask[c];
@@ -83,7 +89,7 @@ __device__ __forceinline__ GridView grid_of(const DeviceArrays &A, const PairCon
     g.ox = ps.origin[0], g.oy = ps.origin[1], g.oz = ps.origin[2];
     g.h0 = ps.h0, g.inv_h0 = ps.inv_h0;
     g.n_levels = ps.n_levels;
-    g.leaf_count = leaf_count;
+    g.leaf_count = kLeafCount;
     g.level_slack2 = 1.002001f;
     return g;
 }
@@ -236,11 +242,6 @@ __device__ __forceinline__ bool shoots(const PairConst &pc, int c) {
 //   interleaves chunks, and the locality of a warp's 32 queries is worth more than its density.)
 constexpr int kKeepFromIter = 3;
 
-struct SearchArgs {
-    int start_level0, leaf_count, defer_from_iter;
-    float reseed_cells;
-};
-
 // what is fixed for all queries of one (pair, class): grid, radius
 struct SearchFrame {
     GridView g;
@@ -248,13 +249,13 @@ struct SearchFrame {
     float r2_prune;
     bool defer;
 };
-__device__ __forceinline__ SearchFrame search_frame(const DeviceArrays &A, const PairConst &pc, const PairState &ps, int c, const SearchArgs &sa) {
+__device__ __forceinline__ SearchFrame search_frame(const DeviceArrays &A, const PairConst &pc, const PairState &ps, int c) {
     SearchFrame f;
-    f.g = grid_of(A, pc, ps, c, sa.leaf_count);
+    f.g = grid_of(A, pc, ps, c);
     const float max_distance_f = 2.5f * ps.thre;
     f.max_dist_sqr = (double)max_distance_f * (double)max_distance_f;
     f.r2_prune = (float)f.max_dist_sqr * 1.0001f;
-    f.defer = ps.iter >= sa.defer_from_iter; // queueing a block's small cells pays once the seeds are good
+    f.defer = ps.iter >= kDeferFromIter; // queueing a block's small cells pays once the seeds are good
     return f;
 }
 
@@ -275,7 +276,7 @@ __device__ __forceinline__ void search_finish(DeviceArrays &A, const PairConst &
 // match that the last increment left far away (the big first corrections) is challenged by a fresh greedy descent.
 template <class Bounds>
 __device__ __forceinline__ void search_one(DeviceArrays &A, const PairConst &pc, int c, int buf, uint32_t gi, const float4 p,
-                                           float orig_bits, const SearchFrame &f, const SearchArgs &sa, bool write_cert) {
+                                           float orig_bits, const SearchFrame &f, bool write_cert) {
     NoStats st;
     int best_j = -1;
     float best_d2 = INFINITY;
@@ -286,22 +287,22 @@ __device__ __forceinline__ void search_one(DeviceArrays &A, const PairConst &pc,
         best_j = pj;
     }
     {
-        const float rs = sa.reseed_cells * f.g.h0;
+        const float rs = kReseedCells * f.g.h0;
         if (best_j < 0 || best_d2 > rs * rs) {
             float d2 = INFINITY;
             int j = -1;
-            walk_greedy_seed(f.g, p.x, p.y, p.z, sa.start_level0, d2, j, st);
+            walk_greedy_seed(f.g, p.x, p.y, p.z, kStartLevel0, d2, j, st);
             if (j >= 0 && d2 < best_d2) best_d2 = d2, best_j = j;
         }
     }
-    const float cert2 = nn_search_walk_b<Bounds>(f.g, p.x, p.y, p.z, f.r2_prune, sa.start_level0, f.defer, best_d2, best_j, st);
+    const float cert2 = nn_search_walk_b<Bounds>(f.g, p.x, p.y, p.z, f.r2_prune, kStartLevel0, f.defer, best_d2, best_j, st);
     if (write_cert) A.src_cert[buf][gi] = make_float4(p.x, p.y, p.z, sqrtf(cert2));
     search_finish(A, pc, c, gi, best_j, best_d2, f.max_dist_sqr, orig_bits);
 }
 
 // direct mode: one warp, 32 consecutive sources of a chunk
 template <class Bounds>
-__device__ __forceinline__ void search_quarter(DeviceArrays &A, int buf, uint32_t chunk, uint32_t sub, const SearchArgs &sa, bool write_cert) {
+__device__ __forceinline__ void search_quarter(DeviceArrays &A, int buf, uint32_t chunk, uint32_t sub, bool write_cert) {
     const ChunkDesc cd = A.it_chunks[chunk];
     const PairConst &pc = A.pc[cd.pair];
     const PairState &ps = A.ps[cd.pair];
@@ -322,13 +323,12 @@ __device__ __forceinline__ void search_quarter(DeviceArrays &A, int buf, uint32_
         A.nn_d2[gi] = INFINITY;
         return;
     }
-    const SearchFrame f = search_frame(A, pc, ps, c, sa);
-    search_one<Bounds>(A, pc, c, buf, gi, p, n.w, f, sa, write_cert);
+    const SearchFrame f = search_frame(A, pc, ps, c);
+    search_one<Bounds>(A, pc, c, buf, gi, p, n.w, f, write_cert);
 }
 
 // keep mode: one block, one chunk. need_list / n_need live in shared memory.
-__device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint32_t chunk, const SearchArgs &sa, uint8_t *need_list,
-                                                  uint32_t *n_need) {
+__device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint32_t chunk, uint8_t *need_list, uint32_t *n_need) {
     const ChunkDesc cd = A.it_chunks[chunk];
     const PairConst &pc = A.pc[cd.pair];
     const PairState &ps = A.ps[cd.pair];
@@ -339,7 +339,7 @@ __device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint
     if (shoots(pc, c)) return;
     const int lane = threadIdx.x & 31;
     const bool active = pc.used[c] && nsg >= 3 && nt >= 3;
-    const SearchFrame f = search_frame(A, pc, ps, c, sa);
+    const SearchFrame f = search_frame(A, pc, ps, c);
     if (threadIdx.x == 0) *n_need = 0u;
     __syncthreads();
     // ---- pass A
@@ -382,7 +382,7 @@ __device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint
     if (threadIdx.x < *n_need) {
         const uint32_t gi = pc.src_base[c] + cd.first + need_list[threadIdx.x];
         const float4 p = A.src_pos[buf][gi]; // (advanced by pass A)
-        search_one<WalkBounds>(A, pc, c, buf, gi, p, A.src_nrm[buf][gi].w, f, sa, true);
+        search_one<WalkBounds>(A, pc, c, buf, gi, p, A.src_nrm[buf][gi].w, f, true);
     }
 }
 
@@ -392,8 +392,7 @@ constexpr int kSearchBlocksPerSm = 10; // 48 registers; the fastest of 8 / 10 / 
 __device__ __forceinline__ int search_mode_of(int it) { return it >= kKeepFromIter ? 2 : (it == kKeepFromIter - 1 ? 1 : 0); }
 
 template <int kMode>
-__global__ void __launch_bounds__(kIterBlock, kSearchBlocksPerSm) k_search(DeviceArrays A, int buf, int it, int start_level0, int leaf_count,
-                                                                          int defer_from_iter, float reseed_cells) {
+__global__ void __launch_bounds__(kIterBlock, kSearchBlocksPerSm) k_search(DeviceArrays A, int buf, int it) {
     buf = loop_buf(A, buf);
     if (it < 0) it = A.ctl->it; // (graph: the device-side loop counter; every running pair is in this iteration)
     if (blockIdx.x == 0 && threadIdx.x == 0) { // first kernel(s) of the iteration: counters and list the later ones use
@@ -402,11 +401,10 @@ __global__ void __launch_bounds__(kIterBlock, kSearchBlocksPerSm) k_search(Devic
         ctl.n_live[buf ^ 1] = 0u;
     }
     if (search_mode_of(it) != kMode) return;
-    const SearchArgs sa = {start_level0, leaf_count, defer_from_iter, reseed_cells};
     if (kMode == 2) {
         __shared__ uint8_t s_need[kIterBlock];
         __shared__ uint32_t s_n_need;
-        for_each_live_chunk(A, buf, 0, [&](uint32_t chunk) { search_keep_chunk(A, buf, chunk, sa, s_need, &s_n_need); });
+        for_each_live_chunk(A, buf, 0, [&](uint32_t chunk) { search_keep_chunk(A, buf, chunk, s_need, &s_n_need); });
     } else {
         const uint32_t n_units = (kIterBlock / 32) * A.ctl->n_live[buf];
         const uint32_t *list = A.live_chunks + (size_t)buf * A.live_stride;
@@ -415,8 +413,8 @@ __global__ void __launch_bounds__(kIterBlock, kSearchBlocksPerSm) k_search(Devic
             if ((threadIdx.x & 31) == 0) u = atomicAdd(&A.ctl->work[0], 1u);
             u = __shfl_sync(0xffffffffu, u, 0);
             if (u >= n_units) break;
-            if (kMode == 1) search_quarter<WalkBounds>(A, buf, list[u / (kIterBlock / 32)], u % (kIterBlock / 32), sa, true);
-            else search_quarter<NoBounds>(A, buf, list[u / (kIterBlock / 32)], u % (kIterBlock / 32), sa, false);
+            if (kMode == 1) search_quarter<WalkBounds>(A, buf, list[u / (kIterBlock / 32)], u % (kIterBlock / 32), true);
+            else search_quarter<NoBounds>(A, buf, list[u / (kIterBlock / 32)], u % (kIterBlock / 32), false);
             __syncwarp();
         }
     }
@@ -426,7 +424,7 @@ __global__ void __launch_bounds__(kIterBlock, kSearchBlocksPerSm) k_search(Devic
 // the one with the smallest squared distance to the line through the source point along its normal; dropped
 // if that value exceeds max_distance (NOT squared); correspondence distance = its squared NN distance.
 // Launched only when a pair of the batch asked for normal shooting.
-__device__ __forceinline__ void search_shoot_chunk(DeviceArrays &A, int buf, uint32_t chunk, int start_level0, int leaf_count) {
+__device__ __forceinline__ void search_shoot_chunk(DeviceArrays &A, int buf, uint32_t chunk) {
     const ChunkDesc cd = A.it_chunks[chunk];
     const PairConst &pc = A.pc[cd.pair];
     const PairState &ps = A.ps[cd.pair];
@@ -445,12 +443,12 @@ __device__ __forceinline__ void search_shoot_chunk(DeviceArrays &A, int buf, uin
         A.nn_d2[gi] = INFINITY;
         return;
     }
-    const GridView g = grid_of(A, pc, ps, c, leaf_count);
+    const GridView g = grid_of(A, pc, ps, c);
     const float max_distance_f = 2.5f * ps.thre;
     int sj = -1;
     float sd2 = INFINITY;
     KnnList kl;
-    knn_search(g, p.x, p.y, p.z, start_level0, kl);
+    knn_search(g, p.x, p.y, p.z, kStartLevel0, kl);
     double min_dist = 1.7976931348623157e308;
     for (int t = 0; t < kl.n; ++t) {
         const float4 q = __ldg(&g.pos[kl.j[t]]);
@@ -469,9 +467,9 @@ __device__ __forceinline__ void search_shoot_chunk(DeviceArrays &A, int buf, uin
     A.nn_idx[gi] = sj;
     A.nn_d2[gi] = sd2;
 }
-__global__ void __launch_bounds__(kIterBlock) k_search_shoot(DeviceArrays A, int buf, int start_level0, int leaf_count) {
+__global__ void __launch_bounds__(kIterBlock) k_search_shoot(DeviceArrays A, int buf) {
     buf = loop_buf(A, buf);
-    for_each_live_chunk(A, buf, 3, [&](uint32_t chunk) { search_shoot_chunk(A, buf, chunk, start_level0, leaf_count); });
+    for_each_live_chunk(A, buf, 3, [&](uint32_t chunk) { search_shoot_chunk(A, buf, chunk); });
 }
 
 // ---- k_resolve ---------------------------------------------------------------------------------
@@ -1086,12 +1084,10 @@ __global__ void __launch_bounds__(kSolveThreads) k_solve(DeviceArrays A, int buf
 //      phases are the same device functions over the same work lists, separated by grid-wide barriers instead of kernel
 //      boundaries. Every block executes the same number of barriers: the loop bounds (LoopCtl::max_iter, the running
 //      counter read after a barrier) are grid-uniform.
-__global__ void __launch_bounds__(kIterBlock, 4) k_icp_loop(DeviceArrays A, int start_level0, int leaf_count, int defer_from_iter,
-                                                           float reseed_cells) {
+__global__ void __launch_bounds__(kIterBlock, 4) k_icp_loop(DeviceArrays A) {
     namespace cg = cooperative_groups;
     cg::grid_group grid = cg::this_grid();
     LoopCtl &ctl = *A.ctl;
-    const SearchArgs sa = {start_level0, leaf_count, defer_from_iter, reseed_cells};
     __shared__ uint8_t s_need[kIterBlock];
     __shared__ uint32_t s_n_need;
     const int n_pairs = ctl.n_pairs, max_iter = ctl.max_iter;
@@ -1103,9 +1099,9 @@ __global__ void __launch_bounds__(kIterBlock, 4) k_icp_loop(DeviceArrays A, int 
         // phase 1: transform + search (+ keep) + claim
         for (uint32_t w = blockIdx.x; w < n_live; w += gridDim.x) {
             const uint32_t chunk = list[w];
-            if (it >= kKeepFromIter) search_keep_chunk(A, buf, chunk, sa, s_need, &s_n_need);
-            else if (it == kKeepFromIter - 1) search_quarter<WalkBounds>(A, buf, chunk, threadIdx.x >> 5, sa, true);
-            else search_quarter<NoBounds>(A, buf, chunk, threadIdx.x >> 5, sa, false);
+            if (it >= kKeepFromIter) search_keep_chunk(A, buf, chunk, s_need, &s_n_need);
+            else if (it == kKeepFromIter - 1) search_quarter<WalkBounds>(A, buf, chunk, threadIdx.x >> 5, true);
+            else search_quarter<NoBounds>(A, buf, chunk, threadIdx.x >> 5, false);
             __syncthreads();
         }
         grid.sync();
@@ -1373,8 +1369,8 @@ __global__ void k_finalize(DeviceArrays A, int n_pairs) {
 
 // ---- k_nn_query: mulls_nn_query — exact 1-NN of arbitrary query points in one target class of pair 0, on the grid
 //      the last registration built (what block1->tree_*->nearestKSearch(p, 1) answers in the reference)
-__global__ void __launch_bounds__(kIterBlock) k_nn_query(DeviceArrays A, int cls, const float *xyz, uint32_t n, int start_level0,
-                                                        int leaf_count, int *out_idx, float *out_d2) {
+__global__ void __launch_bounds__(kIterBlock) k_nn_query(DeviceArrays A, int cls, const float *xyz, uint32_t n, int *out_idx,
+                                                        float *out_d2) {
     const uint32_t i = blockIdx.x * kIterBlock + threadIdx.x;
     if (i >= n) return;
     const PairConst &pc = A.pc[0];
@@ -1382,13 +1378,13 @@ __global__ void __launch_bounds__(kIterBlock) k_nn_query(DeviceArrays A, int cls
     int best_j = -1;
     float best_d2 = INFINITY;
     if (ps.n_tgt[cls] > 0 && !A.hash_used[1]) {
-        const GridView g = grid_of(A, pc, ps, cls, leaf_count);
+        const GridView g = grid_of(A, pc, ps, cls);
         const float px = xyz[3 * i], py = xyz[3 * i + 1], pz = xyz[3 * i + 2];
         const float rmax = 2.5f * pc.thre_unit;
         const float r2 = rmax * rmax * 1.0001f;
         NoStats st;
-        walk_greedy_seed(g, px, py, pz, start_level0, best_d2, best_j, st);
-        nn_search_walk(g, px, py, pz, r2, start_level0, false, best_d2, best_j, st);
+        walk_greedy_seed(g, px, py, pz, kStartLevel0, best_d2, best_j, st);
+        nn_search_walk(g, px, py, pz, r2, kStartLevel0, false, best_d2, best_j, st);
         if (best_j >= 0 && !((double)best_d2 <= (double)rmax * (double)rmax)) best_j = -1;
         if (best_j >= 0) best_j = __float_as_int(__ldg(&g.nrm[best_j]).w);
     }

@@ -77,6 +77,12 @@ int nccl_allreduce_hook(void *user, void *buf, size_t count, int dtype, int op, 
 
 struct mulls_map;
 
+// a device buffer of the context that only grows (grow_scratch)
+struct Scratch {
+    void *p = nullptr;
+    size_t bytes = 0;
+};
+
 struct mulls_ctx {
     int device = 0;
     size_t max_pairs = 0, max_src = 0, max_tgt = 0;
@@ -100,33 +106,23 @@ struct mulls_ctx {
     bool any_keep_less = false;
     bool grid_valid = false; // pair 0's sorted target slices and grid are those of the last registration (mulls_nn_query)
     // tunables
-    int start_level0 = 5;
-    int leaf_count = 32;
     // iteration loop as a CUDA graph: WHILE(pairs running) { search, resolve, accumulate, solve } + posterior, finalize,
-    // collect — one launch, the loop condition is set on the device (no host polling). Built on first use, rebuilt when a
-    // tunable baked into its kernel nodes changes. 0: the host launch loop (per-kernel events for the bench's roofline).
+    // collect — one launch, the loop condition is set on the device (no host polling). Built on first use, rebuilt when
+    // the batch shape baked into its kernel nodes changes. 0: the host launch loop (per-kernel events for the bench's
+    // roofline).
     int use_graph = 1;
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t graph_exec = nullptr;
-    int graph_key[6] = {-1, -1, -1, -1, -1, -1}; // the tunables baked into the kernel nodes
+    int graph_key[2] = {-1, -1}; // the batch shape baked into the kernel nodes
     LoopCtl *h_ctl = nullptr;            // pinned staging of the control block
     int num_sms = 132;
-    int sort_sources = 1;    // 0: sources stay in the caller's order (study switch)
-    int search_blocks = 10;  // resident k_search blocks per SM (= kSearchBlocksPerSm, the instantiated register budget)
-    int defer_from_iter = 3; // k_search queues the small cells of a block (one scan loop per block) from this iteration on
-    int hash_slack = 4;      // table capacity >= hash_slack x cells (power of two): load factor <= 1/hash_slack
-    int reseed_cells_x4 = 16; // a previous match farther than this many quarter level-0 cells is challenged by a greedy descent
     bool any_normal_shooting = false;
     bool any_undistort = false;
-    int zero_copy = 0;     // opt-in: one-shot calls read pinned host clouds in place (slower than the DMA copy)
     // repack host clouds to the 28 B/point wire format on the host cores before the DMA (host_pack.h):
     // 0 never, 1 always, 2 when a call ships at least kPackMinPoints points (small calls are latency-bound: raw rows)
     int host_pack = 2;
-    int poll_pause = 64;   // _mm_pause() count between two cudaEventQuery calls of the launch loop's flow control
-    int stage_wc = 0;      // allocate the pinned staging write-combined (the host only streams into it)
     float4 *h_stage = nullptr; // pinned staging of the packed clouds (allocated on first use)
     size_t h_stage_slots = 0;
-    float h0_min = 0.125f;
     // timing
     cudaEvent_t ev_begin = nullptr, ev_ingest = nullptr, ev_iter = nullptr, ev_end = nullptr, ev_h2d0 = nullptr;
     bool h2d_timed = false;                 // ev_h2d0 was recorded by the upload of the current one-shot call
@@ -141,26 +137,20 @@ struct mulls_ctx {
     // one-shot batch calls with host buffers (mulls_icp_run_batch) are double-buffered: the second half of the batch is
     // packed and copied on the twin's stream while the first half is being registered on this one
     mulls_ctx *twin = nullptr;
-    int double_buffer = 1;
-    int loop_kernel = 1;       // small batches: the whole iteration loop as one cooperative kernel (k_icp_loop)
-    int loop_kernel_blocks = 0; // co-resident blocks of k_icp_loop on this device (0: not yet queried, -1: unavailable)
+    // small batches run the whole iteration loop as one cooperative kernel (k_icp_loop) when every chunk and pair has a
+    // co-resident block: their count on this device (0: not yet queried, -1: unavailable)
+    int loop_kernel_blocks = 0;
     struct Pending {                 // a run that has been enqueued and not yet finished (run_finish)
         uint64_t launches = 0;
         int n_search_ev = 0;
         bool graphed = false, hooked = false, active = false;
     } pend;
     std::vector<size_t> lane_begin; // pair range of every lane for the resident batch
-    // PCA scratch
-    void *pca_buf = nullptr;
-    size_t pca_buf_bytes = 0;
-    // classification scratch (mulls_classify_nground)
-    void *cls_buf = nullptr;
-    size_t cls_buf_bytes = 0;
-    // ground-filter scratch (mulls_fast_ground_filter): per-point part and per-cell part
-    void *gf_buf = nullptr, *gf_cell_buf = nullptr;
-    size_t gf_buf_bytes = 0, gf_cell_buf_bytes = 0;
-    void *vx_buf = nullptr, *ext_buf = nullptr; // voxel filter scratch; clouds handed between the stages of extract_semantic_pts
-    size_t vx_buf_bytes = 0, ext_buf_bytes = 0;
+    // device scratch, grown on demand (grow_scratch)
+    Scratch pca_buf;             // PCA
+    Scratch cls_buf;             // classification (mulls_classify_nground)
+    Scratch gf_buf, gf_cell_buf; // ground filter (mulls_fast_ground_filter): per-point part and per-cell part
+    Scratch vx_buf, ext_buf;     // voxel filter; clouds handed between the stages of extract_semantic_pts
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
     const mulls_map *tree_map = nullptr;
@@ -175,6 +165,18 @@ struct mulls_ctx {
             return MULLS_E_CUDA;                                                                      \
         }                                                                                             \
     } while (0)
+
+// makes s at least `bytes` long (16 at least). The old buffer goes through cudaFree, which waits for the device: no
+// kernel still reads it when it is released.
+static int grow_scratch(mulls_ctx *ctx, Scratch &s, size_t bytes) {
+    bytes = std::max<size_t>(bytes, 16);
+    if (bytes <= s.bytes) return MULLS_OK;
+    if (s.p) cudaFree(s.p);
+    s = Scratch{};
+    CK(cudaMalloc(&s.p, bytes));
+    s.bytes = bytes;
+    return MULLS_OK;
+}
 
 template <typename T>
 static cudaError_t dev_alloc(mulls_ctx *ctx, T **p, size_t n) {
@@ -231,12 +233,8 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (void *p : ctx->allocs) cudaFree(p);
     if (ctx->cub_temp) cudaFree(ctx->cub_temp);
-    if (ctx->pca_buf) cudaFree(ctx->pca_buf);
-    if (ctx->cls_buf) cudaFree(ctx->cls_buf);
-    if (ctx->gf_buf) cudaFree(ctx->gf_buf);
-    if (ctx->gf_cell_buf) cudaFree(ctx->gf_cell_buf);
-    if (ctx->vx_buf) cudaFree(ctx->vx_buf);
-    if (ctx->ext_buf) cudaFree(ctx->ext_buf);
+    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf})
+        if (s->p) cudaFree(s->p);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
     if (ctx->h_flags) cudaFreeHost(ctx->h_flags);
     if (ctx->h_running) cudaFreeHost(ctx->h_running);
@@ -457,29 +455,9 @@ int mulls_set_tunable(mulls_ctx *ctx, const char *name, int value) {
         if (rc != MULLS_OK) return rc;
     }
     std::string n(name);
-    if (n == "start_level") ctx->start_level0 = value;
-    else if (n == "leaf_count") ctx->leaf_count = value;
-    else if (n == "reseed_cells_x4") ctx->reseed_cells_x4 = value;
-    else if (n == "defer_from_iter") ctx->defer_from_iter = value;
-    else if (n == "search_blocks") ctx->search_blocks = value; // (kept for old scripts: the instantiations are fixed now)
-    else if (n == "sort_sources") ctx->sort_sources = value;
-    else if (n == "double_buffer") ctx->double_buffer = value;
-    else if (n == "loop_kernel") ctx->loop_kernel = value;
-    else if (n == "hash_slack") ctx->hash_slack = std::max(2, value);
-    else if (n == "use_graph") ctx->use_graph = value;
-    else if (n == "zero_copy") ctx->zero_copy = value;
+    if (n == "use_graph") ctx->use_graph = value;
     else if (n == "host_pack") ctx->host_pack = value;
-    else if (n == "poll_pause") ctx->poll_pause = value;
-    else if (n == "stage_wc") {
-        if (ctx->stage_wc != value && ctx->h_stage) { // re-allocated with the new flag on the next packed upload
-            cudaFreeHost(ctx->h_stage);
-            ctx->h_stage = nullptr;
-            ctx->h_stage_slots = 0;
-        }
-        ctx->stage_wc = value;
-    }
     else if (n == "pack_threads") PackPool::get().ensure_workers(value);
-    else if (n == "h0_min_mm") ctx->h0_min = (float)value / 1000.0f;
     else return MULLS_E_ARG;
     return MULLS_OK;
 }
@@ -625,9 +603,10 @@ static int build_pair_const(mulls_ctx *ctx, const mulls_icp_params &P, const dou
     return MULLS_OK;
 }
 
-// resident = true: the clouds are copied into HBM (mulls_batch_upload: they must survive the caller's buffers).
-// resident = false (one-shot calls): clouds in PINNED host memory are not copied at all — the ingest kernel
-// streams them over PCIe itself (zero-copy through the UVA alias), pageable ones are staged with cudaMemcpy.
+// Copies the clouds into HBM on the context's stream: repacked on the host cores first when the call ships enough
+// points (host_pack), as caller rows otherwise. resident = true (mulls_batch_upload): the copies are waited for, since
+// the clouds must survive the caller's buffers. resident = false (one-shot calls): the copies stay in flight and the
+// registration that follows waits for them. tgt_on_device: the target views already point into HBM and are read there.
 static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *tgt, const mulls_cloud_view *src,
                        const mulls_icp_params *params, const double *init_guess, const uint32_t *src_index_base,
                        const uint32_t *src_global_n, bool resident = true, bool tgt_on_device = false) {
@@ -698,8 +677,8 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
         ctx->err = "internal: chunk table capacity";
         return MULLS_E_CAPACITY;
     }
-    // the clouds: repacked on the host cores and copied pair by pair (host_pack), or copied as they are, or read in
-    // place (zero-copy, pinned host buffers of one-shot calls)
+    // the clouds: repacked on the host cores and copied pair by pair (host_pack), or copied as they are; a device-resident
+    // target (the local map) is read in place
     size_t host_points = 0;
     for (size_t p = 0; p < n_pairs; ++p)
         for (int s = 0; s < kNumSegs; ++s)
@@ -710,8 +689,7 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
     if (pack) {
         if (!ctx->h_stage) {
             const size_t slots = 2 * ctx->cap_in + 4 * kNumSegs * ctx->max_pairs;
-            CK(cudaHostAlloc((void **)&ctx->h_stage, slots * sizeof(float4),
-                             ctx->stage_wc ? cudaHostAllocWriteCombined : cudaHostAllocDefault));
+            CK(cudaHostAlloc((void **)&ctx->h_stage, slots * sizeof(float4), cudaHostAllocDefault));
             ctx->h_stage_slots = slots;
         }
         CK(cudaStreamSynchronize(ctx->stream)); // the staging may still be read by a copy of a call that failed half-way
@@ -786,15 +764,6 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
                 pc.in_ptr[s] = (const float4 *)v.aos48;
                 continue;
             }
-            if (!resident && ctx->zero_copy) {
-                cudaPointerAttributes attr;
-                if (cudaPointerGetAttributes(&attr, v.aos48) == cudaSuccess && attr.type == cudaMemoryTypeHost &&
-                    attr.devicePointer != nullptr && ((uintptr_t)attr.devicePointer % 16) == 0) {
-                    pc.in_ptr[s] = (const float4 *)attr.devicePointer;
-                    continue;
-                }
-                cudaGetLastError(); // pageable memory: not an error, fall through to the copy
-            }
             CK(cudaMemcpyAsync((void *)(ctx->A.in_aos + 3 * (size_t)pc.in_off[s]), v.aos48, v.n * 48, cudaMemcpyHostToDevice,
                                ctx->stream));
         }
@@ -853,10 +822,10 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
         k_shard_pack_setup<<<1, 1, 0, st>>>(A, 1);
         launches += 2;
     }
-    k_pair_setup<<<(unsigned)ceil_div(np, 128), 128, 0, st>>>(A, np, ctx->h0_min);
+    k_pair_setup<<<(unsigned)ceil_div(np, 128), 128, 0, st>>>(A, np);
     ++launches;
     if (n_inc) {
-        k_make_keys<<<n_inc, kIngestBlock, 0, st>>>(A, ctx->sort_sources);
+        k_make_keys<<<n_inc, kIngestBlock, 0, st>>>(A);
         ++launches;
         if (ctx->any_keep_less) { // random down-sampling of :2866-2892: radix select of the k-th sampling key
             const unsigned pb = (unsigned)ceil_div(np, 64);
@@ -890,13 +859,13 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
         k_gather<<<(unsigned)ceil_div(n_in, 256), 256, 0, st>>>(A, A.keys_b, A.vals_b, n_in);
         const unsigned hb = (unsigned)ceil_div((size_t)n_in + 1, 256);
         k_hash_build<<<hb, 256, 0, st>>>(A, A.keys_b, n_in, 0);
-        k_hash_layout<<<1, 32, 0, st>>>(A, np, ctx->hash_slack);
+        k_hash_layout<<<1, 32, 0, st>>>(A, np);
         k_hash_clear<<<1184, 256, 0, st>>>(A);
         k_hash_build<<<hb, 256, 0, st>>>(A, A.keys_b, n_in, 1);
         k_hash_build<<<hb, 256, 0, st>>>(A, A.keys_b, n_in, 2);
         launches += 6;
     } else {
-        k_hash_layout<<<1, 32, 0, st>>>(A, np, ctx->hash_slack);
+        k_hash_layout<<<1, 32, 0, st>>>(A, np);
         ++launches;
     }
     return MULLS_OK;
@@ -916,22 +885,21 @@ static unsigned resident_grid(const mulls_ctx *ctx, int blocks_per_sm) {
 // it < 0 (recording the iteration graph): all three modes, each checks the device-side iteration counter; the host
 // launch loop knows the iteration and launches the one that runs
 static void launch_search(mulls_ctx *ctx, cudaStream_t st, const DeviceArrays &A, int buf, int it) {
-    const float reseed = 0.25f * (float)ctx->reseed_cells_x4;
     const unsigned grid = resident_grid(ctx, kSearchBlocksPerSm);
     const int mode = it < 0 ? -1 : (it >= kKeepFromIter ? 2 : (it == kKeepFromIter - 1 ? 1 : 0));
-    if (mode < 0 || mode == 0) k_search<0><<<grid, kIterBlock, 0, st>>>(A, buf, it, ctx->start_level0, ctx->leaf_count, ctx->defer_from_iter, reseed);
-    if (mode < 0 || mode == 1) k_search<1><<<grid, kIterBlock, 0, st>>>(A, buf, it, ctx->start_level0, ctx->leaf_count, ctx->defer_from_iter, reseed);
-    if (mode < 0 || mode == 2) k_search<2><<<grid, kIterBlock, 0, st>>>(A, buf, it, ctx->start_level0, ctx->leaf_count, ctx->defer_from_iter, reseed);
+    if (mode < 0 || mode == 0) k_search<0><<<grid, kIterBlock, 0, st>>>(A, buf, it);
+    if (mode < 0 || mode == 1) k_search<1><<<grid, kIterBlock, 0, st>>>(A, buf, it);
+    if (mode < 0 || mode == 2) k_search<2><<<grid, kIterBlock, 0, st>>>(A, buf, it);
 }
 constexpr int kShootBlocksPerSm = 8, kResolveBlocksPerSm = 16, kAccumulateBlocksPerSm = 8;
+constexpr int kPollPause = 64; // _mm_pause() count between two cudaEventQuery calls of the launch loop's flow control
 
 // The iteration loop as a CUDA graph (CUDA 12.4+ conditional nodes): WHILE(handle) { k_search [, k_search_shoot],
 // k_resolve, k_accumulate, k_solve } followed by k_posterior, k_finalize, k_collect. Kernel nodes are recorded once per
 // context with grids sized for its capacity; what a run needs to know (chunk / pair counts, trace switch, loop counter)
 // is read from LoopCtl in device memory. k_solve's last block sets the loop condition: no host polling, one launch.
 static int build_iteration_graph(mulls_ctx *ctx) {
-    const int key[6] = {ctx->start_level0, ctx->leaf_count + (ctx->reseed_cells_x4 << 12), (int)chunk_bucket(ctx),
-                        ctx->any_normal_shooting ? 1 : 0, ctx->defer_from_iter, ctx->search_blocks};
+    const int key[2] = {(int)chunk_bucket(ctx), ctx->any_normal_shooting ? 1 : 0};
     if (ctx->graph_exec && std::memcmp(key, ctx->graph_key, sizeof(key)) == 0) return MULLS_OK;
     if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec), ctx->graph_exec = nullptr;
     if (ctx->graph) cudaGraphDestroy(ctx->graph), ctx->graph = nullptr;
@@ -951,7 +919,7 @@ static int build_iteration_graph(mulls_ctx *ctx) {
     CK(cudaStreamBeginCaptureToGraph(st, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
     launch_search(ctx, st, A, -1, -1);
     if (ctx->any_normal_shooting)
-        k_search_shoot<<<resident_grid(ctx, kShootBlocksPerSm), kIterBlock, 0, st>>>(A, -1, ctx->start_level0, ctx->leaf_count);
+        k_search_shoot<<<resident_grid(ctx, kShootBlocksPerSm), kIterBlock, 0, st>>>(A, -1);
     k_resolve<<<resident_grid(ctx, kResolveBlocksPerSm), kIterBlock, 0, st>>>(A, -1);
     k_accumulate<<<resident_grid(ctx, kAccumulateBlocksPerSm), kIterBlock, 0, st>>>(A, -1);
     k_solve<<<cap_pairs, kSolveThreads, 0, st>>>(A, -1, (unsigned long long)handle);
@@ -1012,7 +980,7 @@ static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace
     }
     // small batches: one cooperative kernel runs the whole loop (every chunk and every pair must find a co-resident block)
     bool looped = false;
-    if (!hook && ctx->use_graph && ctx->loop_kernel && !ctx->any_normal_shooting && n_itc > 0) {
+    if (!hook && ctx->use_graph && !ctx->any_normal_shooting && n_itc > 0) {
         if (ctx->loop_kernel_blocks == 0) {
             int per_sm = 0, coop = 0;
             cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx->device);
@@ -1021,9 +989,7 @@ static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace
             else
                 ctx->loop_kernel_blocks = -1, cudaGetLastError();
         }
-        // `loop_kernel` = how many chunks a co-resident block may have to walk per phase (1: every chunk has its block)
-        looped = ctx->loop_kernel_blocks > 0 && n_itc <= (unsigned)(ctx->loop_kernel * ctx->loop_kernel_blocks) &&
-                 np <= ctx->loop_kernel * ctx->loop_kernel_blocks;
+        looped = ctx->loop_kernel_blocks > 0 && n_itc <= (unsigned)ctx->loop_kernel_blocks && np <= ctx->loop_kernel_blocks;
     }
     const bool graphed = !hook && ctx->use_graph && !looped;
     if (graphed) {
@@ -1034,9 +1000,7 @@ static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace
     int n_search_ev = 0;
     if (looped) {
         DeviceArrays Aarg = A;
-        int a1 = ctx->start_level0, a2 = ctx->leaf_count, a3 = ctx->defer_from_iter;
-        float a4 = 0.25f * (float)ctx->reseed_cells_x4;
-        void *args[] = {&Aarg, &a1, &a2, &a3, &a4};
+        void *args[] = {&Aarg};
         const unsigned grid = std::max(1u, std::min((unsigned)ctx->loop_kernel_blocks, std::max(n_itc, (unsigned)np)));
         CK(cudaLaunchCooperativeKernel((const void *)k_icp_loop, dim3(grid), dim3(kIterBlock), args, 0, st));
         k_posterior<<<n_itc, kIterBlock, 0, st>>>(A);
@@ -1052,7 +1016,7 @@ static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace
             if (it >= 2) {
                 // (poll with pauses: several lanes spinning inside the driver slow each other's launches down)
                 while (cudaEventQuery(ctx->ev_done[it - 2]) == cudaErrorNotReady)
-                    for (int k = 0; k < ctx->poll_pause; ++k) _mm_pause();
+                    for (int k = 0; k < kPollPause; ++k) _mm_pause();
                 // Sharded runs must take this decision identically on every rank (the ranks issue matching collectives):
                 // they read the count the device recorded at the END of iteration it-2 — written once, before
                 // ev_done[it-2] — never the live flag, whose value at this instant depends on each rank's timing.
@@ -1066,7 +1030,7 @@ static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace
             CK(cudaEventRecord(ctx->ev_search[2 * it], st));
             launch_search(ctx, st, A, buf, it);
             if (ctx->any_normal_shooting) {
-                k_search_shoot<<<resident_grid(ctx, kShootBlocksPerSm), kIterBlock, 0, st>>>(A, buf, ctx->start_level0, ctx->leaf_count);
+                k_search_shoot<<<resident_grid(ctx, kShootBlocksPerSm), kIterBlock, 0, st>>>(A, buf);
                 ++launches;
             }
             CK(cudaEventRecord(ctx->ev_search[2 * it + 1], st));
@@ -1212,14 +1176,11 @@ int mulls_batch_run_resident(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_tr
 static int one_shot_batch(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *tgt, const mulls_cloud_view *src,
                           const mulls_icp_params *params, const double *init_guess, mulls_icp_result *out, mulls_icp_trace *trace) {
     const double t0 = wall_ms();
-    const bool split = ctx->double_buffer && ctx->use_graph && n_pairs >= 2 && n_pairs <= ctx->max_pairs;
+    const bool split = ctx->use_graph && n_pairs >= 2 && n_pairs <= ctx->max_pairs;
     if (split && !ctx->twin) {
         mulls_ctx *t = mulls_create(ctx->device, (ctx->max_pairs + 1) / 2, ctx->max_src, ctx->max_tgt);
         if (t) { // (no memory for it: the call simply runs on one context)
-            t->start_level0 = ctx->start_level0, t->leaf_count = ctx->leaf_count, t->reseed_cells_x4 = ctx->reseed_cells_x4;
-            t->defer_from_iter = ctx->defer_from_iter, t->sort_sources = ctx->sort_sources, t->hash_slack = ctx->hash_slack;
-            t->use_graph = ctx->use_graph, t->zero_copy = ctx->zero_copy, t->host_pack = ctx->host_pack, t->poll_pause = ctx->poll_pause;
-            t->stage_wc = ctx->stage_wc, t->h0_min = ctx->h0_min, t->double_buffer = 0;
+            t->use_graph = ctx->use_graph, t->host_pack = ctx->host_pack;
             ctx->twin = t;
         }
     }
@@ -1360,8 +1321,7 @@ int mulls_nn_query(mulls_ctx *ctx, int cls, const float *xyz, size_t n, int32_t 
     CK(cudaMallocAsync((void **)&d_i, n * sizeof(int), st));
     CK(cudaMallocAsync((void **)&d_d, n * sizeof(float), st));
     CK(cudaMemcpyAsync(d_q, xyz, 3 * n * sizeof(float), cudaMemcpyHostToDevice, st));
-    k_nn_query<<<(unsigned)ceil_div(n, kIterBlock), kIterBlock, 0, st>>>(ctx->A, cls, d_q, (uint32_t)n, ctx->start_level0,
-                                                                           ctx->leaf_count, d_i, d_d);
+    k_nn_query<<<(unsigned)ceil_div(n, kIterBlock), kIterBlock, 0, st>>>(ctx->A, cls, d_q, (uint32_t)n, d_i, d_d);
     CK(cudaMemcpyAsync(idx, d_i, n * sizeof(int), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(d2, d_d, n * sizeof(float), cudaMemcpyDeviceToHost, st));
     cudaFreeAsync(d_q, st);
@@ -1412,13 +1372,8 @@ static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_d
     if (rc != MULLS_OK) return rc;
     const size_t n = cloud.n;
     const size_t bytes = n * (9 * sizeof(float) + sizeof(int));
-    if (bytes > ctx->pca_buf_bytes) {
-        if (ctx->pca_buf) cudaFree(ctx->pca_buf);
-        ctx->pca_buf = nullptr;
-        ctx->pca_buf_bytes = 0;
-        CK(cudaMalloc(&ctx->pca_buf, std::max<size_t>(bytes, 16)));
-        ctx->pca_buf_bytes = bytes;
-    }
+    rc = grow_scratch(ctx, ctx->pca_buf, bytes);
+    if (rc != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
     DeviceArrays A = ctx->A;
     A.trace = nullptr;
@@ -1428,12 +1383,12 @@ static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_d
     args.r2 = (float)((double)radius * (double)radius);
     args.k = k;
     args.stride = stride;
-    args.eigenvalues = (float *)ctx->pca_buf;
+    args.eigenvalues = (float *)ctx->pca_buf.p;
     args.principal = args.eigenvalues + 3 * n;
     args.normal = args.principal + 3 * n;
     args.pt_num = (int *)(args.normal + 3 * n);
     args.nbr = nbr;
-    CK(cudaMemsetAsync(ctx->pca_buf, 0, std::max<size_t>(bytes, 16), st));
+    CK(cudaMemsetAsync(ctx->pca_buf.p, 0, std::max<size_t>(bytes, 16), st));
     if (n) {
         k_pca<<<(unsigned)ceil_div(n, kPcaWarps), kPcaWarps * 32, 0, st>>>(A, args);
         ++launches;
@@ -1457,15 +1412,8 @@ int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int
     // radiusSearch order — bit-reproducible against the CPU path; larger or unlimited k: fp64 warp reduction
     uint32_t *nbr = nullptr;
     if (k >= 1 && k <= kPcaListCap && n > 0) {
-        const size_t bytes = n * (size_t)k * sizeof(uint32_t);
-        if (bytes > ctx->cls_buf_bytes) {
-            if (ctx->cls_buf) cudaFree(ctx->cls_buf);
-            ctx->cls_buf = nullptr;
-            ctx->cls_buf_bytes = 0;
-            CK(cudaMalloc(&ctx->cls_buf, bytes));
-            ctx->cls_buf_bytes = bytes;
-        }
-        nbr = (uint32_t *)ctx->cls_buf;
+        if (const int rc = grow_scratch(ctx, ctx->cls_buf, n * (size_t)k * sizeof(uint32_t)); rc != MULLS_OK) return rc;
+        nbr = (uint32_t *)ctx->cls_buf.p;
     }
     int rc = pca_on_device(ctx, cloud, false, radius, k, stride, args, launches, nbr);
     if (rc != MULLS_OK) return rc;
@@ -1797,15 +1745,9 @@ int mulls_map_update(mulls_map *m, const mulls_cloud_view scan_down[MULLS_NUM_CL
             mulls_cloud_view v{(const float *)m->buf[m->cur][c], m->n[c]};
             PcaArgs args;
             uint64_t launches = 0;
-            const size_t nbr_bytes = (size_t)m->n[c] * pca_max_k * sizeof(uint32_t);
-            if (nbr_bytes > ctx->cls_buf_bytes) {
-                if (ctx->cls_buf) cudaFree(ctx->cls_buf);
-                ctx->cls_buf = nullptr;
-                ctx->cls_buf_bytes = 0;
-                CK(cudaMalloc(&ctx->cls_buf, nbr_bytes));
-                ctx->cls_buf_bytes = nbr_bytes;
-            }
-            const int rc = pca_on_device(ctx, v, true, pca_radius, pca_max_k, 1, args, launches, (uint32_t *)ctx->cls_buf);
+            if (const int rc = grow_scratch(ctx, ctx->cls_buf, (size_t)m->n[c] * pca_max_k * sizeof(uint32_t)); rc != MULLS_OK)
+                return rc;
+            const int rc = pca_on_device(ctx, v, true, pca_radius, pca_max_k, 1, args, launches, (uint32_t *)ctx->cls_buf.p);
             if (rc != MULLS_OK) return rc;
             k_map_revector<<<1, kMapBlock, 0, st>>>(m->buf[m->cur][c], m->n[c], args, pca_min_k, lo[k], hi[k], min_linearity,
                                                    m->mid[c], &m->d_state->n_out[c]);
@@ -1931,14 +1873,8 @@ int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mull
     const size_t o_sect = take(2 * n0 * row_b), o_vrows = take(n0 * row_b), o_vertex = take(n0 * row_b);
     const size_t o_sel = take(4 * n0 * sizeof(float4)), o_nbr = take(n0 * (size_t)P.neighbor_k * sizeof(uint32_t));
     const size_t o_l0 = take(n0), o_l = take(n0), o_df = take(n0), o_s4 = take(n0), o_vf = take(n0), o_st = take(sizeof(ClsState));
-    if (off > ctx->cls_buf_bytes) {
-        if (ctx->cls_buf) cudaFree(ctx->cls_buf);
-        ctx->cls_buf = nullptr;
-        ctx->cls_buf_bytes = 0;
-        CK(cudaMalloc(&ctx->cls_buf, off));
-        ctx->cls_buf_bytes = off;
-    }
-    char *base = (char *)ctx->cls_buf;
+    if (const int rc = grow_scratch(ctx, ctx->cls_buf, off); rc != MULLS_OK) return rc;
+    char *base = (char *)ctx->cls_buf.p;
     ClsArgs C;
     std::memset(&C, 0, sizeof(C));
     C.P = P;
@@ -2149,14 +2085,8 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
     const size_t o_hf = take(4 * n), o_hp = take(4 * n), o_dec = take(n), o_cand = take(16 * n), o_shuf = take(4 * n), o_inl = take(n);
     const size_t o_st = take(sizeof(GfState)), o_draws = take(kSacDraws * sizeof(uint32_t));
     const size_t o_tmp = take(std::max(sort_bytes, scan_bytes));
-    if (off > ctx->gf_buf_bytes) {
-        if (ctx->gf_buf) cudaFree(ctx->gf_buf);
-        ctx->gf_buf = nullptr;
-        ctx->gf_buf_bytes = 0;
-        CK(cudaMalloc(&ctx->gf_buf, off));
-        ctx->gf_buf_bytes = off;
-    }
-    char *base = (char *)ctx->gf_buf;
+    if (const int rc = grow_scratch(ctx, ctx->gf_buf, off); rc != MULLS_OK) return rc;
+    char *base = (char *)ctx->gf_buf.p;
     GfArgs A;
     std::memset(&A, 0, sizeof(A));
     A.P = P;
@@ -2212,14 +2142,8 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
         size_t cscan = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, cscan, (uint32_t *)nullptr, (uint32_t *)nullptr, num_grid, st);
         const size_t c_tmp = ctake(cscan);
-        if (coff > ctx->gf_cell_buf_bytes) {
-            if (ctx->gf_cell_buf) cudaFree(ctx->gf_cell_buf);
-            ctx->gf_cell_buf = nullptr;
-            ctx->gf_cell_buf_bytes = 0;
-            CK(cudaMalloc(&ctx->gf_cell_buf, coff));
-            ctx->gf_cell_buf_bytes = coff;
-        }
-        char *cb = (char *)ctx->gf_cell_buf;
+        if (const int rc = grow_scratch(ctx, ctx->gf_cell_buf, coff); rc != MULLS_OK) return rc;
+        char *cb = (char *)ctx->gf_cell_buf.p;
         A.cell_start = (uint32_t *)(cb + c_start), A.cell_end = (uint32_t *)(cb + c_end);
         A.min_z = (float *)(cb + c_minz), A.neighbor_min_z = (float *)(cb + c_nb), A.outlier_thre = (float *)(cb + c_oth);
         A.reliable = (int *)(cb + c_rel);
@@ -2315,14 +2239,8 @@ int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxe
     const size_t o_rows = take(n * row_b), o_out = take(n * row_b), o_key = take(8 * n), o_keys = take(8 * n);
     const size_t o_idx = take(4 * n), o_idxs = take(4 * n), o_head = take(4 * n), o_pos = take(4 * n), o_st = take(sizeof(VxState));
     const size_t o_tmp = take(std::max(sort_bytes, scan_bytes));
-    if (off > ctx->vx_buf_bytes) {
-        if (ctx->vx_buf) cudaFree(ctx->vx_buf);
-        ctx->vx_buf = nullptr;
-        ctx->vx_buf_bytes = 0;
-        CK(cudaMalloc(&ctx->vx_buf, off));
-        ctx->vx_buf_bytes = off;
-    }
-    char *base = (char *)ctx->vx_buf;
+    if (const int rc = grow_scratch(ctx, ctx->vx_buf, off); rc != MULLS_OK) return rc;
+    char *base = (char *)ctx->vx_buf.p;
     VxArgs V;
     V.n = (uint32_t)n;
     V.voxel_size = voxel_size;
@@ -2381,20 +2299,15 @@ int mulls_extract_semantic_pts(mulls_ctx *ctx, mulls_cloud_view pc_raw, const mu
     }
     CK(cudaSetDevice(ctx->device));
     // the clouds handed from stage to stage stay in HBM: pc_down and the ground filter's cloud_unground
-    const size_t row_b = 48, need = 2 * n * row_b;
-    if (need > ctx->ext_buf_bytes) {
-        if (ctx->ext_buf) cudaFree(ctx->ext_buf);
-        ctx->ext_buf = nullptr;
-        ctx->ext_buf_bytes = 0;
-        CK(cudaMalloc(&ctx->ext_buf, need));
-        ctx->ext_buf_bytes = need;
-    }
-    float *d_down = (float *)ctx->ext_buf, *d_ung = (float *)((char *)ctx->ext_buf + n * row_b);
+    const size_t row_b = 48;
+    int rc = grow_scratch(ctx, ctx->ext_buf, 2 * n * row_b);
+    if (rc != MULLS_OK) return rc;
+    float *d_down = (float *)ctx->ext_buf.p, *d_ung = (float *)((char *)ctx->ext_buf.p + n * row_b);
     float ms = 0.f;
     uint64_t launches = 0;
     // :2346 voxel_downsample(pc_raw, pc_down) (pc_sketch, :2348, is not a feature cloud and is not produced)
     size_t n_down = 0;
-    int rc = mulls_voxel_downsample(ctx, pc_raw, params->vf_downsample_resolution, d_down, n, &n_down);
+    rc = mulls_voxel_downsample(ctx, pc_raw, params->vf_downsample_resolution, d_down, n, &n_down);
     if (rc != MULLS_OK) return rc;
     ms += ctx->stats.ms_total, launches += ctx->stats.kernel_launches;
     out->n_down = n_down;

@@ -11,7 +11,6 @@ from mulls_b200.registration import Context
 n_pairs = int(sys.argv[1]) if len(sys.argv) > 1 else 16
 runs = int(sys.argv[2]) if len(sys.argv) > 2 else 3
 cfg = sys.argv[3] if len(sys.argv) > 3 else "c2"
-tun = dict(kv.split("=") for kv in sys.argv[4:])
 from concurrent.futures import ProcessPoolExecutor
 from mulls_b200 import abi
 def _gen(a):
@@ -34,8 +33,6 @@ print(f"box calibration: device copy {2 * a.numel() * 10 / e0.elapsed_time(e1) /
 del a, b
 ctx = Context(0, n_pairs, ns + 16, nt + 16)
 ctx.set_tunable("use_graph", 0)  # host launch loop: per-kernel CUDA events
-for k, v in tun.items():
-    ctx.set_tunable(k, int(v))
 ctx.upload(pairs)
 for r in range(runs):
     res, _ = ctx.run_resident()

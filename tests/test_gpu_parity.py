@@ -429,6 +429,8 @@ def test_graph_loop_equals_host_loop(oracle_mod, small_pair):
     for mode in (1, 0):
         ctx = Context(0, len(pairs), 30000, 30000)
         ctx.set_tunable("use_graph", mode)
+        with pytest.raises(RuntimeError):  # the search parameters are constants of the kernels, not tunables
+            ctx.set_tunable("leaf_count", 16)
         out[mode] = ctx.run_batch(pairs, want_trace=True)
         again = ctx.run_batch(pairs, want_trace=True)  # the recorded graph is re-launched, not rebuilt
         for a, b in zip(out[mode][0], again[0]):
