@@ -12,7 +12,6 @@
  *                                get_multi_metrics_lls_residual :2518-2677, the per-class PCL kd-tree
  *                                build :1209-1232, intersection_filter :2894-2922)
  *   mulls_icp_run_batch      <- the same call made for N independent scan pairs (BASELINE config 4)
- *   mulls_create_pipelined   <- (no reference counterpart: the scheduler that overlaps PCIe copies and kernels)
  *   mulls_batch_upload /
  *   mulls_batch_run_resident <- same, split so that inputs can stay resident in HBM between runs
  *   mulls_icp_run_sharded    <- the same call with the source clouds sharded over ranks
@@ -147,10 +146,6 @@ typedef struct mulls_ctx mulls_ctx;
 /* Create a context on CUDA device `device` able to hold `max_pairs` scan pairs of at most
  * `max_src_pts` source and `max_tgt_pts` target points each (sum over the six classes). */
 mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t max_tgt_pts);
-/* Same, with `n_lanes` independent lanes (own CUDA stream, buffers and host thread each): batch calls split their
- * pairs over the lanes, so that the H2D copy of one slice overlaps the registration of another and small kernels
- * fill each other's tails. Results are identical to a single-lane context (pairs are independent). */
-mulls_ctx *mulls_create_pipelined(int device, size_t max_pairs, size_t max_src_pts, size_t max_tgt_pts, int n_lanes);
 void mulls_destroy(mulls_ctx *ctx);
 const char *mulls_last_error(const mulls_ctx *ctx); /* ctx may be NULL: error of the failed create */
 

@@ -240,7 +240,6 @@ ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int,
 # every symbol include/mulls_b200/abi.h declares
 EXPORTED_SYMBOLS = (
     "mulls_create",
-    "mulls_create_pipelined",
     "mulls_destroy",
     "mulls_last_error",
     "mulls_icp_default_params",
@@ -296,8 +295,6 @@ def load_library() -> C.CDLL:
     vp = C.c_void_p
     lib.mulls_create.restype = vp
     lib.mulls_create.argtypes = [C.c_int, C.c_size_t, C.c_size_t, C.c_size_t]
-    lib.mulls_create_pipelined.restype = vp
-    lib.mulls_create_pipelined.argtypes = [C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
     lib.mulls_destroy.restype = None
     lib.mulls_destroy.argtypes = [vp]
     lib.mulls_last_error.restype = C.c_char_p

@@ -8,7 +8,6 @@
 #include <chrono>
 #include <cstring>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -131,9 +130,6 @@ struct mulls_ctx {
     mulls_run_stats stats{};
     std::vector<void *> allocs;
     std::string err;
-    // pipelined context (mulls_create_pipelined): the batch is split over independent lane contexts, each with
-    // its own stream and buffers, driven by one host thread each
-    std::vector<mulls_ctx *> lanes;
     // one-shot batch calls with host buffers (mulls_icp_run_batch) are double-buffered: the second half of the batch is
     // packed and copied on the twin's stream while the first half is being registered on this one
     mulls_ctx *twin = nullptr;
@@ -145,7 +141,6 @@ struct mulls_ctx {
         int n_search_ev = 0;
         bool graphed = false, hooked = false, active = false;
     } pend;
-    std::vector<size_t> lane_begin; // pair range of every lane for the resident batch
     // device scratch, grown on demand (grow_scratch)
     Scratch pca_buf;             // PCA
     Scratch cls_buf;             // classification (mulls_classify_nground)
@@ -226,8 +221,6 @@ const char *mulls_last_error(const mulls_ctx *ctx) { return ctx ? ctx->err.c_str
 
 void mulls_destroy(mulls_ctx *ctx) {
     if (!ctx) return;
-    for (mulls_ctx *l : ctx->lanes) mulls_destroy(l);
-    ctx->lanes.clear();
     if (ctx->twin) mulls_destroy(ctx->twin), ctx->twin = nullptr;
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
@@ -380,76 +373,8 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     return ctx;
 }
 
-mulls_ctx *mulls_create_pipelined(int device, size_t max_pairs, size_t max_src_pts, size_t max_tgt_pts, int n_lanes) {
-    if (n_lanes <= 1) return mulls_create(device, max_pairs, max_src_pts, max_tgt_pts);
-    if ((size_t)n_lanes > max_pairs) n_lanes = (int)max_pairs;
-    mulls_ctx *ctx = new mulls_ctx();
-    ctx->device = device;
-    ctx->max_pairs = max_pairs;
-    ctx->max_src = max_src_pts;
-    ctx->max_tgt = max_tgt_pts;
-    const size_t per_lane = (max_pairs + n_lanes - 1) / n_lanes;
-    for (int l = 0; l < n_lanes; ++l) {
-        mulls_ctx *c = mulls_create(device, per_lane, max_src_pts, max_tgt_pts);
-        if (!c) { // g_create_error is set by the failed create
-            mulls_destroy(ctx);
-            return nullptr;
-        }
-        ctx->lanes.push_back(c);
-    }
-    return ctx;
-}
-
-} // extern "C"
-
-// Run fn(lane, first_pair, n_pairs_of_lane) on every lane of a pipelined context, one host thread per lane;
-// pairs are split into contiguous, near-equal ranges. Returns the first non-zero code.
-template <typename F>
-static int for_each_lane(mulls_ctx *ctx, size_t n_pairs, F fn) {
-    const size_t L = ctx->lanes.size();
-    std::vector<int> rc(L, MULLS_OK);
-    std::vector<std::thread> th;
-    ctx->lane_begin.assign(L + 1, 0);
-    for (size_t l = 0; l <= L; ++l) ctx->lane_begin[l] = (n_pairs * l) / L;
-    for (size_t l = 0; l < L; ++l) {
-        const size_t b = ctx->lane_begin[l], n = ctx->lane_begin[l + 1] - b;
-        if (n == 0) continue;
-        th.emplace_back([&, l, b, n]() { rc[l] = fn(ctx->lanes[l], b, n); });
-    }
-    for (auto &t : th) t.join();
-    for (size_t l = 0; l < L; ++l)
-        if (rc[l] != MULLS_OK) {
-            ctx->err = ctx->lanes[l]->err;
-            return rc[l];
-        }
-    return MULLS_OK;
-}
-
-static void merge_lane_stats(mulls_ctx *ctx) {
-    mulls_run_stats &S = ctx->stats;
-    S = mulls_run_stats();
-    for (size_t l = 0; l < ctx->lanes.size(); ++l) {
-        if (ctx->lane_begin.size() > l + 1 && ctx->lane_begin[l + 1] == ctx->lane_begin[l]) continue;
-        const mulls_run_stats &s = ctx->lanes[l]->stats;
-        S.kernel_launches += s.kernel_launches;
-        S.algorithmic_bytes += s.algorithmic_bytes;
-        S.iterations += s.iterations;
-        S.search_launches += s.search_launches;
-        S.ms_search += s.ms_search; // summed over concurrently running lanes: not a wall time
-        S.ms_ingest = std::max(S.ms_ingest, s.ms_ingest);
-        S.ms_iterate = std::max(S.ms_iterate, s.ms_iterate);
-        S.ms_total = std::max(S.ms_total, s.ms_total);
-    }
-}
-
-extern "C" {
-
 int mulls_set_tunable(mulls_ctx *ctx, const char *name, int value) {
     if (!ctx || !name) return MULLS_E_ARG;
-    for (mulls_ctx *l : ctx->lanes) {
-        const int rc = mulls_set_tunable(l, name, value);
-        if (rc != MULLS_OK) return rc;
-    }
     if (ctx->twin) {
         const int rc = mulls_set_tunable(ctx->twin, name, value);
         if (rc != MULLS_OK) return rc;
@@ -1014,7 +939,7 @@ static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace
             // flow control: stay at most two iterations ahead of the device and stop launching as soon
             // as every pair has converged or failed (the device mirrors its counter into mapped memory)
             if (it >= 2) {
-                // (poll with pauses: several lanes spinning inside the driver slow each other's launches down)
+                // (poll with pauses: several contexts spinning inside the driver slow each other's launches down)
                 while (cudaEventQuery(ctx->ev_done[it - 2]) == cudaErrorNotReady)
                     for (int k = 0; k < kPollPause; ++k) _mm_pause();
                 // Sharded runs must take this decision identically on every rank (the ranks issue matching collectives):
@@ -1141,32 +1066,10 @@ static int run_finish_inner(mulls_ctx *ctx, mulls_icp_result *out) {
 
 int mulls_batch_upload(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *tgt, const mulls_cloud_view *src,
                        const mulls_icp_params *params, const double *init_guess) {
-    if (ctx && !ctx->lanes.empty()) {
-        if (!tgt || !src || !params || !init_guess || n_pairs == 0) return MULLS_E_ARG;
-        if (n_pairs > ctx->max_pairs) {
-            ctx->err = "more pairs than the context was created for";
-            return MULLS_E_CAPACITY;
-        }
-        ctx->n_pairs = n_pairs;
-        const int rc = for_each_lane(ctx, n_pairs, [&](mulls_ctx *lane, size_t b, size_t n) {
-            return upload_impl(lane, n, tgt + b * kNumClasses, src + b * kNumClasses, params + b, init_guess + 16 * b, nullptr,
-                               nullptr);
-        });
-        ctx->uploaded = (rc == MULLS_OK);
-        return rc;
-    }
     return upload_impl(ctx, n_pairs, tgt, src, params, init_guess, nullptr, nullptr);
 }
 
 int mulls_batch_run_resident(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace *trace) {
-    if (ctx && !ctx->lanes.empty()) {
-        if (!ctx->uploaded) return MULLS_E_ARG;
-        const int rc = for_each_lane(ctx, ctx->n_pairs, [&](mulls_ctx *lane, size_t b, size_t) {
-            return run_impl(lane, out ? out + b : nullptr, trace ? trace + b : nullptr, nullptr, nullptr);
-        });
-        merge_lane_stats(ctx);
-        return rc;
-    }
     return run_impl(ctx, out, trace, nullptr, nullptr);
 }
 
@@ -1227,23 +1130,6 @@ static int one_shot_batch(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view
 int mulls_icp_run_batch(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *tgt, const mulls_cloud_view *src,
                         const mulls_icp_params *params, const double *init_guess, mulls_icp_result *out,
                         mulls_icp_trace *trace) {
-    if (ctx && !ctx->lanes.empty()) {
-        // pipelined: every lane uploads and registers its slice on its own stream — while one slice is being
-        // registered the next one's clouds are already crossing PCIe
-        if (!tgt || !src || !params || !init_guess || n_pairs == 0) return MULLS_E_ARG;
-        if (n_pairs > ctx->max_pairs) {
-            ctx->err = "more pairs than the context was created for";
-            return MULLS_E_CAPACITY;
-        }
-        ctx->n_pairs = n_pairs;
-        ctx->uploaded = false;
-        const int rc = for_each_lane(ctx, n_pairs, [&](mulls_ctx *lane, size_t b, size_t n) {
-            return one_shot_batch(lane, n, tgt + b * kNumClasses, src + b * kNumClasses, params + b, init_guess + 16 * b,
-                                  out ? out + b : nullptr, trace ? trace + b : nullptr);
-        });
-        merge_lane_stats(ctx);
-        return rc;
-    }
     if (!ctx || !tgt || !src || !params || !init_guess || n_pairs == 0) return MULLS_E_ARG;
     return one_shot_batch(ctx, n_pairs, tgt, src, params, init_guess, out, trace);
 }
@@ -1270,7 +1156,6 @@ int mulls_nccl_unique_id(char id[MULLS_NCCL_ID_BYTES]) {
 
 int mulls_nccl_init(mulls_ctx *ctx, int rank, int world, const char id[MULLS_NCCL_ID_BYTES]) {
     if (!ctx || !id || world < 1 || rank < 0 || rank >= world) return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     NcclApi &api = nccl_api();
     if (!api.ok) {
         ctx->err = "libnccl.so.2 not found (or too old)";
@@ -1294,10 +1179,9 @@ int mulls_icp_run_sharded_nccl(mulls_ctx *ctx, void *comm, const mulls_cloud_vie
                                const uint32_t src_global_n[MULLS_NUM_CLASSES], const mulls_icp_params *params,
                                const double init_guess[16], mulls_icp_result *out, mulls_icp_trace *trace) {
     if (!ctx) return MULLS_E_ARG;
-    mulls_ctx *owner = ctx->lanes.empty() ? ctx : ctx->lanes[0];
-    if (!comm) comm = owner->nccl_comm;
+    if (!comm) comm = ctx->nccl_comm;
     if (!comm || !nccl_api().ok) {
-        owner->err = "no NCCL communicator: call mulls_nccl_init first (or pass an ncclComm_t)";
+        ctx->err = "no NCCL communicator: call mulls_nccl_init first (or pass an ncclComm_t)";
         return MULLS_E_COMM;
     }
     return mulls_icp_run_sharded(ctx, tgt, src_shard, src_index_base, src_global_n, params, init_guess, nccl_allreduce_hook, comm, out,
@@ -1306,7 +1190,6 @@ int mulls_icp_run_sharded_nccl(mulls_ctx *ctx, void *comm, const mulls_cloud_vie
 
 int mulls_nn_query(mulls_ctx *ctx, int cls, const float *xyz, size_t n, int32_t *idx, float *d2) {
     if (!ctx || cls < 0 || cls >= kNumClasses || (n > 0 && (!xyz || !idx || !d2))) return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0]; // (a pipelined context answers for the first pair of its first lane)
     if (!ctx->grid_valid) {
         ctx->err = "mulls_nn_query: no registration has run on this context since its last upload";
         return MULLS_E_ARG;
@@ -1338,7 +1221,6 @@ int mulls_icp_run_sharded(mulls_ctx *ctx, const mulls_cloud_view tgt[MULLS_NUM_C
                           const mulls_icp_params *params, const double init_guess[16], mulls_allreduce_fn allreduce,
                           void *user, mulls_icp_result *out, mulls_icp_trace *trace) {
     if (!ctx || !allreduce || !params) return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     if (params->keep_less_source_points && !params->apply_motion_undistortion_while_registration) {
         // the down-sampling quota and its sampling keys are defined over the WHOLE source cloud (:2866-2892); a
         // shard-local plan would keep ~world times too many points and a different subset than the unsharded run
@@ -1404,7 +1286,6 @@ int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int
     if (!ctx || !out || !out->eigenvalues || !out->principal || !out->normal || !out->pt_num || stride < 1 ||
         !(radius > 0.f))
         return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     PcaArgs args;
     uint64_t launches = 0;
     const size_t n = cloud.n;
@@ -1537,7 +1418,6 @@ void mulls_map_destroy(mulls_map *m) {
 
 mulls_map *mulls_map_create(mulls_ctx *ctx, size_t max_pts_per_class) {
     if (!ctx || max_pts_per_class == 0 || max_pts_per_class >= (1ull << 31)) return nullptr;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     if (cudaSetDevice(ctx->device) != cudaSuccess) return nullptr;
     mulls_map *m = new mulls_map();
     m->ctx = ctx;
@@ -1775,7 +1655,6 @@ int mulls_icp_run_to_map(mulls_ctx *ctx, mulls_map *m, const mulls_cloud_view sr
                          const mulls_icp_params *params, const double init_guess[16], mulls_icp_result *out,
                          mulls_icp_trace *trace) {
     if (!ctx || !m || !src || !params || !init_guess) return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     if (ctx != m->ctx) {
         ctx->err = "mulls_icp_run_to_map: the map belongs to another context";
         return MULLS_E_ARG;
@@ -1835,7 +1714,6 @@ void mulls_classify_default_params(mulls_classify_params *p) {
 int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_classify_params *params,
                            mulls_classify_out *out) {
     if (!ctx || !params || !out || (cloud_in.n > 0 && !cloud_in.aos48)) return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     const mulls_classify_params &P = *params;
     if (P.use_distance_adaptive_pca) {
         ctx->err = "mulls_classify_nground: use_distance_adaptive_pca is not implemented";
@@ -2047,7 +1925,6 @@ void mulls_ground_default_params(mulls_ground_params *p) { // extract_semantic_p
 int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_ground_params *params,
                              mulls_ground_out *out) {
     if (!ctx || !params || !out || (cloud_in.n > 0 && !cloud_in.aos48)) return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     const mulls_ground_params &P = *params;
     if (P.estimate_ground_normal_method != 0 && P.estimate_ground_normal_method != 3) {
         ctx->err = "mulls_fast_ground_filter: estimate_ground_normal_method 1 / 2 (pcl::NormalEstimation) are not implemented";
@@ -2205,7 +2082,6 @@ extern "C" {
 
 int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxel_size, float *out, size_t cap, size_t *n_out) {
     if (!ctx || !n_out || (cloud_in.n > 0 && (!cloud_in.aos48 || !out))) return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     *n_out = 0;
     const size_t n = cloud_in.n;
     if (n == 0) return MULLS_OK;
@@ -2288,7 +2164,6 @@ int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxe
 int mulls_extract_semantic_pts(mulls_ctx *ctx, mulls_cloud_view pc_raw, const mulls_extract_params *params,
                                mulls_extract_out *out) {
     if (!ctx || !params || !out || (pc_raw.n > 0 && !pc_raw.aos48)) return MULLS_E_ARG;
-    if (!ctx->lanes.empty()) ctx = ctx->lanes[0];
     out->n_down = out->n_ground = out->n_ground_down = 0;
     for (int k = 0; k < MULLS_OUT_COUNT; ++k) out->cls.n[k] = 0;
     const size_t n = pc_raw.n;

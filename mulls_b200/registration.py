@@ -87,15 +87,9 @@ class Constraint:
 class Context:
     """Thin RAII wrapper of a mulls_ctx (one CUDA device, one stream)."""
 
-    def __init__(self, device: int = 0, max_pairs: int = 1, max_src_pts: int = 150000, max_tgt_pts: int = 150000,
-                 lanes: int = 1):
-        """lanes > 1: mulls_create_pipelined — batch calls are split over `lanes` native lanes (own stream, buffers
-        and host thread each) inside the library."""
+    def __init__(self, device: int = 0, max_pairs: int = 1, max_src_pts: int = 150000, max_tgt_pts: int = 150000):
         self.lib = abi.load_library()
-        if lanes > 1:
-            self.handle = self.lib.mulls_create_pipelined(device, max_pairs, max_src_pts, max_tgt_pts, lanes)
-        else:
-            self.handle = self.lib.mulls_create(device, max_pairs, max_src_pts, max_tgt_pts)
+        self.handle = self.lib.mulls_create(device, max_pairs, max_src_pts, max_tgt_pts)
         if not self.handle:
             raise RuntimeError(self.lib.mulls_last_error(None).decode())
         self.max_pairs = max_pairs
@@ -313,14 +307,22 @@ class PipelinedContext:
         bounds = [(n * i) // k for i in range(k + 1)]
         return [pairs[bounds[i]:bounds[i + 1]] for i in range(k)]
 
-    def run_batch(self, pairs):
-        """Host buffers in, results out; slices are uploaded and registered concurrently."""
-        parts = self._split(pairs)
-        futs = [self.pool.submit(lambda c=c, p=p: c.run_batch(p)[0] if p else []) for c, p in zip(self.lanes, parts)]
-        out = []
+    @staticmethod
+    def _join(futs, want_trace: bool):
+        out, traces = [], []
         for f in futs:
-            out += f.result()
-        return out
+            o, t = f.result()
+            out += o
+            traces += t or []
+        return out, (traces if want_trace else None)
+
+    def run_batch(self, pairs, want_trace: bool = False):
+        """Host buffers in, results out; slices are uploaded and registered concurrently. Returns (results, traces)
+        in the order of `pairs`, as Context.run_batch does."""
+        parts = self._split(pairs)
+        futs = [self.pool.submit(lambda c=c, p=p: c.run_batch(p, want_trace) if p else ([], None))
+                for c, p in zip(self.lanes, parts)]
+        return self._join(futs, want_trace)
 
     def upload(self, pairs):
         self._slices = self._split(pairs)
@@ -328,12 +330,12 @@ class PipelinedContext:
             if p:
                 c.upload(p)
 
-    def run_resident(self):
-        futs = [self.pool.submit(lambda c=c, p=p: c.run_resident()[0] if p else []) for c, p in zip(self.lanes, self._slices)]
-        out = []
-        for f in futs:
-            out += f.result()
-        return out
+    def run_resident(self, want_trace: bool = False):
+        """One pass over the resident batch, the slices registered concurrently. Returns (results, traces) as
+        Context.run_resident does."""
+        futs = [self.pool.submit(lambda c=c, p=p: c.run_resident(want_trace) if p else ([], None))
+                for c, p in zip(self.lanes, self._slices)]
+        return self._join(futs, want_trace)
 
     def run_resident_steps(self, k: int):
         """k passes over the resident batch; every lane runs its k passes back to back (no per-step barrier

@@ -301,27 +301,31 @@ def test_keep_less_source_points(ctx, oracle_mod, small_pair):
     assert not np.array_equal(r1[0]["T"], r2[0]["T"])
 
 
-def test_native_pipelined_context_equals_single_lane(small_pair):
-    """mulls_create_pipelined: the batch is split over native lanes (own stream + host thread each); results are
-    bit-identical to a one-lane context, for one-shot and resident runs, with fewer pairs than lanes too."""
-    from mulls_b200.registration import Context
+def test_pipelined_context_equals_single_context(small_pair):
+    """PipelinedContext: the batch is split over independent contexts (own stream + host thread each); results are
+    bit-identical to one context, for one-shot and resident runs, with fewer pairs than contexts too."""
+    from mulls_b200.registration import Context, PipelinedContext
 
     pairs = [small_pair, synth.make_pair(1003, "small"), small_pair, synth.make_pair(1004, "small"), small_pair]
     one = Context(0, 5, 100000, 100000)
     ref, _ = one.run_batch(pairs)
-    pipe = Context(0, 5, 100000, 100000, lanes=3)
+    pipe = PipelinedContext(0, 3, 2, 100000, 100000)
     got, tr = pipe.run_batch(pairs, want_trace=True)
+    assert len(got) == len(tr) == len(pairs)
     for a, b in zip(ref, got):
         np.testing.assert_array_equal(a["T"], b["T"])
         assert a["code"] == b["code"] and a["n_corr"] == b["n_corr"]
     assert tr[4]["n_iter"] == got[4]["iters"]
     pipe.upload(pairs)
     again, _ = pipe.run_resident()
+    assert len(again) == len(pairs)
     for a, b in zip(ref, again):
         np.testing.assert_array_equal(a["T"], b["T"])
+        assert a["code"] == b["code"] and a["n_corr"] == b["n_corr"]
     st = pipe.stats()
-    assert st["iterations"] == sum(r["iters"] for r in ref) and st["kernel_launches"] > 0
-    few, _ = pipe.run_batch(pairs[:2])  # fewer pairs than lanes
+    assert sum(s["iterations"] for s in st) == sum(r["iters"] for r in ref)
+    assert sum(s["kernel_launches"] for s in st) > 0
+    few, _ = pipe.run_batch(pairs[:2])  # fewer pairs than contexts
     np.testing.assert_array_equal(few[1]["T"], ref[1]["T"])
     one.close()
     pipe.close()
@@ -346,10 +350,10 @@ def test_normal_shooting_correspondences(ctx, oracle_mod, small_pair):
 def test_host_packed_wire_format_is_bit_identical(oracle_mod, small_pair):
     """The "host_pack" tunable repacks the 48-byte rows to the 28 B (32 B with motion undistortion) wire format on
     the host cores before the DMA (csrc/host_pack.h). Every result bit must be the same as with the raw rows: one
-    context, a pipelined context (lanes share the worker pool), resident re-runs, the undistortion variant (format 2),
+    context, a pipelined context (its contexts share the worker pool), resident re-runs, the undistortion variant (format 2),
     ragged / empty classes, and the resident-map path (device rows for the target, packed source)."""
     from mulls_b200.map_manager import LocalMap
-    from mulls_b200.registration import Context
+    from mulls_b200.registration import Context, PipelinedContext
 
     rng = np.random.default_rng(11)
     src_u = [s.copy() for s in small_pair["src"]]
@@ -388,7 +392,7 @@ def test_host_packed_wire_format_is_bit_identical(oracle_mod, small_pair):
     np.testing.assert_array_equal(one[0]["T"], ref[3]["T"])
     raw.close()
 
-    pipe = Context(0, 5, 100000, 100000, lanes=3)
+    pipe = PipelinedContext(0, 3, 2, 100000, 100000)
     pipe.set_tunable("host_pack", 1)
     same(*pipe.run_batch(pairs, want_trace=True))
     pipe.upload(pairs)
