@@ -126,8 +126,6 @@ struct LoopCtl {
 // All device pointers of a context, passed by value to the kernels.
 struct DeviceArrays {
     const float4 *in_aos;   // input clouds, 3 float4 per point (pcl::PointXYZINormal)
-    float4 *stg_pos;        // staging (input order): x y z intensity  (source: initial guess applied)
-    float4 *stg_nrm;        // staging: nx ny nz orig_index(bits)
     uint64_t *keys_a, *keys_b;
     uint32_t *vals_a, *vals_b;
     float4 *tgt_pos, *tgt_nrm;       // target SoA, Morton-sorted inside each (pair,class) slice

@@ -7,7 +7,7 @@
 // before the DMA:
 //   format 1 (28 B/point):  [n x float4 (x y z intensity)] [n x 3 floats (nx ny nz)]   (padded to a float4 boundary)
 //   format 2 (32 B/point):  [n x float4 (x y z intensity)] [n x float4 (nx ny nz curvature)]
-// k_ingest_transform reads either format or the raw rows (format 0: device-resident clouds of the local map, PCA).
+// The ingest (load_input_point, kernels_ingest.cuh) reads either format or the raw rows (format 0: device-resident clouds of the local map, PCA).
 // The pool is a process-wide set of detached worker threads fed by every context / lane; the submitting thread
 // helps until its own jobs are done.
 #pragma once

@@ -7,96 +7,116 @@
 
 namespace mulls {
 
-// ---- k_ingest_transform: AoS48 -> staging SoA; source gets the initial guess (double math, float store,
-//      pcl::transformPointCloudWithNormals semantics); bbox reductions for the intersection filter.
-// kUndistort = false: the instantiation for batches in which no pair asks for motion undistortion (no slerp code, 32
-// registers, 8 blocks per SM — the kernel is a latency-bound stream: 28 B read + 32 B written per point)
-template <bool kUndistort>
-__global__ void __launch_bounds__(kIngestBlock, kUndistort ? 4 : 6) k_ingest_transform(DeviceArrays A) {
-    const ChunkDesc cd = A.in_chunks[blockIdx.x];
-    const PairConst &pc = A.pc[cd.pair];
-    const uint32_t seg = cd.seg;
-    const uint32_t local = cd.first + threadIdx.x;
-    const bool valid = local < pc.in_n[seg];
+// ---- load_input_point: input point `local` of segment `seg`, read from whichever of the three layouts is behind
+//      in_ptr (block-uniform): the caller's 48-byte rows, or the host-packed wire formats (host_pack.h). A source point
+//      gets the motion undistortion and the initial guess (double math, float store,
+//      pcl::transformPointCloudWithNormals semantics). The bbox pass, k_make_keys and k_gather each recompute the point
+//      here instead of reading a staged copy: one function, so every recomputation gives the same bits.
+// kUndistort = false: the instantiation for batches in which no pair asks for motion undistortion (no slerp code).
+// kNormals = false: position only (nrm untouched); the position does not depend on the normal, so its bits are the same.
+template <bool kUndistort, bool kNormals>
+__device__ __forceinline__ void load_input_point(const PairConst &pc, uint32_t seg, uint32_t local, float4 &pos, float4 &nrm) {
     const bool is_src = seg >= kNumClasses;
     const int cls = seg % kNumClasses;
-    float x = 0, y = 0, z = 0;
-    if (valid) {
-        const size_t gi = (size_t)pc.in_off[seg] + local;
-        // three layouts behind in_ptr (block-uniform): the caller's 48-byte rows, or the host-packed wire formats
-        float nx, ny, nz, intensity, curvature = 0.0f;
-        const uint32_t fmt = pc.in_fmt[seg];
-        if (fmt == 0u) {
-            const float4 *in = pc.in_ptr[seg] + 3 * (size_t)local;
-            const float4 a = in[0]; // x y z _
+    const bool undistort = kUndistort && is_src && pc.undistort && cls != MULLS_VERTEX;
+    float x, y, z, intensity = 0.0f, curvature = 0.0f;
+    float nx = 0.0f, ny = 0.0f, nz = 0.0f;
+    const uint32_t fmt = pc.in_fmt[seg];
+    if (fmt == 0u) {
+        const float4 *in = pc.in_ptr[seg] + 3 * (size_t)local;
+        const float4 a = in[0]; // x y z _
+        x = a.x, y = a.y, z = a.z;
+        if (kNormals) {
             const float4 b = in[1]; // nx ny nz _
             const float4 c = in[2]; // intensity curvature _ _
-            x = a.x, y = a.y, z = a.z;
             nx = b.x, ny = b.y, nz = b.z;
             intensity = c.x, curvature = c.y;
-        } else {
-            const float4 *in = pc.in_ptr[seg];
-            const float4 a = in[local]; // x y z intensity
-            x = a.x, y = a.y, z = a.z, intensity = a.w;
-            if (fmt == 1u) {
+        } else if (undistort) {
+            curvature = reinterpret_cast<const float *>(in + 2)[1];
+        }
+    } else {
+        const float4 *in = pc.in_ptr[seg];
+        const float4 a = in[local]; // x y z intensity
+        x = a.x, y = a.y, z = a.z, intensity = a.w;
+        if (fmt == 1u) {
+            if (kNormals) {
                 const float *nr = reinterpret_cast<const float *>(in + pc.in_n[seg]) + 3 * (size_t)local;
                 nx = nr[0], ny = nr[1], nz = nr[2];
-            } else {
-                const float4 b = in[(size_t)pc.in_n[seg] + local]; // nx ny nz curvature
-                nx = b.x, ny = b.y, nz = b.z, curvature = b.w;
             }
+        } else if (kNormals) {
+            const float4 b = in[(size_t)pc.in_n[seg] + local]; // nx ny nz curvature
+            nx = b.x, ny = b.y, nz = b.z, curvature = b.w;
+        } else if (undistort) {
+            curvature = in[(size_t)pc.in_n[seg] + local].w;
         }
-        if (is_src) {
-            const double *t = pc.init;
-            int n_apply = 1;
-            if (kUndistort && pc.undistort) {
-                if (cls == MULLS_VERTEX) {
-                    n_apply = 2; // not undistorted and not re-cloned: the initial guess lands twice (reference behaviour)
-                } else {
-                    const float curv = curvature; // timestamp ratio of the point inside its frame
-                    if (!(curv < 0.0f || (double)curv > 1.0)) {
-                        const double s = (double)curv;
-                        double scale0, scale1;
-                        if (pc.ud_linear) {
-                            scale0 = 1.0 - s;
-                            scale1 = s;
-                        } else {
-                            scale0 = sin((1.0 - s) * pc.ud_theta) / pc.ud_sin_theta;
-                            scale1 = sin(s * pc.ud_theta) / pc.ud_sin_theta;
-                        }
-                        if (pc.ud_neg) scale1 = -scale1;
-                        const double qx = scale1 * pc.ud_q[0], qy = scale1 * pc.ud_q[1], qz = scale1 * pc.ud_q[2],
-                                     qw = scale0 + scale1 * pc.ud_q[3];
-                        const double vx = x, vy = y, vz = z;
-                        double ux = qy * vz - qz * vy, uy = qz * vx - qx * vz, uz = qx * vy - qy * vx;
-                        ux += ux, uy += uy, uz += uz;
-                        const double rx = vx + qw * ux + (qy * uz - qz * uy);
-                        const double ry = vy + qw * uy + (qz * ux - qx * uz);
-                        const double rz = vz + qw * uz + (qx * uy - qy * ux);
-                        x = (float)(rx + s * pc.ud_t[0]);
-                        y = (float)(ry + s * pc.ud_t[1]);
-                        z = (float)(rz + s * pc.ud_t[2]);
+    }
+    if (is_src) {
+        const double *t = pc.init;
+        int n_apply = 1;
+        if (kUndistort && pc.undistort) {
+            if (cls == MULLS_VERTEX) {
+                n_apply = 2; // not undistorted and not re-cloned: the initial guess lands twice (reference behaviour)
+            } else {
+                const float curv = curvature; // timestamp ratio of the point inside its frame
+                if (!(curv < 0.0f || (double)curv > 1.0)) {
+                    const double s = (double)curv;
+                    double scale0, scale1;
+                    if (pc.ud_linear) {
+                        scale0 = 1.0 - s;
+                        scale1 = s;
+                    } else {
+                        scale0 = sin((1.0 - s) * pc.ud_theta) / pc.ud_sin_theta;
+                        scale1 = sin(s * pc.ud_theta) / pc.ud_sin_theta;
                     }
+                    if (pc.ud_neg) scale1 = -scale1;
+                    const double qx = scale1 * pc.ud_q[0], qy = scale1 * pc.ud_q[1], qz = scale1 * pc.ud_q[2],
+                                 qw = scale0 + scale1 * pc.ud_q[3];
+                    const double vx = x, vy = y, vz = z;
+                    double ux = qy * vz - qz * vy, uy = qz * vx - qx * vz, uz = qx * vy - qy * vx;
+                    ux += ux, uy += uy, uz += uz;
+                    const double rx = vx + qw * ux + (qy * uz - qz * uy);
+                    const double ry = vy + qw * uy + (qz * ux - qx * uz);
+                    const double rz = vz + qw * uz + (qx * uy - qy * ux);
+                    x = (float)(rx + s * pc.ud_t[0]);
+                    y = (float)(ry + s * pc.ud_t[1]);
+                    z = (float)(rz + s * pc.ud_t[2]);
                 }
             }
-            for (int rep = 0; rep < n_apply; ++rep) {
-                const double px = x, py = y, pz = z, qx = nx, qy = ny, qz = nz;
-                x = (float)(t[0] * px + t[1] * py + t[2] * pz + t[3]);
-                y = (float)(t[4] * px + t[5] * py + t[6] * pz + t[7]);
-                z = (float)(t[8] * px + t[9] * py + t[10] * pz + t[11]);
+        }
+        for (int rep = 0; rep < n_apply; ++rep) {
+            const double px = x, py = y, pz = z;
+            x = (float)(t[0] * px + t[1] * py + t[2] * pz + t[3]);
+            y = (float)(t[4] * px + t[5] * py + t[6] * pz + t[7]);
+            z = (float)(t[8] * px + t[9] * py + t[10] * pz + t[11]);
+            if (kNormals) {
+                const double qx = nx, qy = ny, qz = nz;
                 nx = (float)(t[0] * qx + t[1] * qy + t[2] * qz);
                 ny = (float)(t[4] * qx + t[5] * qy + t[6] * qz);
                 nz = (float)(t[8] * qx + t[9] * qy + t[10] * qz);
             }
         }
-        A.stg_pos[gi] = make_float4(x, y, z, intensity);
-        A.stg_nrm[gi] = make_float4(nx, ny, nz, __int_as_float((int)local));
     }
-    // bbox: source ground/pillar/facade (cregistration.hpp:2912-2915) and all target points (grid extent)
+    pos = make_float4(x, y, z, intensity);
+    if (kNormals) nrm = make_float4(nx, ny, nz, __int_as_float((int)local));
+}
+
+// ---- k_ingest_bbox: bbox reductions for the intersection filter: source ground/pillar/facade
+//      (cregistration.hpp:2912-2915) and all target points (grid extent). Reads positions only, writes nothing per point.
+template <bool kUndistort>
+__global__ void __launch_bounds__(kIngestBlock) k_ingest_bbox(DeviceArrays A) {
+    const ChunkDesc cd = A.in_chunks[blockIdx.x];
+    const PairConst &pc = A.pc[cd.pair];
+    const uint32_t seg = cd.seg;
+    const bool is_src = seg >= kNumClasses;
+    const int cls = seg % kNumClasses;
     const bool want = is_src ? (cls == MULLS_GROUND || cls == MULLS_PILLAR || cls == MULLS_FACADE) : true;
     if (!want) return; // block-uniform
-    float mn[3] = {valid ? x : FLT_MAX, valid ? y : FLT_MAX, valid ? z : FLT_MAX};
-    float mx[3] = {valid ? x : -FLT_MAX, valid ? y : -FLT_MAX, valid ? z : -FLT_MAX};
+    const uint32_t local = cd.first + threadIdx.x;
+    const bool valid = local < pc.in_n[seg];
+    float4 p = make_float4(0.f, 0.f, 0.f, 0.f), unused;
+    if (valid) load_input_point<kUndistort, false>(pc, seg, local, p, unused);
+    float mn[3] = {valid ? p.x : FLT_MAX, valid ? p.y : FLT_MAX, valid ? p.z : FLT_MAX};
+    float mx[3] = {valid ? p.x : -FLT_MAX, valid ? p.y : -FLT_MAX, valid ? p.z : -FLT_MAX};
 #pragma unroll
     for (int d = 0; d < 3; ++d)
 #pragma unroll
@@ -207,6 +227,7 @@ __global__ void k_pair_setup(DeviceArrays A, int n_pairs) {
 
 // ---- k_make_keys: intersection filter (cfilter.hpp:950-981: strictly inside) + 64-bit sort key
 //      [pair*12+seg | morton36(cell)]; filtered-out points sort to the very end.
+template <bool kUndistort>
 __global__ void __launch_bounds__(kIngestBlock) k_make_keys(DeviceArrays A) {
     const ChunkDesc cd = A.in_chunks[blockIdx.x];
     const PairConst &pc = A.pc[cd.pair];
@@ -217,7 +238,8 @@ __global__ void __launch_bounds__(kIngestBlock) k_make_keys(DeviceArrays A) {
     bool inside = false;
     if (valid) {
         const size_t gi = (size_t)pc.in_off[seg] + local;
-        const float4 p = A.stg_pos[gi];
+        float4 p, unused;
+        load_input_point<kUndistort, false>(pc, seg, local, p, unused);
         const double *b = ps.ibb;
         inside = (double)p.x > b[0] && (double)p.x < b[3] && (double)p.y > b[1] && (double)p.y < b[4] &&
                  (double)p.z > b[2] && (double)p.z < b[5];
@@ -400,29 +422,52 @@ __global__ void k_seg_offsets(DeviceArrays A, int n_pairs) {
     }
 }
 
-// ---- k_gather: sorted order -> final SoA slices (targets, and source buffer 0)
+// Sorted elements i-1 and i (kcur = keys[i]): the target cells that start at i are those of levels 0..top, where top
+// is the highest level at which the two Morton codes differ (every level at the start of a target segment); -1: none.
+__device__ __forceinline__ int cell_top(const uint64_t *keys, uint32_t i, uint64_t kcur) {
+    if (kcur == ~0ull || ((uint32_t)(kcur >> 36) % kNumSegs) >= kNumClasses) return -1;
+    if (i == 0) return kMaxLevels - 1;
+    const uint64_t kprev = keys[i - 1];
+    if ((kprev >> 36) != (kcur >> 36)) return kMaxLevels - 1;
+    const uint64_t diff = (kcur ^ kprev) & ((1ull << 36) - 1);
+    if (diff == 0) return -1; // same finest cell: no boundary at any level
+    return (63 - __clzll((long long)diff)) / 3;
+}
+
+// ---- k_gather: sorted order -> final SoA slices (targets, and source buffer 0), each point recomputed from the input
+//      by load_input_point (normal .w = the point's index in its input cloud). Also counts the grid cells of every
+//      (pair, class) -> PairState::hash_entries, from which k_hash_layout sizes the tables.
+template <bool kUndistort>
 __global__ void __launch_bounds__(256) k_gather(DeviceArrays A, const uint64_t *keys, const uint32_t *vals, uint32_t n_total) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_total) return;
-    const uint64_t key = keys[i];
-    if (key == ~0ull) return;
+    const uint64_t key = i < n_total ? keys[i] : ~0ull;
     const uint32_t sg = (uint32_t)(key >> 36);
     const uint32_t pair = sg / kNumSegs, seg = sg % kNumSegs;
+    const int top = cell_top(keys, i, key);
+    const int cnt = top < 0 ? 0 : min(top, A.ps[pair].n_levels - 1) + 1;
+    // one atomic per warp when all its lanes hold points of the same target segment (the common case)
+    const bool is_tgt = key != ~0ull && seg < kNumClasses;
+    const unsigned grp = __match_any_sync(0xffffffffu, is_tgt ? sg : 0xffffffffu);
+    if (grp == 0xffffffffu) {
+        const int tot = __reduce_add_sync(0xffffffffu, cnt);
+        if ((threadIdx.x & 31) == 0 && tot > 0) atomicAdd(&A.ps[pair].hash_entries[seg], (unsigned)tot);
+    } else if (cnt > 0) {
+        atomicAdd(&A.ps[pair].hash_entries[seg], (unsigned)cnt);
+    }
+    if (key == ~0ull) return;
     const PairConst &pc = A.pc[pair];
+    float4 pos, nrm;
+    load_input_point<kUndistort, true>(pc, seg, vals[i] - pc.in_off[seg], pos, nrm);
     const uint32_t local = i - A.ps[pair].seg_start[seg];
-    const uint32_t v = vals[i];
-    const float4 pos = A.stg_pos[v];
-    const float4 nrm = A.stg_nrm[v];
     if (seg < kNumClasses) {
         const uint32_t d = pc.tgt_base[seg] + local;
         A.tgt_pos[d] = pos;
         A.tgt_nrm[d] = nrm;
     } else {
         const uint32_t d = pc.src_base[seg - kNumClasses] + local;
-        float4 n2 = nrm;
-        if (pc.sharded) n2.w = __int_as_float(__float_as_int(nrm.w) + (int)pc.src_index_base[seg - kNumClasses]);
+        if (pc.sharded) nrm.w = __int_as_float(__float_as_int(nrm.w) + (int)pc.src_index_base[seg - kNumClasses]);
         A.src_pos[0][d] = pos;
-        A.src_nrm[0][d] = n2;
+        A.src_nrm[0][d] = nrm;
         A.src_prevj[0][d] = -1;
         A.src_cert[0][d] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
@@ -430,101 +475,77 @@ __global__ void __launch_bounds__(256) k_gather(DeviceArrays A, const uint64_t *
 
 // ---- hashed multi-level grid over a target class --------------------------------------------
 // Entry = {key_lo, key_hi | child mask << 16, start, count} (grid_key.cuh); (0, 0) marks an empty slot.
-__device__ __forceinline__ void hash_insert(HashEntry *table, uint32_t mask, uint32_t klo, uint32_t khi, uint32_t start) {
-    uint32_t slot = cell_hash(klo, khi) & mask;
-    const unsigned long long packed = (unsigned long long)klo | ((unsigned long long)khi << 32);
+// The slot follows from the key alone; the child mask rides along in the claimed word.
+__device__ __forceinline__ void hash_insert(HashEntry *table, uint32_t hmask, uint32_t klo, uint32_t khi, uint32_t children,
+                                            uint32_t start, uint32_t count) {
+    uint32_t slot = cell_hash(klo, khi) & hmask;
+    const unsigned long long packed = (unsigned long long)klo | ((unsigned long long)(khi | (children << 16)) << 32);
     while (true) {
         unsigned long long *kp = reinterpret_cast<unsigned long long *>(&table[slot]);
-        unsigned long long old = atomicCAS(kp, 0ull, packed);
-        if (old == 0ull) {
-            table[slot].start = start;
+        if (atomicCAS(kp, 0ull, packed) == 0ull) {
+            *reinterpret_cast<uint2 *>(&table[slot].start) = make_uint2(start, count);
             return;
         }
-        slot = (slot + 1) & mask;
-    }
-}
-// key_hi carries, above the 16 key bits, the 8-bit mask of existing children (set while closing cells)
-__device__ __forceinline__ HashEntry *hash_find(HashEntry *table, uint32_t mask, uint32_t klo, uint32_t khi) {
-    uint32_t slot = cell_hash(klo, khi) & mask;
-    while (true) {
-        const uint32_t lo = *reinterpret_cast<volatile uint32_t *>(&table[slot].key_lo);
-        const uint32_t hi = *reinterpret_cast<volatile uint32_t *>(&table[slot].key_hi);
-        if (lo == klo && (hi & kKeyHiMask) == khi) return &table[slot];
-        if (lo == 0u && hi == 0u) return nullptr;
-        slot = (slot + 1) & mask;
+        slot = (slot + 1) & hmask;
     }
 }
 
-// k_hash_build: thread i looks at the boundary between sorted elements i-1 and i. Where the Morton
-// prefix changes, a new cell starts at every level up to the highest differing one.
-//   mode 0: count the cells per (pair, class)          -> PairState::hash_entries
-//   mode 1: open cells: insert {key, start}
-//   mode 2: close cells: write the count of every cell the previous point ended
-__global__ void __launch_bounds__(256) k_hash_build(DeviceArrays A, const uint64_t *keys, uint32_t n_total, int mode) {
+// End of the cell of sorted element b at the level of `shift` (= 3 * level): the keys in [b, end) are those equal to
+// p = keys[b] >> shift, a prefix of [b, hi) since the keys are sorted. Galloping search: O(log size) loads, starting
+// next to b, so the many small cells cost a load or two.
+__device__ __forceinline__ uint32_t cell_end(const uint64_t *keys, uint32_t b, uint32_t hi, uint64_t p, int shift) {
+    uint32_t in = b, out = hi, step = 1;
+    while (in + step < hi) {
+        if ((keys[in + step] >> shift) != p) {
+            out = in + step;
+            break;
+        }
+        in += step;
+        step <<= 1;
+    }
+    while (out - in > 1) {
+        const uint32_t mid = in + (out - in) / 2;
+        if ((keys[mid] >> shift) == p) in = mid;
+        else out = mid;
+    }
+    return out;
+}
+
+// k_hash_build: thread i opens the cells that start at sorted element i (cell_top), at levels 0..min(top, L-1), and
+// writes each entry complete. A level-l cell ends where the last of its children (level l-1 cells, contiguous in Morton
+// order) ends; the first child is the level-(l-1) cell opened at i, the others are found by galloping from its end, and
+// their octants (x bit | y bit << 1 | z bit << 2 of the child's coordinates) make the child mask.
+__global__ void __launch_bounds__(256) k_hash_build(DeviceArrays A, const uint64_t *keys, uint32_t n_total) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool in_range = i <= n_total;
-    const uint64_t kcur = (in_range && i < n_total) ? keys[i] : ~0ull;
-    const uint64_t kprev = (in_range && i > 0) ? keys[i - 1] : ~0ull;
-    const bool cur_t = kcur != ~0ull && ((uint32_t)(kcur >> 36) % kNumSegs) < kNumClasses;
-    const bool prev_t = kprev != ~0ull && ((uint32_t)(kprev >> 36) % kNumSegs) < kNumClasses;
-    const bool same_seg = cur_t && prev_t && (kcur >> 36) == (kprev >> 36);
-    const uint64_t mmask = (1ull << 36) - 1;
-    int top = kMaxLevels - 1; // highest level at which the cell changes
-    bool boundary = true;
-    if (same_seg) {
-        const uint64_t diff = (kcur ^ kprev) & mmask;
-        if (diff == 0) boundary = false; // same finest cell: no boundary at any level
-        else top = (63 - __clzll((long long)diff)) / 3;
-    }
-    if (mode == 0) {
-        uint32_t sg = cur_t ? (uint32_t)(kcur >> 36) : 0xffffffffu;
-        int cnt = 0;
-        if (cur_t && boundary) {
-            const int L = A.ps[sg / kNumSegs].n_levels;
-            cnt = min(top, L - 1) + 1;
-        }
-        const unsigned grp = __match_any_sync(0xffffffffu, sg);
-        if (grp == 0xffffffffu) {
-            const int tot = __reduce_add_sync(0xffffffffu, cnt);
-            if ((threadIdx.x & 31) == 0 && tot > 0 && cur_t)
-                atomicAdd(&A.ps[sg / kNumSegs].hash_entries[sg % kNumSegs], (unsigned)tot);
-        } else if (cnt > 0) {
-            atomicAdd(&A.ps[sg / kNumSegs].hash_entries[sg % kNumSegs], (unsigned)cnt);
-        }
-        return;
-    }
-    if (!boundary || A.hash_used[1]) return;
-    if (mode == 1) {
-        if (!cur_t) return;
-        const uint32_t sg = (uint32_t)(kcur >> 36);
-        const uint32_t pair = sg / kNumSegs, cls = sg % kNumSegs;
-        const PairState &ps = A.ps[pair];
-        const int L = ps.n_levels;
-        const uint32_t local = i - ps.seg_start[cls];
-        HashEntry *table = A.hash + ps.hash_base[cls];
-        const uint64_t m = kcur & mmask;
-        const uint32_t x0 = compact12(m), y0 = compact12(m >> 1), z0 = compact12(m >> 2);
-        for (int l = 0; l <= top && l < L; ++l)
-            hash_insert(table, ps.hash_mask[cls], cell_key_lo(x0 >> l, y0 >> l, z0 >> l), cell_key_hi(z0 >> l, l), local);
-    } else {
-        if (!prev_t) return;
-        const uint32_t sg = (uint32_t)(kprev >> 36);
-        const uint32_t pair = sg / kNumSegs, cls = sg % kNumSegs;
-        const PairState &ps = A.ps[pair];
-        const int L = ps.n_levels;
-        const uint32_t local_end = i - ps.seg_start[cls];
-        HashEntry *table = A.hash + ps.hash_base[cls];
-        const uint64_t m = kprev & mmask;
-        const uint32_t x0 = compact12(m), y0 = compact12(m >> 1), z0 = compact12(m >> 2);
-        for (int l = 0; l <= top && l < L; ++l) {
-            const uint32_t x = x0 >> l, y = y0 >> l, z = z0 >> l;
-            HashEntry *e = hash_find(table, ps.hash_mask[cls], cell_key_lo(x, y, z), cell_key_hi(z, l));
-            if (e) e->count = local_end - e->start;
-            if (l + 1 < L) { // tell the parent which of its 8 children exists (child = x bit | y bit << 1 | z bit << 2)
-                HashEntry *par = hash_find(table, ps.hash_mask[cls], cell_key_lo(x >> 1, y >> 1, z >> 1), cell_key_hi(z >> 1, l + 1));
-                if (par) atomicOr(&par->key_hi, 1u << (16 + ((x & 1u) | ((y & 1u) << 1) | ((z & 1u) << 2))));
+    if (i >= n_total || A.hash_used[1]) return;
+    const uint64_t kcur = keys[i];
+    const int top = cell_top(keys, i, kcur);
+    if (top < 0) return;
+    const uint32_t sg = (uint32_t)(kcur >> 36);
+    const uint32_t pair = sg / kNumSegs, cls = sg % kNumSegs;
+    const PairState &ps = A.ps[pair];
+    const int L = ps.n_levels;
+    const uint32_t seg_begin = ps.seg_start[cls], seg_end = seg_begin + ps.seg_count[cls];
+    HashEntry *table = A.hash + ps.hash_base[cls];
+    const uint32_t hmask = ps.hash_mask[cls];
+    const uint64_t m = kcur & ((1ull << 36) - 1);
+    const uint32_t x0 = compact12(m), y0 = compact12(m >> 1), z0 = compact12(m >> 2);
+    uint32_t end = cell_end(keys, i, seg_end, kcur, 0);
+    for (int l = 0; l <= top && l < L; ++l) {
+        uint32_t children = 0;
+        if (l > 0) {
+            const int shift = 3 * l;
+            const uint64_t p = kcur >> shift;
+            children = 1u << ((kcur >> (shift - 3)) & 7u);
+            while (end < seg_end) {
+                const uint64_t k = keys[end];
+                if ((k >> shift) != p) break;
+                children |= 1u << ((k >> (shift - 3)) & 7u);
+                end = cell_end(keys, end, seg_end, k >> (shift - 3), shift - 3);
             }
         }
+        const uint32_t x = x0 >> l, y = y0 >> l, z = z0 >> l;
+        hash_insert(table, hmask, cell_key_lo(x, y, z), cell_key_hi(z, l), children, i - seg_begin, end - i);
     }
 }
 

@@ -46,7 +46,7 @@ struct MapRow {
     float4 a, b, c; // x y z 1 | nx ny nz 0 | intensity curvature 0 0
 };
 
-// pcl::transformPointCloudWithNormals (double math, float store), as k_ingest_transform
+// pcl::transformPointCloudWithNormals (double math, float store), as load_input_point (kernels_ingest.cuh)
 __device__ __forceinline__ void map_transform(MapRow &r, const double *t) {
     const double px = r.a.x, py = r.a.y, pz = r.a.z, qx = r.b.x, qy = r.b.y, qz = r.b.z;
     r.a.x = (float)(t[0] * px + t[1] * py + t[2] * pz + t[3]);

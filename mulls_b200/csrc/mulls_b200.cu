@@ -288,8 +288,6 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     if ((e = dev_alloc(ctx, &(ptr), (n))) != cudaSuccess) return fail(#ptr, e)
     ALLOC(in, 3 * cin);
     A.in_aos = in;
-    ALLOC(A.stg_pos, cin);
-    ALLOC(A.stg_nrm, cin);
     ALLOC(A.keys_a, cin);
     ALLOC(A.keys_b, cin);
     ALLOC(A.vals_a, cin);
@@ -308,8 +306,8 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     ALLOC(A.corr_j, cs);
     ALLOC(A.corr_w, cs);
     ALLOC(A.claim, ct);
-    // hash pool: every class table has a power-of-two capacity >= 2x its cells; cells are typically
-    // 2-3 per target point, so 12 entries per point (192 B) leave room for the rounding.
+    // hash pool: every class table has a power-of-two capacity >= 2x its cells; on a 64-beam scan pair the cells of all
+    // levels are about 0.55 per target point, so 12 entries per point (192 B) leave room for kHashSlack and the rounding.
     {
         size_t pool = 12 * ct + 64 * max_pairs * kNumClasses;
         if (pool >= (1ull << 32)) pool = (1ull << 32) - 1;
@@ -734,8 +732,8 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
     ++launches;
     const unsigned n_inc = (unsigned)ctx->h_in_chunks.size();
     if (n_inc) {
-        if (ctx->any_undistort) k_ingest_transform<true><<<n_inc, kIngestBlock, 0, st>>>(A);
-        else k_ingest_transform<false><<<n_inc, kIngestBlock, 0, st>>>(A);
+        if (ctx->any_undistort) k_ingest_bbox<true><<<n_inc, kIngestBlock, 0, st>>>(A);
+        else k_ingest_bbox<false><<<n_inc, kIngestBlock, 0, st>>>(A);
         ++launches;
     }
     if (hook) { // sharded source: the intersection filter needs the bbox over all shards
@@ -750,7 +748,8 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
     k_pair_setup<<<(unsigned)ceil_div(np, 128), 128, 0, st>>>(A, np);
     ++launches;
     if (n_inc) {
-        k_make_keys<<<n_inc, kIngestBlock, 0, st>>>(A);
+        if (ctx->any_undistort) k_make_keys<true><<<n_inc, kIngestBlock, 0, st>>>(A);
+        else k_make_keys<false><<<n_inc, kIngestBlock, 0, st>>>(A);
         ++launches;
         if (ctx->any_keep_less) { // random down-sampling of :2866-2892: radix select of the k-th sampling key
             const unsigned pb = (unsigned)ceil_div(np, 64);
@@ -781,14 +780,13 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
         launches += 2;
     }
     if (n_in) {
-        k_gather<<<(unsigned)ceil_div(n_in, 256), 256, 0, st>>>(A, A.keys_b, A.vals_b, n_in);
-        const unsigned hb = (unsigned)ceil_div((size_t)n_in + 1, 256);
-        k_hash_build<<<hb, 256, 0, st>>>(A, A.keys_b, n_in, 0);
+        const unsigned nb = (unsigned)ceil_div(n_in, 256);
+        if (ctx->any_undistort) k_gather<true><<<nb, 256, 0, st>>>(A, A.keys_b, A.vals_b, n_in);
+        else k_gather<false><<<nb, 256, 0, st>>>(A, A.keys_b, A.vals_b, n_in);
         k_hash_layout<<<1, 32, 0, st>>>(A, np);
         k_hash_clear<<<1184, 256, 0, st>>>(A);
-        k_hash_build<<<hb, 256, 0, st>>>(A, A.keys_b, n_in, 1);
-        k_hash_build<<<hb, 256, 0, st>>>(A, A.keys_b, n_in, 2);
-        launches += 6;
+        k_hash_build<<<nb, 256, 0, st>>>(A, A.keys_b, n_in);
+        launches += 4;
     } else {
         k_hash_layout<<<1, 32, 0, st>>>(A, np);
         ++launches;
