@@ -141,7 +141,7 @@ struct DeviceArrays {
     unsigned *claim;                 // duplicate_check_table (:1760) as an atomicMin table of source indices
     HashEntry *hash;                 // pool; per-class tables are laid out on the device each run
     uint32_t hash_pool_entries;
-    uint32_t *hash_used;             // [0] entries laid out this run, [1] overflow flag
+    uint32_t *hash_used;             // [0] entries laid out this run, [1] overflow flag, [2] pool needed on overflow
     uint32_t *blk_kept;              // per iteration chunk: sources kept by the block
     double *partials;                // per iteration chunk: kTerms doubles
     double *post_partials;           // per iteration chunk: VTPV, n_obs

@@ -552,6 +552,12 @@ __global__ void __launch_bounds__(256) k_hash_build(DeviceArrays A, const uint64
 // k_hash_layout: single block. Power-of-two table per (pair, class) with load factor <= 0.5, carved out
 // of the pool in order; flags overflow instead of writing out of bounds.
 constexpr uint64_t kHashSlack = 4; // first choice: table capacity >= kHashSlack x cells
+__device__ __forceinline__ uint64_t hash_table_cap(int attempt, uint32_t cells) {
+    const uint64_t want = (attempt == 0) ? kHashSlack * cells : (attempt == 1) ? 2ull * cells : (5ull * cells) / 4 + 1;
+    uint64_t cap = 16;
+    while (cap < want) cap <<= 1;
+    return cap;
+}
 __global__ void k_hash_layout(DeviceArrays A, int n_pairs) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
     // load factor <= 1/kHashSlack if the pool allows it (a miss costs ~1.4 probes instead of 2.5 at 1/2), else
@@ -562,15 +568,13 @@ __global__ void k_hash_layout(DeviceArrays A, int n_pairs) {
         for (int p = 0; p < n_pairs && !overflow; ++p) {
             PairState &ps = A.ps[p];
             for (int c = 0; c < kNumClasses; ++c) {
-                const uint64_t want = (attempt == 0) ? kHashSlack * ps.hash_entries[c] : (attempt == 1) ? 2ull * ps.hash_entries[c] : (5ull * ps.hash_entries[c]) / 4 + 1;
-                uint32_t cap = 16;
-                while (cap < want) cap <<= 1;
+                const uint64_t cap = hash_table_cap(attempt, ps.hash_entries[c]);
                 if (used + cap > A.hash_pool_entries) {
                     overflow = true;
                     break;
                 }
                 ps.hash_base[c] = (uint32_t)used;
-                ps.hash_mask[c] = cap - 1;
+                ps.hash_mask[c] = (uint32_t)(cap - 1);
                 used += cap;
             }
         }
@@ -578,12 +582,25 @@ __global__ void k_hash_layout(DeviceArrays A, int n_pairs) {
         A.hash_used[1] = overflow ? 1u : 0u;
         if (!overflow) return;
     }
-    // overflow: degenerate tables that are never searched (every kernel checks hash_used[1]); the run reports it
-    for (int p = 0; p < n_pairs; ++p)
+    // overflow: [2] = the pool the last attempt needs (saturated), from which the host grows the pool and runs the call
+    // again; [0] stays 0 (k_hash_clear clears nothing). The tables are degenerate and never searched (the searches check
+    // hash_used[1]), and every pair stops here: the iteration phases after the search would otherwise read neighbour
+    // indices that no search of this run has written.
+    uint64_t need = 0;
+    for (int p = 0; p < n_pairs; ++p) {
+        PairState &ps = A.ps[p];
         for (int c = 0; c < kNumClasses; ++c) {
-            A.ps[p].hash_base[c] = 0;
-            A.ps[p].hash_mask[c] = 0;
+            need += hash_table_cap(2, ps.hash_entries[c]);
+            ps.hash_base[c] = 0;
+            ps.hash_mask[c] = 0;
         }
+        if (ps.status == kRunning) {
+            ps.status = kDone;
+            *A.h_running = atomicSub(A.running, 1) - 1;
+        }
+    }
+    __threadfence_system();
+    A.hash_used[2] = need < 0xffffffffull ? (uint32_t)need : 0xffffffffu;
 }
 
 __global__ void __launch_bounds__(256) k_hash_clear(DeviceArrays A) {

@@ -213,7 +213,45 @@ __global__ void __launch_bounds__(kPcaWarps * 32) k_pca(DeviceArrays A, PcaArgs 
                 if (cl < kk) v = trial;
             }
             T = v;
-            // rebuild the list with everything up to and including T (at most kk-1 below + the ties)
+            // Everything below T and every tie at T fit the list: the tie rule below picks among all the ties. Else the
+            // list keeps the ties to take only — those with the lowest ORIGINAL indices among ALL the ties in the cells,
+            // not among the ones a capped list would happen to hold: lim = the need-th smallest index of a tie, by
+            // bisection on the original index.
+            int n_below = 0, n_at = 0;
+            for (int c = 0; c < 27; ++c) {
+                const uint32_t start = __shfl_sync(0xffffffffu, my_start, c), count = __shfl_sync(0xffffffffu, my_count, c);
+                for (uint32_t t = lane; t < count; t += 32) {
+                    const float4 q = __ldg(&pos[start + t]);
+                    const float d2 = flann_l2(p.x, p.y, p.z, q.x, q.y, q.z);
+                    n_below += (d2 < rb2 && __float_as_uint(d2) < T) ? 1 : 0;
+                    n_at += (d2 < rb2 && __float_as_uint(d2) == T) ? 1 : 0;
+                }
+            }
+            for (int o = 16; o > 0; o >>= 1) {
+                n_below += __shfl_xor_sync(0xffffffffu, n_below, o);
+                n_at += __shfl_xor_sync(0xffffffffu, n_at, o);
+            }
+            const int need = kk - n_below; // >= 1: count(key < T) < kk <= count(key <= T)
+            uint32_t lim = 0xffffffffu;    // all ties
+            if (n_below + n_at > kPcaCap) {
+                lim = 0;
+                for (int bit = 30; bit >= 0; --bit) {
+                    const uint32_t trial = lim | (1u << bit);
+                    int cl = 0;
+                    for (int c = 0; c < 27; ++c) {
+                        const uint32_t start = __shfl_sync(0xffffffffu, my_start, c), count = __shfl_sync(0xffffffffu, my_count, c);
+                        for (uint32_t t = lane; t < count; t += 32) {
+                            const float4 q = __ldg(&pos[start + t]);
+                            const float d2 = flann_l2(p.x, p.y, p.z, q.x, q.y, q.z);
+                            cl += (d2 < rb2 && __float_as_uint(d2) == T &&
+                                   (uint32_t)__float_as_int(__ldg(&nrm[start + t]).w) < trial) ? 1 : 0;
+                        }
+                    }
+                    for (int o = 16; o > 0; o >>= 1) cl += __shfl_xor_sync(0xffffffffu, cl, o);
+                    if (cl < need) lim = trial;
+                }
+            }
+            // rebuild the list: the n_below entries below T and the ties up to lim (all of them, or the `need` to take)
             int mt = 0;
             for (int c = 0; c < 27; ++c) {
                 const uint32_t start = __shfl_sync(0xffffffffu, my_start, c), count = __shfl_sync(0xffffffffu, my_count, c);
@@ -224,7 +262,8 @@ __global__ void __launch_bounds__(kPcaWarps * 32) k_pca(DeviceArrays A, PcaArgs 
                     if (base + lane < count) {
                         const float4 q = __ldg(&pos[j]);
                         d2 = flann_l2(p.x, p.y, p.z, q.x, q.y, q.z);
-                        in = d2 < rb2 && __float_as_uint(d2) <= T;
+                        in = d2 < rb2 && (__float_as_uint(d2) < T || (__float_as_uint(d2) == T &&
+                                                                      (uint32_t)__float_as_int(__ldg(&nrm[j]).w) <= lim));
                     }
                     const unsigned b = __ballot_sync(0xffffffffu, in);
                     const int off = mt + __popc(b & ((1u << lane) - 1u));

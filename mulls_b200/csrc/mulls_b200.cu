@@ -92,7 +92,7 @@ struct mulls_ctx {
     size_t cub_temp_bytes = 0;
     mulls_icp_result *d_results = nullptr;
     mulls_icp_result *h_results = nullptr; // pinned
-    uint32_t *h_flags = nullptr;           // pinned copy of hash_used
+    uint32_t *h_flags = nullptr;           // pinned copy of hash_used (3 words)
     int *h_running = nullptr;              // mapped pinned: pairs still iterating
     std::vector<cudaEvent_t> ev_done;      // one per iteration (launch-loop flow control)
     mulls_icp_trace *d_trace = nullptr;
@@ -140,6 +140,9 @@ struct mulls_ctx {
         uint64_t launches = 0;
         int n_search_ev = 0;
         bool graphed = false, hooked = false, active = false;
+        mulls_icp_trace *trace = nullptr; // what run_finish needs to run the call again after growing the hash pool
+        mulls_allreduce_fn hook = nullptr;
+        void *user = nullptr;
     } pend;
     // device scratch, grown on demand (grow_scratch)
     Scratch pca_buf;             // PCA
@@ -306,15 +309,18 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     ALLOC(A.corr_j, cs);
     ALLOC(A.corr_w, cs);
     ALLOC(A.claim, ct);
-    // hash pool: every class table has a power-of-two capacity >= 2x its cells; on a 64-beam scan pair the cells of all
-    // levels are about 0.55 per target point, so 12 entries per point (192 B) leave room for kHashSlack and the rounding.
+    // hash pool: every class table has a power-of-two capacity of 1.25x to 8x its cells (k_hash_layout). On a 64-beam
+    // scan pair the cells of all levels are about 0.55 per target point, so 12 entries per point (192 B) leave room for
+    // kHashSlack and the rounding. That is a first size, not a bound: a point opens up to one cell per level (12), and
+    // sparse clouds come close to it (about 7 cells per point for 20 000 points spread over a 500 m cube). When the
+    // target clouds of a call need more, the pool grows to what they need and the call runs again (grow_hash_pool).
     {
         size_t pool = 12 * ct + 64 * max_pairs * kNumClasses;
         if (pool >= (1ull << 32)) pool = (1ull << 32) - 1;
         A.hash_pool_entries = (uint32_t)pool;
         ALLOC(A.hash, pool);
     }
-    ALLOC(A.hash_used, 2);
+    ALLOC(A.hash_used, 3);
     ALLOC(A.ctl, 1);
     ALLOC(A.blk_kept, ctx->cap_it_chunks);
     ALLOC(A.partials, ctx->cap_it_chunks * kTerms);
@@ -349,7 +355,7 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     A.trace = ctx->d_trace; // written only when LoopCtl::trace_on is set for the run
     if ((e = cudaMallocHost((void **)&ctx->h_results, max_pairs * (sizeof(mulls_icp_result) + sizeof(uint64_t)))) != cudaSuccess)
         return fail("pinned results", e);
-    if ((e = cudaMallocHost((void **)&ctx->h_flags, 2 * sizeof(uint32_t))) != cudaSuccess) return fail("pinned flags", e);
+    if ((e = cudaMallocHost((void **)&ctx->h_flags, 3 * sizeof(uint32_t))) != cudaSuccess) return fail("pinned flags", e);
     if ((e = cudaMallocHost((void **)&ctx->h_ctl, sizeof(LoopCtl))) != cudaSuccess) return fail("pinned control block", e);
     // radix-sort temp storage for the largest possible sort
     {
@@ -857,6 +863,31 @@ static int build_iteration_graph(mulls_ctx *ctx) {
     return MULLS_OK;
 }
 
+// After a run whose grid did not fit the hash pool (h_flags copied back, stream synchronised): grows the pool to the
+// entries k_hash_layout found the target clouds need, so that the same inputs fit when they run again. The iteration
+// graph has the old pool's address baked into its kernel nodes: it is dropped, and recorded anew by its next use.
+static int grow_hash_pool(mulls_ctx *ctx) {
+    const uint32_t need = ctx->h_flags[2];
+    DeviceArrays &A = ctx->A;
+    if (need <= A.hash_pool_entries || need == 0xffffffffu) {
+        ctx->err = "hash pool exhausted (the target clouds need " + std::to_string(need) + " grid entries)";
+        return MULLS_E_CAPACITY;
+    }
+    HashEntry *fresh = nullptr;
+    if (cudaMalloc(&fresh, (size_t)need * sizeof(HashEntry)) != cudaSuccess) {
+        cudaGetLastError();
+        ctx->err = "hash pool exhausted, and no device memory to grow it to " + std::to_string(need) + " entries";
+        return MULLS_E_CAPACITY;
+    }
+    std::replace(ctx->allocs.begin(), ctx->allocs.end(), (void *)A.hash, (void *)fresh);
+    CK(cudaFree(A.hash));
+    A.hash = fresh;
+    A.hash_pool_entries = need;
+    if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec), ctx->graph_exec = nullptr;
+    if (ctx->graph) cudaGraphDestroy(ctx->graph), ctx->graph = nullptr;
+    return MULLS_OK;
+}
+
 // Launch the whole path on the resident inputs. If `hook` is given (sharded mode) it is called between
 // the phases that need a cross-rank exchange.
 static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace *trace, mulls_allreduce_fn hook, void *user,
@@ -1007,10 +1038,11 @@ static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace
         ++launches;
     }
     CK(cudaMemcpyAsync(ctx->h_results, ctx->d_results, np * (sizeof(mulls_icp_result) + sizeof(uint64_t)), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     if (trace) CK(cudaMemcpyAsync(trace, ctx->d_trace, np * sizeof(mulls_icp_trace), cudaMemcpyDeviceToHost, st));
     CK(cudaEventRecord(ctx->ev_end, st));
     ctx->pend.launches = launches, ctx->pend.n_search_ev = n_search_ev, ctx->pend.graphed = graphed, ctx->pend.hooked = hook != nullptr;
+    ctx->pend.trace = trace, ctx->pend.hook = hook, ctx->pend.user = user;
     ctx->pend.active = true;
     if (!finish_now) return MULLS_OK;
     return run_finish_inner(ctx, out);
@@ -1029,8 +1061,12 @@ static int run_finish_inner(mulls_ctx *ctx, mulls_icp_result *out) {
     // (graph: three k_search forms, k_resolve, k_accumulate, k_solve per executed iteration + posterior, finalize, collect)
     if (graphed) launches += (uint64_t)ctx->h_ctl->it * (6u + (ctx->any_normal_shooting ? 1u : 0u)) + 3u;
     if (ctx->h_flags[1]) {
-        ctx->err = "hash pool exhausted (target clouds produce more grid cells than the context reserves)";
-        return MULLS_E_CAPACITY;
+        // the grid did not fit (k_hash_layout stopped every pair): grow the pool and run the call again on the inputs
+        // still in HBM. The grown pool holds the layout's last attempt by construction, so this happens at most once. A
+        // sharded run grows on every rank alike: the target clouds, and so their grids, are the same on all of them.
+        const int rc = grow_hash_pool(ctx);
+        if (rc != MULLS_OK) return rc;
+        return run_impl_inner(ctx, out, ctx->pend.trace, ctx->pend.hook, ctx->pend.user, true);
     }
     if (out) std::memcpy(out, ctx->h_results, np * sizeof(mulls_icp_result));
     // statistics
@@ -1259,6 +1295,15 @@ static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_d
     A.trace = nullptr;
     rc = launch_ingest(ctx, A, false, launches);
     if (rc != MULLS_OK) return rc;
+    // the grid must fit the hash pool before k_pca reads it: else grow the pool and build the grid again from the
+    // cloud already in HBM (it fits by construction)
+    CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (ctx->h_flags[1]) {
+        if ((rc = grow_hash_pool(ctx)) != MULLS_OK) return rc;
+        A.hash = ctx->A.hash, A.hash_pool_entries = ctx->A.hash_pool_entries;
+        if ((rc = launch_ingest(ctx, A, false, launches)) != MULLS_OK) return rc;
+    }
     args.radius = radius;
     args.r2 = (float)((double)radius * (double)radius);
     args.k = k;
@@ -1273,7 +1318,6 @@ static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_d
         k_pca<<<(unsigned)ceil_div(n, kPcaWarps), kPcaWarps * 32, 0, st>>>(A, args);
         ++launches;
     }
-    CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     ctx->uploaded = false; // the resident batch was replaced by the PCA cloud
     return MULLS_OK;
 }
@@ -1305,10 +1349,6 @@ int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int
     }
     CK(cudaStreamSynchronize(st));
     CK(cudaGetLastError());
-    if (ctx->h_flags[1]) {
-        ctx->err = "hash pool exhausted";
-        return MULLS_E_CAPACITY;
-    }
     ctx->stats = mulls_run_stats();
     ctx->stats.kernel_launches = launches;
     return MULLS_OK;
@@ -1637,10 +1677,6 @@ int mulls_map_update(mulls_map *m, const mulls_cloud_view scan_down[MULLS_NUM_CL
             CK(cudaEventRecord(m->ev1, st));
             CK(cudaStreamSynchronize(st));
             CK(cudaGetLastError());
-            if (ctx->h_flags[1]) {
-                ctx->err = "hash pool exhausted";
-                return MULLS_E_CAPACITY;
-            }
             for (int k = 0; k < 2; ++k) m->n[cls[k]] = m->h_state->n_out[cls[k]];
             cudaEventElapsedTime(&m->last.ms_update, m->ev0, m->ev1);
         }
@@ -1821,10 +1857,6 @@ int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mull
     }
     CK(cudaStreamSynchronize(st));
     CK(cudaGetLastError());
-    if (n > 0 && ctx->h_flags[1]) {
-        ctx->err = "hash pool exhausted";
-        return MULLS_E_CAPACITY;
-    }
     // results
     const float4 *src[MULLS_OUT_COUNT];
     size_t cnt[MULLS_OUT_COUNT];

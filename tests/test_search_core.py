@@ -250,3 +250,61 @@ def test_single_dense_spot_with_a_stack_too_small_to_split_it(lib):
         idx, d2, cert = run(lib, tgt, q, 3.5, leaf=leaf, want_cert=True)
         check(idx, d2, bi, bd, 3.5)
         assert np.all(cert.astype(np.float64) <= second_nearest_sq(tgt, q, idx) * (1 + 1e-5) + 1e-9)
+
+
+def cell_size_for(tgt_xyz):
+    """k_pair_setup: the level-0 cell doubles from 0.125 m until 4092 cells span the extent of the targets"""
+    ext = float((tgt_xyz.max(0).astype(np.float64) - tgt_xyz.min(0).astype(np.float64)).max())
+    h0 = 0.125
+    while (ext + 8 * h0) * 1.001 > h0 * 4092:
+        h0 *= 2
+    return h0
+
+
+@pytest.mark.parametrize("ext", [509.0, 511.0, 20000.0])
+def test_grid_extents_around_the_cell_doubling(lib, ext):
+    """extents just below and above the first doubling of the level-0 cell, and one of 20 km, with points in the
+    extreme cells of the grid"""
+    rng = np.random.default_rng(int(ext))
+    corners = np.array([[x, y, z] for x in (0, ext) for y in (0, ext) for z in (0, ext)], np.float32)
+    clusters = np.clip((corners[:, None, :] + rng.uniform(-1, 1, (8, 50, 3)) * 0.8).reshape(-1, 3), 0, ext)
+    tgt = np.concatenate([rng.uniform(0, ext, (6000, 3)), corners, clusters]).astype(np.float32)
+    h0 = cell_size_for(tgt)
+    assert h0 == {509.0: 0.125, 511.0: 0.25, 20000.0: 8.0}[ext]
+    q = np.concatenate([tgt[rng.integers(0, len(tgt), 500)] + rng.normal(0, 0.3, (500, 3)),
+                        corners + rng.normal(0, 1.0, corners.shape), clusters[::5] + 0.3,
+                        rng.uniform(-10, ext + 10, (300, 3))]).astype(np.float32)
+    bi, bd = brute(tgt, q)
+    for leaf in (32, 4):
+        for mode in (0, 1):
+            idx, d2 = run(lib, tgt, q, 3.5, leaf=leaf, h0=h0, mode=mode)
+            check(idx, d2, bi, bd, 3.5)
+
+
+@pytest.mark.parametrize("cloud", ["lattice", "duplicates", "dense_spot"])
+def test_clouds_far_from_the_origin(lib, cloud):
+    """boundary lattice, exact duplicates and a dense spot moved to (+6 km, -3 km, +40 m): cell boundaries o + x*h stay
+    exact there, and so do the answers"""
+    rng = np.random.default_rng(31)
+    if cloud == "lattice":
+        ax = np.arange(24, dtype=np.float32) * np.float32(0.0625)
+        g = np.stack(np.meshgrid(ax, ax, ax[:6], indexing="ij"), -1).reshape(-1, 3)
+        tgt = g[rng.permutation(len(g))]
+        q = np.concatenate([tgt[:300], tgt[300:600] + np.float32(0.03125),
+                            (rng.integers(-8, 40, (300, 3)) * np.float32(0.125)).astype(np.float32)])
+    elif cloud == "duplicates":
+        base = rng.uniform(-8, 8, (2000, 3)).astype(np.float32)
+        tgt = np.tile(base, (3, 1))[rng.permutation(6000)]
+        q = np.concatenate([base[:300], base[300:900] + rng.normal(0, 0.2, (600, 3)).astype(np.float32)])
+    else:
+        tgt = np.concatenate([rng.uniform(0, 0.1, (5000, 3)) + 1.0, rng.uniform(-3, 5, (2000, 3))]).astype(np.float32)
+        q = np.concatenate([tgt[::50] + np.float32(0.001), rng.uniform(-4, 6, (300, 3))]).astype(np.float32)
+    off = np.array([6000.0, -3000.0, 40.0])
+    tgt = (tgt + off).astype(np.float32)
+    q = (q + off).astype(np.float32)
+    bi, bd = brute(tgt, q)
+    for radius in (3.5, 0.2):
+        for leaf in (32, 2):
+            for mode in (0, 1):
+                idx, d2 = run(lib, tgt, q, radius, leaf=leaf, mode=mode)
+                check(idx, d2, bi, bd, radius)
