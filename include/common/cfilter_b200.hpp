@@ -1,5 +1,5 @@
 // Drop-in shims: lo::CFilter<PointT>::classify_nground_pts (include/common/cfilter.hpp:2058-2290), fast_ground_filter
-// (:1658-2036) and voxel_downsample (:83-165) over the mulls_b200 C-ABI. A MULLS maintainer replaces the BODY of classify_nground_pts by
+// (:1658-2036), voxel_downsample (:83-165) and sor_filter (:203-247) over the mulls_b200 C-ABI. A MULLS maintainer replaces the BODY of classify_nground_pts by
 //
 //     return lo::b200::classify_nground_pts<PointT>(cloud_in, cloud_pillar, ... );      // all arguments forwarded
 //
@@ -11,6 +11,7 @@
 #define MULLS_B200_CFILTER_SHIM_HPP
 
 #include <cfloat>
+#include <cstdint>
 #include <vector>
 
 #include "common/cregistration_b200.hpp" // thread_context, view_of
@@ -163,6 +164,35 @@ bool voxel_downsample(const typename pcl::PointCloud<PointT>::Ptr &cloud_in, typ
     }
     cloud_out->points.insert(cloud_out->points.end(), rows.begin(), rows.begin() + n_out);
     return true;
+}
+
+// lo::CFilter<PointT>::sor_filter (include/common/cfilter.hpp:203-222): pcl::StatisticalOutlierRemoval with mean_k and
+// n_std (mulls_sor_filter). cloud_out's points become the kept rows of cloud_in, all 48 bytes of each, in input order —
+// what PCL's filter() copies; cloud_out may be cloud_in. Returns false (cloud_out untouched) when the call is refused:
+// at most mean_k finite points, mean_k outside 1..63, no device.
+template <typename PointT>
+bool sor_filter(typename pcl::PointCloud<PointT>::Ptr &cloud_in, typename pcl::PointCloud<PointT>::Ptr &cloud_out, int mean_k,
+                double n_std) {
+    static_assert(sizeof(PointT) == 48, "the C-ABI consumes pcl::PointXYZINormal rows (48 bytes)");
+    const size_t n = cloud_in->points.size();
+    mulls_ctx *ctx = thread_context(1, n);
+    std::vector<uint8_t> keep((n + 7) / 8 + 1, 0);
+    if (!ctx || mulls_sor_filter(ctx, view_of<PointT>(cloud_in), mean_k, n_std, keep.data(), nullptr, nullptr) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return false;
+    }
+    std::vector<PointT> kept;
+    kept.reserve(n);
+    for (size_t i = 0; i < n; ++i)
+        if ((keep[i >> 3] >> (i & 7)) & 1u) kept.push_back(cloud_in->points[i]);
+    cloud_out->points.swap(kept);
+    return true;
+}
+
+// lo::CFilter<PointT>::sor_filter, the in-place overload (include/common/cfilter.hpp:224-247)
+template <typename PointT>
+bool sor_filter(typename pcl::PointCloud<PointT>::Ptr &cloud_in_out, int mean_k, double n_std) {
+    return sor_filter<PointT>(cloud_in_out, cloud_in_out, mean_k, n_std);
 }
 
 // lo::CFilter<PointT>::extract_semantic_pts (include/common/cfilter.hpp:2295-2413): same names, order, types and

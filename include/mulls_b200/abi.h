@@ -30,6 +30,7 @@
  *   mulls_fast_ground_filter <- lo::CFilter<PointT>::fast_ground_filter, include/common/cfilter.hpp:1658-2036
  *   mulls_voxel_downsample   <- lo::CFilter<PointT>::voxel_downsample, include/common/cfilter.hpp:83-165
  *   mulls_extract_semantic_pts <- lo::CFilter<PointT>::extract_semantic_pts, include/common/cfilter.hpp:2295-2413
+ *   mulls_sor_filter         <- lo::CFilter<PointT>::sor_filter, include/common/cfilter.hpp:203-247
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
  *
@@ -437,6 +438,29 @@ typedef struct mulls_extract_out {
 
 int mulls_extract_semantic_pts(mulls_ctx *ctx, mulls_cloud_view pc_raw, const mulls_extract_params *params,
                                mulls_extract_out *out);
+
+/* lo::CFilter<PointT>::sor_filter, include/common/cfilter.hpp:203-247 (both overloads; test/mulls_slam.cpp:1008-1009 runs it
+ * with mean_k 20, n_std 2.0 on the merged map): pcl::StatisticalOutlierRemoval, PCL 1.10 applyFilterIndices (SURVEY
+ * Appendix B item 10). For every point with finite x, y, z: the mean of the square roots of the squared (FLANN float)
+ * distances to its mean_k nearest other points, summed in double in ascending order, stored as float (mean_dist[i]; 0 for
+ * the other points). Then, in input order and in double, sum and sum of squares (the float square widened), mean =
+ * sum / n_valid, stddev = sqrt((sq_sum - sum * sum / n_valid) / (n_valid - 1)), threshold = mean + n_std * stddev, and
+ * point i is kept iff NOT (mean_dist[i] > threshold) — a NaN threshold keeps every point. keep_bits: bit i % 8 of byte
+ * i / 8 (LSB first) set for a kept point; stats->n_kept counts them. Kept rows are meant to be gathered in input order.
+ * Defined where the reference is not:
+ *   - points with a non-finite coordinate never enter the neighbour search (PCL would hand them to FLANN, as the merged
+ *     map claims is_dense); they get distance 0 and count towards neither n_valid nor the neighbours of others
+ *   - at most mean_k finite points: MULLS_E_ARG (PCL would read past its neighbour vector)
+ *   - mean_k < 1 or mean_k > 63: MULLS_E_ARG
+ * A cloud of more than the context's max_tgt_pts points: MULLS_E_CAPACITY. The call replaces the batch resident on the
+ * context (as mulls_pca_features does). */
+typedef struct mulls_sor_stats {
+    double mean, stddev, threshold;
+    uint64_t n_valid, n_kept;
+} mulls_sor_stats;
+int mulls_sor_filter(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double n_std,
+                     uint8_t *keep_bits /* [(n+7)/8] */, float *mean_dist /* [n] or NULL */,
+                     mulls_sor_stats *stats /* or NULL */);
 
 /* The wire format the library ships host clouds in when the "host_pack" tunable is on (csrc/host_pack.h): the 28 of the
  * 48 bytes of a pcl::PointXYZINormal row (utility.hpp:40) that the path reads, repacked on the host cores into pinned

@@ -104,6 +104,17 @@ class PcaOut(C.Structure):
     ]
 
 
+class SorStats(C.Structure):
+    """mulls_sor_stats: what pcl::StatisticalOutlierRemoval computed (mean, stddev, threshold) and the point counts."""
+    _fields_ = [
+        ("mean", C.c_double),
+        ("stddev", C.c_double),
+        ("threshold", C.c_double),
+        ("n_valid", C.c_uint64),
+        ("n_kept", C.c_uint64),
+    ]
+
+
 class MapParams(C.Structure):
     """mulls_map_params: the arguments of MapManager::update_local_map (include/pgo/map_manager.h:22-32)."""
     _fields_ = [
@@ -270,6 +281,7 @@ EXPORTED_SYMBOLS = (
     "mulls_fast_ground_filter",
     "mulls_voxel_downsample",
     "mulls_extract_semantic_pts",
+    "mulls_sor_filter",
     "mulls_scan_probe",
     "mulls_scan_read",
     "mulls_pose_write",
@@ -334,6 +346,9 @@ def load_library() -> C.CDLL:
     lib.mulls_voxel_downsample.argtypes = [vp, CloudView, C.c_float, C.POINTER(C.c_float), C.c_size_t, C.POINTER(C.c_size_t)]
     lib.mulls_extract_semantic_pts.restype = C.c_int
     lib.mulls_extract_semantic_pts.argtypes = [vp, CloudView, C.POINTER(ExtractParams), C.POINTER(ExtractOut)]
+    lib.mulls_sor_filter.restype = C.c_int
+    lib.mulls_sor_filter.argtypes = [vp, CloudView, C.c_int, C.c_double, C.POINTER(C.c_uint8), C.POINTER(C.c_float),
+                                     C.POINTER(SorStats)]
     lib.mulls_pack_rows.restype = C.c_int
     lib.mulls_pack_rows.argtypes = [C.POINTER(C.c_float), C.c_size_t, C.c_int, C.POINTER(C.c_float)]
     lib.mulls_scan_probe.restype = C.c_int

@@ -100,9 +100,14 @@ __device__ __forceinline__ void load_input_point(const PairConst &pc, uint32_t s
     if (kNormals) nrm = make_float4(nx, ny, nz, __int_as_float((int)local));
 }
 
+// a point whose three coordinates are finite: kFiniteOnly ingests (mulls_sor_filter) leave every other point out of the
+// grid's extent and out of the grid
+__device__ __forceinline__ bool finite_xyz(const float4 &p) { return isfinite(p.x) && isfinite(p.y) && isfinite(p.z); }
+
 // ---- k_ingest_bbox: bbox reductions for the intersection filter: source ground/pillar/facade
 //      (cregistration.hpp:2912-2915) and all target points (grid extent). Reads positions only, writes nothing per point.
-template <bool kUndistort>
+// kFiniteOnly: points with a non-finite coordinate do not enter the box (an infinite extent has no grid).
+template <bool kUndistort, bool kFiniteOnly = false>
 __global__ void __launch_bounds__(kIngestBlock) k_ingest_bbox(DeviceArrays A) {
     const ChunkDesc cd = A.in_chunks[blockIdx.x];
     const PairConst &pc = A.pc[cd.pair];
@@ -112,9 +117,10 @@ __global__ void __launch_bounds__(kIngestBlock) k_ingest_bbox(DeviceArrays A) {
     const bool want = is_src ? (cls == MULLS_GROUND || cls == MULLS_PILLAR || cls == MULLS_FACADE) : true;
     if (!want) return; // block-uniform
     const uint32_t local = cd.first + threadIdx.x;
-    const bool valid = local < pc.in_n[seg];
+    bool valid = local < pc.in_n[seg];
     float4 p = make_float4(0.f, 0.f, 0.f, 0.f), unused;
     if (valid) load_input_point<kUndistort, false>(pc, seg, local, p, unused);
+    if (kFiniteOnly) valid = valid && finite_xyz(p);
     float mn[3] = {valid ? p.x : FLT_MAX, valid ? p.y : FLT_MAX, valid ? p.z : FLT_MAX};
     float mx[3] = {valid ? p.x : -FLT_MAX, valid ? p.y : -FLT_MAX, valid ? p.z : -FLT_MAX};
 #pragma unroll
@@ -227,7 +233,8 @@ __global__ void k_pair_setup(DeviceArrays A, int n_pairs) {
 
 // ---- k_make_keys: intersection filter (cfilter.hpp:950-981: strictly inside) + 64-bit sort key
 //      [pair*12+seg | morton36(cell)]; filtered-out points sort to the very end.
-template <bool kUndistort>
+// kFiniteOnly: points with a non-finite coordinate are filtered out as well.
+template <bool kUndistort, bool kFiniteOnly = false>
 __global__ void __launch_bounds__(kIngestBlock) k_make_keys(DeviceArrays A) {
     const ChunkDesc cd = A.in_chunks[blockIdx.x];
     const PairConst &pc = A.pc[cd.pair];
@@ -243,6 +250,7 @@ __global__ void __launch_bounds__(kIngestBlock) k_make_keys(DeviceArrays A) {
         const double *b = ps.ibb;
         inside = (double)p.x > b[0] && (double)p.x < b[3] && (double)p.y > b[1] && (double)p.y < b[4] &&
                  (double)p.z > b[2] && (double)p.z < b[5];
+        if (kFiniteOnly) inside = inside && finite_xyz(p);
         uint64_t key = ~0ull;
         if (inside) {
             const int hi = (1 << kCoordBits) - 1;

@@ -94,110 +94,12 @@ __device__ __forceinline__ GridView grid_of(const DeviceArrays &A, const PairCon
     return g;
 }
 
-// squared distance from p to the (slightly inflated) box of cell (x,y,z) at a level with cell size hl
-__device__ __forceinline__ float cell_dist2(const GridView &g, float px, float py, float pz, float hl, int x, int y,
-                                            int z, float margin) {
-    const float ax = slab_dist(g.ox + (float)x * hl, g.ox + (float)(x + 1) * hl, px, margin);
-    const float ay = slab_dist(g.oy + (float)y * hl, g.oy + (float)(y + 1) * hl, py, margin);
-    const float az = slab_dist(g.oz + (float)z * hl, g.oz + (float)(z + 1) * hl, pz, margin);
-    return ax * ax + ay * ay + az * az;
-}
-
 // ------------------------------------------------------------------------------------------------
 // exact k nearest targets (k = 10) for the normal-shooting correspondences of :1732-1737
-// (pcl::registration::CorrespondenceEstimationNormalShooting): same hierarchy as nn_search, the pruning bound is
-// the current k-th best distance and there is no search radius — the level pyramid of a pair that uses normal
-// shooting goes up to a block that spans the whole grid, so the result is exact however far the targets are.
-// Total order (d2, original index). A rarely used option: plain per-thread DFS with its stack in local memory,
-// kept out of k_search (own kernel, k_search_shoot).
+// (pcl::registration::CorrespondenceEstimationNormalShooting): knn_search (search_core.cuh) with a list of 10. A rarely
+// used option, kept out of k_search (own kernel, k_search_shoot).
 // ------------------------------------------------------------------------------------------------
 constexpr int kShootK = 10;
-constexpr int kShootStack = 48; // DFS entries: at most 7 stay behind per descended level
-
-struct KnnList {
-    float d2[kShootK];
-    int j[kShootK];
-    int n;
-};
-__device__ __forceinline__ float knn_bound(const KnnList &kl) { return kl.n < kShootK ? INFINITY : kl.d2[kShootK - 1]; }
-
-__device__ __forceinline__ void knn_insert(const GridView &g, KnnList &kl, float d2, int j) {
-    if (kl.n == kShootK) {
-        const float w = kl.d2[kShootK - 1];
-        if (d2 > w) return;
-        if (d2 == w && __float_as_int(__ldg(&g.nrm[j]).w) >= __float_as_int(__ldg(&g.nrm[kl.j[kShootK - 1]]).w)) return;
-    }
-    for (int i = 0; i < kl.n; ++i)
-        if (kl.j[i] == j) return; // a point is met again when the search ascends a level
-    int pos = (kl.n < kShootK) ? kl.n : kShootK - 1;
-    while (pos > 0) {
-        const float dp = kl.d2[pos - 1];
-        bool before = d2 < dp;
-        if (d2 == dp) before = __float_as_int(__ldg(&g.nrm[j]).w) < __float_as_int(__ldg(&g.nrm[kl.j[pos - 1]]).w);
-        if (!before) break;
-        kl.d2[pos] = kl.d2[pos - 1];
-        kl.j[pos] = kl.j[pos - 1];
-        --pos;
-    }
-    kl.d2[pos] = d2;
-    kl.j[pos] = j;
-    if (kl.n < kShootK) ++kl.n;
-}
-
-__device__ __forceinline__ void knn_search(const GridView &g, float px, float py, float pz, int start_level, KnnList &kl) {
-    kl.n = 0;
-    const int c0x = (int)floorf((px - g.ox) * g.inv_h0);
-    const int c0y = (int)floorf((py - g.oy) * g.inv_h0);
-    const int c0z = (int)floorf((pz - g.oz) * g.inv_h0);
-    const int L = g.n_levels;
-    const float margin = 1e-3f * g.h0;
-    uint2 st_cell[kShootStack]; // pack_cell(x, y, z, level, 0)
-    float st_d2[kShootStack];
-    for (int l = min(max(start_level, 1), L - 1);; ++l) {
-        const float H = g.h0 * (float)(1 << l);
-        const int ncell = (1 << kCoordBits) >> l;
-        for (int k = 0; k < 8; ++k) { // own cell first, then the half-side neighbours
-            int x = (c0x >> l) + ((k & 1) ? ((((c0x >> (l - 1)) & 1) ? 1 : -1)) : 0);
-            int y = (c0y >> l) + ((k & 2) ? ((((c0y >> (l - 1)) & 1) ? 1 : -1)) : 0);
-            int z = (c0z >> l) + ((k & 4) ? ((((c0z >> (l - 1)) & 1) ? 1 : -1)) : 0);
-            if (ncell == 2) x = k & 1, y = (k >> 1) & 1, z = k >> 2; // top of the full pyramid: the 8 cells ARE the grid
-            if (x < 0 || y < 0 || z < 0 || x >= ncell || y >= ncell || z >= ncell) continue;
-            int sp = 0;
-            st_cell[0] = pack_cell((uint32_t)x, (uint32_t)y, (uint32_t)z, l, 0u);
-            st_d2[0] = cell_dist2(g, px, py, pz, H, x, y, z, margin);
-            sp = 1;
-            while (sp > 0) {
-                --sp;
-                if (st_d2[sp] > knn_bound(kl) * 1.0001f + 1e-12f) continue;
-                const uint2 ce = st_cell[sp];
-                const int lv = (int)((ce.y >> 4) & 0xfu);
-                const int cx = (int)(ce.x & 0xfffu), cy = (int)((ce.x >> 12) & 0xfffu), cz = (int)((ce.x >> 24) | ((ce.y & 0xfu) << 8));
-                uint32_t start, count, cmask;
-                if (!probe_cell(g, (uint32_t)cx, (uint32_t)cy, (uint32_t)cz, lv, start, count, cmask)) continue;
-                if (count <= (uint32_t)g.leaf_count || lv == 0 || sp + 8 > kShootStack) {
-                    for (uint32_t jj = start; jj < start + count; ++jj) {
-                        const float4 q = __ldg(&g.pos[jj]);
-                        knn_insert(g, kl, flann_l2(px, py, pz, q.x, q.y, q.z), (int)jj);
-                    }
-                } else {
-                    const float hc = 0.5f * g.h0 * (float)(1 << lv);
-                    for (int ch = 7; ch >= 0; --ch) {
-                        if (!((cmask >> ch) & 1u)) continue;
-                        const int x2 = 2 * cx + (ch & 1), y2 = 2 * cy + ((ch >> 1) & 1), z2 = 2 * cz + (ch >> 2);
-                        const float d2c = cell_dist2(g, px, py, pz, hc, x2, y2, z2, margin);
-                        if (d2c > knn_bound(kl) * 1.0001f + 1e-12f) continue;
-                        st_cell[sp] = pack_cell((uint32_t)x2, (uint32_t)y2, (uint32_t)z2, lv - 1, 0u);
-                        st_d2[sp] = d2c;
-                        ++sp;
-                    }
-                }
-            }
-        }
-        const float cover = 0.999f * 0.5f * H; // every target closer than this has been examined
-        if (kl.n == kShootK && kl.d2[kShootK - 1] <= cover * cover) break;
-        if (l == L - 1) break; // the top block spans the whole grid: everything has been examined
-    }
-}
 
 // ---- k_search ----------------------------------------------------------------------------------
 // what every search kernel does first: cregistration.hpp:1260 — incremental in-place update of the float source
@@ -447,8 +349,8 @@ __device__ __forceinline__ void search_shoot_chunk(DeviceArrays &A, int buf, uin
     const float max_distance_f = 2.5f * ps.thre;
     int sj = -1;
     float sd2 = INFINITY;
-    KnnList kl;
-    knn_search(g, p.x, p.y, p.z, kStartLevel0, kl);
+    KnnList<kShootK> kl;
+    knn_search(g, p.x, p.y, p.z, kStartLevel0, kShootK, kl);
     double min_dist = 1.7976931348623157e308;
     for (int t = 0; t < kl.n; ++t) {
         const float4 q = __ldg(&g.pos[kl.j[t]]);

@@ -25,6 +25,7 @@
 #include "kernels_map.cuh"
 #include "kernels_classify.cuh"
 #include "kernels_ground.cuh"
+#include "kernels_sor.cuh"
 
 using namespace mulls;
 
@@ -149,6 +150,7 @@ struct mulls_ctx {
     Scratch cls_buf;             // classification (mulls_classify_nground)
     Scratch gf_buf, gf_cell_buf; // ground filter (mulls_fast_ground_filter): per-point part and per-cell part
     Scratch vx_buf, ext_buf;     // voxel filter; clouds handed between the stages of extract_semantic_pts
+    Scratch sor_buf;             // statistical outlier filter: mean distances, keep mask, statistics
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
     const mulls_map *tree_map = nullptr;
@@ -229,7 +231,7 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (void *p : ctx->allocs) cudaFree(p);
     if (ctx->cub_temp) cudaFree(ctx->cub_temp);
-    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf})
+    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf})
         if (s->p) cudaFree(s->p);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
     if (ctx->h_flags) cudaFreeHost(ctx->h_flags);
@@ -726,9 +728,10 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
 }
 
 // Ingest phase on the resident inputs: state reset, initial guess, intersection filter, Morton sort,
-// hashed multi-level grid. Shared by the registration path and mulls_pca_features.
+// hashed multi-level grid. Shared by the registration path and mulls_pca_features. finite_only (mulls_sor_filter, no
+// source, no motion undistortion): points with a non-finite coordinate stay out of the bbox and of the grid.
 static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &launches, mulls_allreduce_fn hook = nullptr,
-                         void *user = nullptr) {
+                         void *user = nullptr, bool finite_only = false) {
     cudaStream_t st = ctx->stream;
     const int np = (int)ctx->n_pairs;
     const uint32_t n_in = (uint32_t)ctx->n_in;
@@ -739,6 +742,7 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
     const unsigned n_inc = (unsigned)ctx->h_in_chunks.size();
     if (n_inc) {
         if (ctx->any_undistort) k_ingest_bbox<true><<<n_inc, kIngestBlock, 0, st>>>(A);
+        else if (finite_only) k_ingest_bbox<false, true><<<n_inc, kIngestBlock, 0, st>>>(A);
         else k_ingest_bbox<false><<<n_inc, kIngestBlock, 0, st>>>(A);
         ++launches;
     }
@@ -755,6 +759,7 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
     ++launches;
     if (n_inc) {
         if (ctx->any_undistort) k_make_keys<true><<<n_inc, kIngestBlock, 0, st>>>(A);
+        else if (finite_only) k_make_keys<false, true><<<n_inc, kIngestBlock, 0, st>>>(A);
         else k_make_keys<false><<<n_inc, kIngestBlock, 0, st>>>(A);
         ++launches;
         if (ctx->any_keep_less) { // random down-sampling of :2866-2892: radix select of the k-th sampling key
@@ -1352,6 +1357,89 @@ int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int
     ctx->stats = mulls_run_stats();
     ctx->stats.kernel_launches = launches;
     return MULLS_OK;
+}
+
+// ================================================================================================
+// Statistical outlier removal (CFilter::sor_filter, cfilter.hpp:203-247): kernels_sor.cuh
+// ================================================================================================
+static int sor_filter_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double n_std, uint8_t *keep_bits, float *mean_dist,
+                           mulls_sor_stats *stats) {
+    if (!ctx || mean_k < 1 || mean_k > kSorMaxMeanK || (cloud.n > 0 && (!cloud.aos48 || !keep_bits))) return MULLS_E_ARG;
+    const size_t n = cloud.n;
+    if (n > ctx->max_tgt) {
+        ctx->err = "mulls_sor_filter: the cloud exceeds max_tgt_pts of the context";
+        return MULLS_E_CAPACITY;
+    }
+    if (n <= (size_t)mean_k) { // (checked again on the finite points after the ingest)
+        ctx->err = "mulls_sor_filter: the cloud needs more than mean_k finite points";
+        return MULLS_E_ARG;
+    }
+    // the cloud becomes the only target class of a one-pair batch; normal_shooting_on asks k_pair_setup for the full
+    // level pyramid, whose top block spans the whole grid (the search has no radius)
+    mulls_icp_params P;
+    mulls_icp_default_params(&P);
+    std::strcpy(P.used_feature_type, "100000");
+    P.apply_intersection_filter = 0;
+    P.normal_shooting_on = 1;
+    P.max_iter_num = 0;
+    mulls_cloud_view tgt[MULLS_NUM_CLASSES] = {cloud, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
+    mulls_cloud_view src[MULLS_NUM_CLASSES] = {{nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
+    const double ident[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    int rc = upload_impl(ctx, 1, tgt, src, &P, ident, nullptr, nullptr, /*resident=*/false);
+    ctx->uploaded = false; // the resident batch is replaced by the cloud
+    if (rc != MULLS_OK) return rc;
+    const size_t words = ceil_div(n, 32);
+    const size_t off_bits = ceil_div(n * sizeof(float), 16) * 16, off_stats = off_bits + ceil_div(words * 4, 16) * 16;
+    if ((rc = grow_scratch(ctx, ctx->sor_buf, off_stats + sizeof(mulls_sor_stats))) != MULLS_OK) return rc;
+    float *d_dist = (float *)ctx->sor_buf.p;
+    uint32_t *d_keep = (uint32_t *)((char *)ctx->sor_buf.p + off_bits);
+    mulls_sor_stats *d_stats = (mulls_sor_stats *)((char *)ctx->sor_buf.p + off_stats);
+    cudaStream_t st = ctx->stream;
+    DeviceArrays A = ctx->A;
+    A.trace = nullptr;
+    uint64_t launches = 0;
+    if ((rc = launch_ingest(ctx, A, false, launches, nullptr, nullptr, /*finite_only=*/true)) != MULLS_OK) return rc;
+    // the grid must fit the hash pool before the search reads it (else grow the pool and build the grid again from the
+    // cloud already in HBM), and the finite points must be more than mean_k
+    int n_valid = 0;
+    CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&n_valid, (const char *)A.ps + offsetof(PairState, n_tgt), sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (ctx->h_flags[1]) {
+        if ((rc = grow_hash_pool(ctx)) != MULLS_OK) return rc;
+        A.hash = ctx->A.hash, A.hash_pool_entries = ctx->A.hash_pool_entries;
+        if ((rc = launch_ingest(ctx, A, false, launches, nullptr, nullptr, true)) != MULLS_OK) return rc;
+    }
+    if (n_valid <= mean_k) {
+        ctx->err = "mulls_sor_filter: " + std::to_string(n_valid) + " finite points, mean_k + 1 = " + std::to_string(mean_k + 1) +
+                   " neighbours wanted per point";
+        return MULLS_E_ARG;
+    }
+    CK(cudaMemsetAsync(d_dist, 0, n * sizeof(float), st)); // non-finite points: distance 0, as PCL
+    const unsigned nb = (unsigned)ceil_div((size_t)n_valid, kSorBlock);
+    if (mean_k + 1 <= 16) k_sor_dist<16><<<nb, kSorBlock, 0, st>>>(A, mean_k, d_dist);
+    else if (mean_k + 1 <= 32) k_sor_dist<32><<<nb, kSorBlock, 0, st>>>(A, mean_k, d_dist);
+    else k_sor_dist<64><<<nb, kSorBlock, 0, st>>>(A, mean_k, d_dist);
+    k_sor_stats<<<1, 32, 0, st>>>(A, d_dist, (uint32_t)n, n_std, d_stats);
+    k_sor_mark<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(d_dist, (uint32_t)n, d_stats, d_keep);
+    launches += 3;
+    CK(cudaGetLastError());
+    mulls_sor_stats h_stats;
+    CK(cudaMemcpyAsync(keep_bits, d_keep, (n + 7) / 8, cudaMemcpyDeviceToHost, st));
+    if (mean_dist) CK(cudaMemcpyAsync(mean_dist, d_dist, n * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&h_stats, d_stats, sizeof(h_stats), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (stats) *stats = h_stats;
+    ctx->stats = mulls_run_stats();
+    ctx->stats.kernel_launches = launches;
+    return MULLS_OK;
+}
+int mulls_sor_filter(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double n_std, uint8_t *keep_bits, float *mean_dist,
+                     mulls_sor_stats *stats) {
+    const int rc = sor_filter_impl(ctx, cloud, mean_k, n_std, keep_bits, mean_dist, stats);
+    // an error exit may leave the copy of the caller's cloud in flight: nothing is handed back before the stream drains
+    if (rc != MULLS_OK && ctx && ctx->stream) cudaStreamSynchronize(ctx->stream);
+    return rc;
 }
 
 // ================================================================================================

@@ -463,4 +463,118 @@ MULLS_HD float nn_search_walk(const GridView &g, float px, float py, float pz, f
     return nn_search_walk_b<WalkBounds>(g, px, py, pz, r2_prune, start_level, defer_scan, best_d2, best_j, st);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Exact k nearest targets with no search radius: same hierarchy as nn_search_walk, the pruning bound is the current k-th
+// best distance. Callers: the normal-shooting correspondences of cregistration.hpp:1732-1737
+// (pcl::registration::CorrespondenceEstimationNormalShooting, k = 10: k_search_shoot) and the statistical outlier
+// filter of cfilter.hpp:203-247 (pcl::StatisticalOutlierRemoval, k = mean_k + 1: k_sor_dist). Both build the full level
+// pyramid, whose top 2x2x2 block spans the whole grid, so the result is exact however far the targets are.
+// Total order (d2, original index). Plain per-thread DFS with its stack and the list in thread-local arrays.
+// kCap: the capacity of the list (compile time, it sizes the arrays); k <= kCap: the neighbours wanted.
+// ------------------------------------------------------------------------------------------------
+constexpr int kKnnStack = 48; // DFS entries: at most 7 stay behind per descended level
+
+template <int kCap>
+struct KnnList {
+    float d2[kCap];
+    int j[kCap];
+    int n;
+};
+
+// original index of sorted target j (tie-break of the total order)
+MULLS_HD int knn_orig(const GridView &g, int j) { return f2i_bits(ld_point(&g.nrm[j]).w); }
+
+template <int kCap>
+MULLS_HD float knn_bound(const KnnList<kCap> &kl, int k) { return kl.n < k ? INFINITY : kl.d2[k - 1]; }
+
+template <int kCap>
+MULLS_HD void knn_insert(const GridView &g, KnnList<kCap> &kl, int k, float d2, int j) {
+    if (kl.n == k) {
+        const float w = kl.d2[k - 1];
+        if (d2 > w) return;
+        if (d2 == w && knn_orig(g, j) >= knn_orig(g, kl.j[k - 1])) return;
+    }
+    for (int i = 0; i < kl.n; ++i)
+        if (kl.j[i] == j) return; // a point is met again when the search ascends a level
+    int pos = (kl.n < k) ? kl.n : k - 1;
+    while (pos > 0) {
+        const float dp = kl.d2[pos - 1];
+        bool before = d2 < dp;
+        if (d2 == dp) before = knn_orig(g, j) < knn_orig(g, kl.j[pos - 1]);
+        if (!before) break;
+        kl.d2[pos] = kl.d2[pos - 1];
+        kl.j[pos] = kl.j[pos - 1];
+        --pos;
+    }
+    kl.d2[pos] = d2;
+    kl.j[pos] = j;
+    if (kl.n < k) ++kl.n;
+}
+
+// squared distance from p to the (slightly inflated) box of cell (x,y,z) at a level with cell size hl
+MULLS_HD float cell_dist2(const GridView &g, float px, float py, float pz, float hl, int x, int y, int z, float margin) {
+    const float ax = slab_dist(g.ox + (float)x * hl, g.ox + (float)(x + 1) * hl, px, margin);
+    const float ay = slab_dist(g.oy + (float)y * hl, g.oy + (float)(y + 1) * hl, py, margin);
+    const float az = slab_dist(g.oz + (float)z * hl, g.oz + (float)(z + 1) * hl, pz, margin);
+    return ax * ax + ay * ay + az * az;
+}
+
+// kl receives the min(k, targets) nearest targets, ascending under the total order. 1 <= k <= kCap.
+template <int kCap>
+MULLS_HD void knn_search(const GridView &g, float px, float py, float pz, int start_level, int k, KnnList<kCap> &kl) {
+    kl.n = 0;
+    const int c0x = (int)floorf((px - g.ox) * g.inv_h0);
+    const int c0y = (int)floorf((py - g.oy) * g.inv_h0);
+    const int c0z = (int)floorf((pz - g.oz) * g.inv_h0);
+    const int L = g.n_levels;
+    const float margin = 1e-3f * g.h0;
+    uint2 st_cell[kKnnStack]; // pack_cell(x, y, z, level, 0)
+    float st_d2[kKnnStack];
+    const int l0 = start_level < 1 ? 1 : start_level;
+    for (int l = l0 < L - 1 ? l0 : L - 1;; ++l) {
+        const float H = g.h0 * (float)(1 << l);
+        const int ncell = 4096 >> l;
+        for (int b = 0; b < 8; ++b) { // own cell first, then the half-side neighbours
+            int x = (c0x >> l) + ((b & 1) ? ((((c0x >> (l - 1)) & 1) ? 1 : -1)) : 0);
+            int y = (c0y >> l) + ((b & 2) ? ((((c0y >> (l - 1)) & 1) ? 1 : -1)) : 0);
+            int z = (c0z >> l) + ((b & 4) ? ((((c0z >> (l - 1)) & 1) ? 1 : -1)) : 0);
+            if (ncell == 2) x = b & 1, y = (b >> 1) & 1, z = b >> 2; // top of the full pyramid: the 8 cells ARE the grid
+            if (x < 0 || y < 0 || z < 0 || x >= ncell || y >= ncell || z >= ncell) continue;
+            int sp = 0;
+            st_cell[0] = pack_cell((uint32_t)x, (uint32_t)y, (uint32_t)z, l, 0u);
+            st_d2[0] = cell_dist2(g, px, py, pz, H, x, y, z, margin);
+            sp = 1;
+            while (sp > 0) {
+                --sp;
+                if (st_d2[sp] > knn_bound(kl, k) * 1.0001f + 1e-12f) continue;
+                const uint2 ce = st_cell[sp];
+                const int lv = (int)((ce.y >> 4) & 0xfu);
+                const int cx = (int)(ce.x & 0xfffu), cy = (int)((ce.x >> 12) & 0xfffu), cz = (int)((ce.x >> 24) | ((ce.y & 0xfu) << 8));
+                uint32_t start, count, cmask;
+                if (!probe_cell(g, (uint32_t)cx, (uint32_t)cy, (uint32_t)cz, lv, start, count, cmask)) continue;
+                if (count <= (uint32_t)g.leaf_count || lv == 0 || sp + 8 > kKnnStack) {
+                    for (uint32_t jj = start; jj < start + count; ++jj) {
+                        const float4 q = ld_point(&g.pos[jj]);
+                        knn_insert(g, kl, k, flann_l2(px, py, pz, q.x, q.y, q.z), (int)jj);
+                    }
+                } else {
+                    const float hc = 0.5f * g.h0 * (float)(1 << lv);
+                    for (int ch = 7; ch >= 0; --ch) {
+                        if (!((cmask >> ch) & 1u)) continue;
+                        const int x2 = 2 * cx + (ch & 1), y2 = 2 * cy + ((ch >> 1) & 1), z2 = 2 * cz + (ch >> 2);
+                        const float d2c = cell_dist2(g, px, py, pz, hc, x2, y2, z2, margin);
+                        if (d2c > knn_bound(kl, k) * 1.0001f + 1e-12f) continue;
+                        st_cell[sp] = pack_cell((uint32_t)x2, (uint32_t)y2, (uint32_t)z2, lv - 1, 0u);
+                        st_d2[sp] = d2c;
+                        ++sp;
+                    }
+                }
+            }
+        }
+        const float cover = 0.999f * 0.5f * H; // every target closer than this has been examined
+        if (kl.n == k && kl.d2[k - 1] <= cover * cover) break;
+        if (l == L - 1) break; // the top block spans the whole grid: everything has been examined
+    }
+}
+
 } // namespace mulls

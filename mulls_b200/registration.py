@@ -273,6 +273,21 @@ class Context:
             res[abi.OUT_NAMES[k]] = np.ascontiguousarray(cbufs[k][: out.cls.n[k]])
         return res
 
+    def sor_filter(self, cloud: np.ndarray, mean_k: int, n_std: float):
+        """CFilter::sor_filter (cfilter.hpp:203-247, pcl::StatisticalOutlierRemoval) on the GPU. Returns (keep: bool[n],
+        the kept points being cloud[keep]; mean_dist: float32[n], 0 for non-finite points; stats: dict of mean, stddev,
+        threshold, n_valid, n_kept)."""
+        c = abi.as_aos48(cloud)
+        n = c.shape[0]
+        bits = np.zeros(max((n + 7) // 8, 1), np.uint8)
+        dist = np.zeros(max(n, 1), np.float32)
+        st = abi.SorStats()
+        self._check(self.lib.mulls_sor_filter(self.handle, abi.cloud_view(c), int(mean_k), float(n_std),
+                                              bits.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                              dist.ctypes.data_as(C.POINTER(C.c_float)), C.byref(st)))
+        keep = np.unpackbits(bits, bitorder="little")[:n].astype(bool)
+        return keep, dist[:n], {k: getattr(st, k) for k, _ in abi.SorStats._fields_}
+
     def stats(self) -> dict:
         s = abi.RunStats()
         self._check(self.lib.mulls_get_stats(self.handle, C.byref(s)))

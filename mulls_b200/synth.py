@@ -299,6 +299,34 @@ def make_sequence(seed: int, n_frames: int, config: str = "small", n_points: int
     return {"scans": scans, "poses": poses, "params": kitti_urban_params(max_iter)}
 
 
+def make_merged_map(seed: int, n_sweeps: int, n_points: int = 120000, n_copies: int = 1,
+                    outlier_ratio: float = 0.002) -> np.ndarray:
+    """The cloud test/mulls_slam.cpp:1008-1009 hands to CFilter::sor_filter (pc_map_merged): every sweep of a drive,
+    moved by its pose into the map frame, plus `outlier_ratio` of isolated points scattered over the map's box (what the
+    filter is there to remove). n_copies > 1 repeats the drive's map shifted 200 m along x each time: a longer street
+    from the same sweeps, cheap to make. Returns (n, 12) float32 rows."""
+    scene = make_scene(seed)
+    M = gt_motion()
+    rng = np.random.default_rng(seed)
+    pose = np.eye(4)
+    parts = []
+    for k in range(n_sweeps):
+        sc = np.concatenate(scan(scene, _sensor_pose(pose), seed * 7919 + k, n_points=n_points), axis=0).astype(np.float64)
+        sc[:, 0:3] = sc[:, 0:3] @ pose[:3, :3].T + pose[:3, 3]
+        sc[:, 3:6] = sc[:, 3:6] @ pose[:3, :3].T
+        parts.append(sc)
+        pose = pose @ M
+    drive = np.concatenate(parts, axis=0)
+    drive = np.concatenate([drive + np.array([200.0 * c, 0, 0, 0, 0, 0, 0]) for c in range(n_copies)], axis=0)
+    lo, hi = drive[:, :3].min(0), drive[:, :3].max(0)
+    n_out = int(len(drive) * outlier_ratio)
+    out = np.zeros((n_out, 7))
+    out[:, :3] = rng.uniform(lo, hi, (n_out, 3))
+    out[:, 5] = 1.0
+    cloud = np.concatenate([drive, out], axis=0)
+    return abi.as_aos48(cloud[rng.permutation(len(cloud))].astype(np.float32))
+
+
 def pose_error(T_a: np.ndarray, T_b: np.ndarray):
     """Translation (m) and rotation (rad) difference, the formulas of nav/odom_error_compute.h:65-82."""
     dt = float(np.linalg.norm(T_a[:3, 3] - T_b[:3, 3]))
