@@ -65,6 +65,7 @@ bool classify_nground_pts(typename pcl::PointCloud<PointT>::Ptr &cloud_in, typen
     p.feature_pts_ratio_guess = feature_pts_ratio_guess;
     p.sharpen_with_nms = sharpen_with_nms;
     p.use_distance_adaptive_pca = use_distance_adaptive_pca;
+    p.pca_unit_distance = 30.0f; // the unit classify_nground_pts hands get_pc_pca_feature (cfilter.hpp:2093)
     p.random_seed = call_seed++;
 
     const size_t n = cloud_in->points.size();
@@ -272,6 +273,7 @@ bool extract_semantic_pts(BlockPtr in_block, float vf_downsample_resolution, flo
     P.classify.feature_pts_ratio_guess = feature_pts_ratio_guess;
     P.classify.sharpen_with_nms = sharpen_with_nms_on;
     P.classify.use_distance_adaptive_pca = use_distance_adaptive_pca;
+    P.classify.pca_unit_distance = 30.0f; // cfilter.hpp:2093
     P.classify.random_seed = call_seed++;
 
     const size_t n = in_block->pc_raw->points.size();

@@ -180,6 +180,7 @@ class ClassifyParams(C.Structure):
         ("sharpen_with_nms", C.c_int32),
         ("use_distance_adaptive_pca", C.c_int32),
         ("random_seed", C.c_uint32),
+        ("pca_unit_distance", C.c_float),
     ]
 
 
@@ -261,6 +262,7 @@ EXPORTED_SYMBOLS = (
     "mulls_get_stats",
     "mulls_icp_run_sharded",
     "mulls_pca_features",
+    "mulls_pca_features_adaptive",
     "mulls_map_default_params",
     "mulls_map_create",
     "mulls_map_destroy",
@@ -338,6 +340,8 @@ def load_library() -> C.CDLL:
                                                C.POINTER(IcpResult), C.POINTER(IcpTrace)]
     lib.mulls_pca_features.restype = C.c_int
     lib.mulls_pca_features.argtypes = [vp, CloudView, C.c_float, C.c_int, C.c_int, C.POINTER(PcaOut)]
+    lib.mulls_pca_features_adaptive.restype = C.c_int
+    lib.mulls_pca_features_adaptive.argtypes = [vp, CloudView, C.c_float, C.c_int, C.c_int, C.c_float, C.POINTER(PcaOut)]
     lib.mulls_ground_default_params.restype = None
     lib.mulls_ground_default_params.argtypes = [C.POINTER(GroundParams)]
     lib.mulls_fast_ground_filter.restype = C.c_int
@@ -536,6 +540,7 @@ def default_classify_params() -> ClassifyParams:
     p.sharpen_with_nms = 1
     p.use_distance_adaptive_pca = 0
     p.random_seed = 0
+    p.pca_unit_distance = 0.0
     return p
 
 

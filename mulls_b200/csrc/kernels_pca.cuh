@@ -7,10 +7,13 @@
 // One WARP per query on the same Morton-sorted cloud + hashed grid the registration path builds: lanes
 // probe the 27 cells of the level whose cell size covers the radius in parallel, stream the candidates
 // into a shared-memory list, radix-select the k-th smallest distance when more than k are in range, and
-// reduce mean and covariance with shuffles. fp64 accumulation; the 3x3 symmetric eigen problem is solved
+// reduce mean and covariance with shuffles. k_pca<true> gives every query its distance-adaptive radius (one warp per
+// query keeps it warp-uniform); k_pca<false> is the fixed radius. fp64 accumulation; the 3x3 symmetric eigen problem is solved
 // by cyclic Jacobi in fp64 (the reference's float SelfAdjointEigenSolver agrees to float rounding, which
 // is the tolerance the parity tests state).
 #pragma once
+#include <type_traits>
+
 #include "device_math.cuh"
 #include "device_types.cuh"
 #include "kernels_ingest.cuh"
@@ -33,6 +36,21 @@ struct PcaArgs {
     uint32_t *nbr; // [n][k]
 };
 constexpr int kPcaListCap = 64;
+
+// Distance-adaptive neighbourhoods (get_pc_pca_feature with distance_adaptive_on, pca.hpp:310-326): a query farther than
+// unit_dist from the origin searches the radius sqrt(dist / unit_dist) * radius. `radius` / `r2` stay the base radius,
+// which the close / far split of the neighbour lists keeps reading (pca.hpp:337).
+struct PcaAdaptiveArgs : PcaArgs {
+    float unit_dist; // > 0
+};
+template <bool kAdaptive> using PcaKernelArgs = std::conditional_t<kAdaptive, PcaAdaptiveArgs, PcaArgs>;
+
+// dist = std::sqrt(float x*x + y*y + z*z) (the float overload, widened); strict `dist > unit_dist`; the radius is the
+// double product narrowed to float
+__device__ __forceinline__ float pca_adaptive_radius(float x, float y, float z, float radius, float unit_dist) {
+    const double dist = (double)__fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
+    return dist > (double)unit_dist ? (float)(__dsqrt_rn(__ddiv_rn(dist, (double)unit_dist)) * (double)radius) : radius;
+}
 
 __device__ inline void jacobi_eig3(double A[3][3], double w[3], double V[3][3]) {
     for (int i = 0; i < 3; ++i)
@@ -94,7 +112,8 @@ __device__ __forceinline__ int count_less(const uint32_t *keys, int m, uint32_t 
     return c;
 }
 
-__global__ void __launch_bounds__(kPcaWarps * 32) k_pca(DeviceArrays A, PcaArgs P) {
+template <bool kAdaptive>
+__global__ void __launch_bounds__(kPcaWarps * 32) k_pca(DeviceArrays A, PcaKernelArgs<kAdaptive> P) {
     __shared__ uint32_t s_key[kPcaWarps][kPcaCap]; // d2 bits
     __shared__ int s_idx[kPcaWarps][kPcaCap];      // sorted-position of the neighbour
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -110,14 +129,21 @@ __global__ void __launch_bounds__(kPcaWarps * 32) k_pca(DeviceArrays A, PcaArgs 
     const float4 p = pos[qi];
     uint32_t *keys = s_key[warp];
     int *idxs = s_idx[warp];
+    // this query's search radius (warp-uniform: one warp serves one query)
+    float radius = P.radius, r2 = P.r2;
+    if constexpr (kAdaptive) {
+        radius = pca_adaptive_radius(p.x, p.y, p.z, P.radius, P.unit_dist);
+        r2 = (float)((double)radius * (double)radius);
+    }
 
-    // level whose cells are at least as wide as the radius: its 3x3x3 block around p covers the sphere
+    // level whose cells are at least as wide as the radius: its 3x3x3 block around p covers the sphere (the adaptive
+    // ingest builds the full pyramid, whose top block spans the grid whatever the radius)
     int lq = 0;
-    while (lq < ps.n_levels - 1 && 0.999f * ps.h0 * (float)(1 << lq) < P.radius) ++lq;
+    while (lq < ps.n_levels - 1 && 0.999f * ps.h0 * (float)(1 << lq) < radius) ++lq;
     // Progressive radius: a 3x3x3 block of level-l cells contains every point within 0.999*h_l of p. Where the cloud is
     // dense the k nearest neighbours lie well inside the radius, so start two levels finer and accept the first level
     // whose guaranteed sphere already holds k points — same neighbours, a fraction of the candidates.
-    float rb2 = P.r2; // squared acceptance bound of the candidate stream
+    float rb2 = r2; // squared acceptance bound of the candidate stream
     uint32_t my_start = 0, my_count = 0;
     int m = 0;       // entries in the list (capped)
     int m_total = 0; // neighbours within the bound
@@ -125,9 +151,9 @@ __global__ void __launch_bounds__(kPcaWarps * 32) k_pca(DeviceArrays A, PcaArgs 
         const bool last = l >= lq;
         if (!last) {
             const float cover = 0.999f * ps.h0 * (float)(1 << l);
-            rb2 = fminf(cover * cover, P.r2);
+            rb2 = fminf(cover * cover, r2);
         } else {
-            rb2 = P.r2;
+            rb2 = r2;
         }
         const int ncell = (1 << kCoordBits) >> l;
         const int cx = ((int)floorf((p.x - ps.origin[0]) * ps.inv_h0)) >> l;

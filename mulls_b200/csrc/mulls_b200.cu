@@ -1276,15 +1276,20 @@ int mulls_icp_run_sharded(mulls_ctx *ctx, const mulls_cloud_view tgt[MULLS_NUM_C
 } // extern "C"
 
 // PCA features of one cloud (host rows, or rows already in HBM) into ctx->pca_buf; `args` receives the device arrays.
-// Nothing is synchronised: the caller consumes the arrays on ctx->stream.
+// unit_dist > 0: distance-adaptive neighbourhoods (k_pca<true>). Nothing is synchronised: the caller consumes the arrays
+// on ctx->stream.
 static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_device, float radius, int k, int stride,
-                         PcaArgs &args, uint64_t &launches, uint32_t *nbr = nullptr) {
+                         PcaArgs &args, uint64_t &launches, uint32_t *nbr = nullptr, float unit_dist = 0.f) {
+    const bool adaptive = unit_dist > 0.f;
     // the cloud becomes the only target class of a one-pair batch: same filter-less ingest, same grid
     mulls_icp_params P;
     mulls_icp_default_params(&P);
     std::strcpy(P.used_feature_type, "100000");
     P.apply_intersection_filter = 0;
     P.dis_thre_unit = radius; // the grid's top level then covers 2.5 x radius
+    // an adaptive radius grows without bound with the range: normal_shooting_on asks k_pair_setup for the full level
+    // pyramid, whose top block spans the whole grid
+    if (adaptive) P.normal_shooting_on = 1;
     P.max_iter_num = 0;
     mulls_cloud_view tgt[MULLS_NUM_CLASSES] = {cloud, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
     mulls_cloud_view src[MULLS_NUM_CLASSES] = {{nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
@@ -1319,17 +1324,23 @@ static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_d
     args.pt_num = (int *)(args.normal + 3 * n);
     args.nbr = nbr;
     CK(cudaMemsetAsync(ctx->pca_buf.p, 0, std::max<size_t>(bytes, 16), st));
-    if (n) {
-        k_pca<<<(unsigned)ceil_div(n, kPcaWarps), kPcaWarps * 32, 0, st>>>(A, args);
+    if (n && adaptive) {
+        PcaAdaptiveArgs aa;
+        static_cast<PcaArgs &>(aa) = args;
+        aa.unit_dist = unit_dist;
+        k_pca<true><<<(unsigned)ceil_div(n, kPcaWarps), kPcaWarps * 32, 0, st>>>(A, aa);
+        ++launches;
+    } else if (n) {
+        k_pca<false><<<(unsigned)ceil_div(n, kPcaWarps), kPcaWarps * 32, 0, st>>>(A, args);
         ++launches;
     }
     ctx->uploaded = false; // the resident batch was replaced by the PCA cloud
     return MULLS_OK;
 }
 
-extern "C" {
-
-int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int k, int stride, mulls_pca_out *out) {
+// mulls_pca_features / mulls_pca_features_adaptive (unit_dist > 0)
+static int pca_features_impl(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int k, int stride, float unit_dist,
+                             mulls_pca_out *out) {
     if (!ctx || !out || !out->eigenvalues || !out->principal || !out->normal || !out->pt_num || stride < 1 ||
         !(radius > 0.f))
         return MULLS_E_ARG;
@@ -1343,7 +1354,7 @@ int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int
         if (const int rc = grow_scratch(ctx, ctx->cls_buf, n * (size_t)k * sizeof(uint32_t)); rc != MULLS_OK) return rc;
         nbr = (uint32_t *)ctx->cls_buf.p;
     }
-    int rc = pca_on_device(ctx, cloud, false, radius, k, stride, args, launches, nbr);
+    int rc = pca_on_device(ctx, cloud, false, radius, k, stride, args, launches, nbr, unit_dist);
     if (rc != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
     if (n) {
@@ -1357,6 +1368,18 @@ int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int
     ctx->stats = mulls_run_stats();
     ctx->stats.kernel_launches = launches;
     return MULLS_OK;
+}
+
+extern "C" {
+
+int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int k, int stride, mulls_pca_out *out) {
+    return pca_features_impl(ctx, cloud, radius, k, stride, 0.f, out);
+}
+
+int mulls_pca_features_adaptive(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int k, int stride, float unit_dist,
+                                mulls_pca_out *out) {
+    if (!(unit_dist > 0.f)) return MULLS_E_ARG;
+    return pca_features_impl(ctx, cloud, radius, k, stride, unit_dist, out);
 }
 
 // ================================================================================================
@@ -1831,16 +1854,19 @@ void mulls_classify_default_params(mulls_classify_params *p) {
     p->sharpen_with_nms = 1;
     p->use_distance_adaptive_pca = 0;
     p->random_seed = 0;
+    p->pca_unit_distance = 0.f;
 }
 
 int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_classify_params *params,
                            mulls_classify_out *out) {
     if (!ctx || !params || !out || (cloud_in.n > 0 && !cloud_in.aos48)) return MULLS_E_ARG;
     const mulls_classify_params &P = *params;
-    if (P.use_distance_adaptive_pca) {
-        ctx->err = "mulls_classify_nground: use_distance_adaptive_pca is not implemented";
+    // the reference names two units (30 at cfilter.hpp:2093, 35 as get_pc_pca_feature's default): the caller picks one
+    if (P.use_distance_adaptive_pca && !(P.pca_unit_distance > 0.f)) {
+        ctx->err = "mulls_classify_nground: use_distance_adaptive_pca needs pca_unit_distance > 0";
         return MULLS_E_UNSUPPORTED;
     }
+    const float unit_dist = P.use_distance_adaptive_pca ? P.pca_unit_distance : 0.f;
     if (P.neighbor_k < 1 || P.neighbor_k > kPcaListCap || !(P.neighbor_searching_radius > 0.f)) {
         ctx->err = "mulls_classify_nground: neighbor_k must be 1..64 and the radius positive";
         return MULLS_E_ARG;
@@ -1914,7 +1940,8 @@ int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mull
     if (n > 0) {
         // :2089-2097 PCA of every pca_down_rate-th point, with the neighbour lists
         mulls_cloud_view v{(const float *)C.rows, n};
-        const int rc = pca_on_device(ctx, v, true, P.neighbor_searching_radius, P.neighbor_k, stride, C.F, launches, nbr);
+        const int rc = pca_on_device(ctx, v, true, P.neighbor_searching_radius, P.neighbor_k, stride, C.F, launches, nbr,
+                                     unit_dist);
         if (rc != MULLS_OK) return rc;
         C.keys_a = ctx->A.keys_a;
         C.keys_b = ctx->A.keys_b;

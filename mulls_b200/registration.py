@@ -211,8 +211,9 @@ class Context:
                                             idx.ctypes.data_as(C.POINTER(C.c_int32)), d2.ctypes.data_as(C.POINTER(C.c_float))))
         return idx, d2
 
-    def pca_features(self, cloud: np.ndarray, radius: float, k: int, stride: int = 1) -> dict:
-        """PrincipleComponentAnalysis::get_pc_pca_feature (pca.hpp:294-354) on the GPU."""
+    def pca_features(self, cloud: np.ndarray, radius: float, k: int, stride: int = 1, unit_dist=None) -> dict:
+        """PrincipleComponentAnalysis::get_pc_pca_feature (pca.hpp:294-354) on the GPU. With `unit_dist`,
+        distance_adaptive_on = true: points farther than unit_dist from the origin search sqrt(dist / unit_dist) * radius."""
         c = abi.as_aos48(cloud)
         n = c.shape[0]
         ev = np.zeros((n, 3), np.float32)
@@ -221,8 +222,12 @@ class Context:
         cnt = np.zeros(n, np.int32)
         out = abi.PcaOut(ev.ctypes.data_as(C.POINTER(C.c_float)), pr.ctypes.data_as(C.POINTER(C.c_float)),
                          nr.ctypes.data_as(C.POINTER(C.c_float)), cnt.ctypes.data_as(C.POINTER(C.c_int32)))
-        self._check(self.lib.mulls_pca_features(self.handle, abi.cloud_view(c), float(radius), int(k), int(stride),
-                                                C.byref(out)))
+        if unit_dist is None:
+            rc = self.lib.mulls_pca_features(self.handle, abi.cloud_view(c), float(radius), int(k), int(stride), C.byref(out))
+        else:
+            rc = self.lib.mulls_pca_features_adaptive(self.handle, abi.cloud_view(c), float(radius), int(k), int(stride),
+                                                      float(unit_dist), C.byref(out))
+        self._check(rc)
         return {"eigenvalues": ev, "principal": pr, "normal": nr, "pt_num": cnt}
 
     def classify_nground(self, cloud_in: np.ndarray, params: abi.ClassifyParams) -> dict:
