@@ -1,5 +1,7 @@
 // Drop-in shims: lo::CFilter<PointT>::classify_nground_pts (include/common/cfilter.hpp:2058-2290), fast_ground_filter
-// (:1658-2036), voxel_downsample (:83-165) and sor_filter (:203-247) over the mulls_b200 C-ABI. A MULLS maintainer replaces the BODY of classify_nground_pts by
+// (:1658-2036), voxel_downsample (:83-165), sor_filter (:203-247), scanner_filter (:914-929) and the raw-scan corrections
+// vertical_intrinsic_calibration (:250-291), get_pts_timestamp_ratio_in_frame (:412-467), apply_motion_compensation and
+// batch_apply_motion_compensation (:470-549) over the mulls_b200 C-ABI. A MULLS maintainer replaces the BODY of classify_nground_pts by
 //
 //     return lo::b200::classify_nground_pts<PointT>(cloud_in, cloud_pillar, ... );      // all arguments forwarded
 //
@@ -196,10 +198,28 @@ bool sor_filter(typename pcl::PointCloud<PointT>::Ptr &cloud_in_out, int mean_k,
     return sor_filter<PointT>(cloud_in_out, cloud_in_out, mean_k, n_std);
 }
 
+// lo::CFilter<PointT>::scanner_filter (include/common/cfilter.hpp:914-929) in float, on the host: drops the points within
+// self_radius of the scanner axis (the ego vehicle) or below z_min_thre_global, and the points within ghost_radius that
+// lie at or below z_min_thre_ghost (underground ghosts). The kept rows stay in input order; the cloud shrinks in place.
+template <typename PointT>
+bool scanner_filter(const typename pcl::PointCloud<PointT>::Ptr &cloud_in_out, float self_radius, float ghost_radius,
+                    float z_min_thre_ghost, float z_min_thre_global) {
+    std::vector<PointT> kept;
+    kept.reserve(cloud_in_out->points.size());
+    for (const PointT &p : cloud_in_out->points) {
+        const float dis_square = p.x * p.x + p.y * p.y;
+        if (dis_square > self_radius * self_radius && p.z > z_min_thre_global)
+            if (dis_square > ghost_radius * ghost_radius || p.z > z_min_thre_ghost) kept.push_back(p);
+    }
+    cloud_in_out->points.swap(kept);
+    return true;
+}
+
 // lo::CFilter<PointT>::extract_semantic_pts (include/common/cfilter.hpp:2295-2413): same names, order, types and
-// defaults as :2295-2318. Covers :2346-2399 — voxel_downsample, pc_sketch, fast_ground_filter, classify_nground_pts and
+// defaults as :2295-2318. With apply_scanner_filter (and no semantic_assisted) pc_raw first goes through scanner_filter
+// as at :2334-2343, and shrinks in place as in the reference. Covers :2346-2399 — voxel_downsample, pc_sketch, fast_ground_filter, classify_nground_pts and
 // the feature count — with the three heavy stages chained in HBM (mulls_extract_semantic_pts): replace those lines of
-// the member by a call forwarding every argument. The pre-filters on pc_raw (:2328-2342) and
+// the member by a call forwarding every argument. The semantic-mask pre-filter (:2331-2332) and
 // update_parameters_self_adaptive (:2406-2410) are CFilter members and stay where they are, before / after the call.
 template <typename PointT, typename BlockPtr>
 bool extract_semantic_pts(BlockPtr in_block, float vf_downsample_resolution, float gf_grid_resolution, float gf_max_grid_height_diff,
@@ -223,8 +243,15 @@ bool extract_semantic_pts(BlockPtr in_block, float vf_downsample_resolution, flo
                           float roi_max_y = 0.0) {
     static_assert(sizeof(PointT) == 48, "the C-ABI consumes pcl::PointXYZINormal rows (48 bytes)");
     static thread_local uint32_t call_seed = 0;
-    (void)use_adpative_parameters, (void)extract_curb_or_not, (void)approx_scanner_height, (void)underground_thre;
-    (void)semantic_assisted, (void)apply_roi_filtering, (void)roi_min_y, (void)roi_max_y;
+    (void)use_adpative_parameters, (void)extract_curb_or_not;
+    (void)apply_roi_filtering, (void)roi_min_y, (void)roi_max_y;
+    if (!semantic_assisted && apply_scanner_filter) { // :2331-2343 (the semantic mask branch is not covered)
+        float self_ring_radius = 1.75;
+        float ghost_radius = 20.0;
+        float z_min = -approx_scanner_height - 4.0;
+        float z_min_min = -approx_scanner_height + underground_thre;
+        scanner_filter<PointT>(in_block->pc_raw, self_ring_radius, ghost_radius, z_min, z_min_min);
+    }
     mulls_extract_params P;
     P.vf_downsample_resolution = vf_downsample_resolution;
     mulls_ground_default_params(&P.ground);
@@ -316,6 +343,132 @@ bool extract_semantic_pts(BlockPtr in_block, float vf_downsample_resolution, flo
                                        in_block->pc_beam_down->points.size() + in_block->pc_facade_down->points.size() +
                                        in_block->pc_roof_down->points.size() + in_block->pc_vertex->points.size(); // :2398-2399
     return true;
+}
+
+// ---- raw-scan corrections (mulls_vertical_intrinsic_calibration, mulls_timestamp_ratio, mulls_motion_compensation):
+// the cloud's rows go to the device, the changed column comes back and is scattered into points[i]. A refused call (no
+// device) logs the error and leaves the cloud as it was.
+
+// lo::CFilter<PointT>::vertical_intrinsic_calibration (include/common/cfilter.hpp:250-291), same defaults
+template <typename PointT>
+bool vertical_intrinsic_calibration(typename pcl::PointCloud<PointT>::Ptr &cloud_in_out, double var_vertical_ang_d = 0.0,
+                                    bool inverse_z = false) {
+    static_assert(sizeof(PointT) == 48, "the C-ABI consumes pcl::PointXYZINormal rows (48 bytes)");
+    if (var_vertical_ang_d == 0) return false; // :252-253
+    const size_t n = cloud_in_out->points.size();
+    mulls_ctx *ctx = thread_context(1, n);
+    std::vector<float> xyz(3 * n + 1);
+    int applied = 0;
+    if (!ctx || mulls_vertical_intrinsic_calibration(ctx, view_of<PointT>(cloud_in_out), var_vertical_ang_d, inverse_z ? 1 : 0,
+                                                     xyz.data(), &applied) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return false;
+    }
+    for (size_t i = 0; i < n; ++i) {
+        PointT &p = cloud_in_out->points[i];
+        p.x = xyz[3 * i], p.y = xyz[3 * i + 1], p.z = xyz[3 * i + 2];
+    }
+    return applied != 0;
+}
+
+// lo::CFilter<PointT>::get_pts_timestamp_ratio_in_frame (include/common/cfilter.hpp:412-467), same defaults: the
+// curvature of every point becomes its timestamp ratio in the frame
+template <typename PointT>
+bool get_pts_timestamp_ratio_in_frame(typename pcl::PointCloud<PointT>::Ptr &cloud_in_out, bool timestamp_availiable = true,
+                                      double scan_begin_ang_anticlock_x_positive_deg = 180.0, float scan_duration_ms = 100) {
+    static_assert(sizeof(PointT) == 48, "the C-ABI consumes pcl::PointXYZINormal rows (48 bytes)");
+    const size_t n = cloud_in_out->points.size();
+    mulls_ctx *ctx = thread_context(1, n);
+    std::vector<float> ratio(n + 1);
+    if (!ctx || mulls_timestamp_ratio(ctx, view_of<PointT>(cloud_in_out), timestamp_availiable ? 1 : 0,
+                                      scan_begin_ang_anticlock_x_positive_deg, scan_duration_ms, ratio.data()) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return false;
+    }
+    for (size_t i = 0; i < n; ++i) cloud_in_out->points[i].curvature = ratio[i];
+    return true;
+}
+
+// apply_motion_compensation over n_clouds (in[k] -> out[k]) pairs in one device call; out[k] may be in[k]. When two
+// pairs share a cloud the reference's sequential order matters, and the pairs are run one call each, in order.
+template <typename PointT>
+bool motion_compensation(const typename pcl::PointCloud<PointT>::Ptr *in, const typename pcl::PointCloud<PointT>::Ptr *out,
+                         int n_clouds, const Eigen::Matrix4d &Tran, float s_ambigous_thre) {
+    static_assert(sizeof(PointT) == 48, "the C-ABI consumes pcl::PointXYZINormal rows (48 bytes)");
+    for (int a = 0; a < n_clouds; ++a)
+        for (int b = a + 1; b < n_clouds; ++b)
+            if (in[a].get() == in[b].get() || in[a].get() == out[b].get() || out[a].get() == in[b].get() ||
+                out[a].get() == out[b].get()) {
+                bool ok = true;
+                for (int k = 0; k < n_clouds; ++k) ok = motion_compensation<PointT>(in + k, out + k, 1, Tran, s_ambigous_thre) && ok;
+                return ok;
+            }
+    double T[16];
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) T[4 * r + c] = Tran(r, c);
+    mulls_cloud_view views[MULLS_NUM_CLASSES];
+    std::vector<float> xyz[MULLS_NUM_CLASSES];
+    float *dst[MULLS_NUM_CLASSES];
+    size_t total = 0;
+    for (int k = 0; k < n_clouds; ++k) {
+        views[k] = view_of<PointT>(in[k]);
+        xyz[k].resize(3 * views[k].n + 1);
+        dst[k] = xyz[k].data();
+        total += views[k].n;
+    }
+    mulls_ctx *ctx = thread_context(1, total);
+    if (!ctx || mulls_motion_compensation(ctx, views, n_clouds, T, s_ambigous_thre, dst) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return false;
+    }
+    for (int k = 0; k < n_clouds; ++k) {
+        if (out[k].get() != in[k].get()) *out[k] = *in[k]; // :496
+        for (size_t i = 0; i < views[k].n; ++i) {
+            PointT &p = out[k]->points[i];
+            p.x = xyz[k][3 * i], p.y = xyz[k][3 * i + 1], p.z = xyz[k][3 * i + 2];
+        }
+    }
+    return true;
+}
+
+// lo::CFilter<PointT>::apply_motion_compensation, in place (include/common/cfilter.hpp:470-491)
+template <typename PointT>
+void apply_motion_compensation(typename pcl::PointCloud<PointT>::Ptr pc_in_out, Eigen::Matrix4d &Tran, float s_ambigous_thre = 0.000) {
+    motion_compensation<PointT>(&pc_in_out, &pc_in_out, 1, Tran, s_ambigous_thre);
+}
+
+// lo::CFilter<PointT>::apply_motion_compensation, pc_in -> pc_out (include/common/cfilter.hpp:493-516)
+template <typename PointT>
+void apply_motion_compensation(const typename pcl::PointCloud<PointT>::Ptr pc_in, typename pcl::PointCloud<PointT>::Ptr pc_out,
+                               Eigen::Matrix4d &Tran, float s_ambigous_thre = 0.0) {
+    motion_compensation<PointT>(&pc_in, &pc_out, 1, Tran, s_ambigous_thre);
+}
+
+// lo::CFilter<PointT>::batch_apply_motion_compensation, in place (include/common/cfilter.hpp:519-531): five or six
+// clouds in one call, with the threshold 0 of the calls it makes
+template <typename PointT>
+void batch_apply_motion_compensation(typename pcl::PointCloud<PointT>::Ptr pc_ground, typename pcl::PointCloud<PointT>::Ptr pc_pillar,
+                                     typename pcl::PointCloud<PointT>::Ptr pc_beam, typename pcl::PointCloud<PointT>::Ptr pc_facade,
+                                     typename pcl::PointCloud<PointT>::Ptr pc_roof, typename pcl::PointCloud<PointT>::Ptr pc_vertex,
+                                     Eigen::Matrix4d &Tran, bool undistort_keypoints_or_not = false) {
+    const typename pcl::PointCloud<PointT>::Ptr c[6] = {pc_ground, pc_pillar, pc_beam, pc_facade, pc_roof, pc_vertex};
+    motion_compensation<PointT>(c, c, undistort_keypoints_or_not ? 6 : 5, Tran, 0.0f);
+}
+
+// lo::CFilter<PointT>::batch_apply_motion_compensation, into the *_undistort clouds (include/common/cfilter.hpp:534-549)
+template <typename PointT>
+void batch_apply_motion_compensation(
+    const typename pcl::PointCloud<PointT>::Ptr pc_ground, const typename pcl::PointCloud<PointT>::Ptr pc_pillar,
+    const typename pcl::PointCloud<PointT>::Ptr pc_beam, const typename pcl::PointCloud<PointT>::Ptr pc_facade,
+    const typename pcl::PointCloud<PointT>::Ptr pc_roof, const typename pcl::PointCloud<PointT>::Ptr pc_vertex,
+    typename pcl::PointCloud<PointT>::Ptr pc_ground_undistort, typename pcl::PointCloud<PointT>::Ptr pc_pillar_undistort,
+    typename pcl::PointCloud<PointT>::Ptr pc_beam_undistort, typename pcl::PointCloud<PointT>::Ptr pc_facade_undistort,
+    typename pcl::PointCloud<PointT>::Ptr pc_roof_undistort, typename pcl::PointCloud<PointT>::Ptr pc_vertex_undistort,
+    Eigen::Matrix4d &Tran, bool undistort_keypoints_or_not = false) {
+    const typename pcl::PointCloud<PointT>::Ptr in[6] = {pc_ground, pc_pillar, pc_beam, pc_facade, pc_roof, pc_vertex};
+    const typename pcl::PointCloud<PointT>::Ptr out[6] = {pc_ground_undistort, pc_pillar_undistort, pc_beam_undistort,
+                                                          pc_facade_undistort, pc_roof_undistort, pc_vertex_undistort};
+    motion_compensation<PointT>(in, out, undistort_keypoints_or_not ? 6 : 5, Tran, 0.0f);
 }
 
 } // namespace b200

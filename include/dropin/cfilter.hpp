@@ -3,8 +3,10 @@
 // reference's own cfilter.hpp is pulled in with its class renamed to CFilter_reference, and lo::CFilter<PointT> is
 // defined here as a class derived from it whose extract_semantic_pts (cfilter.hpp:2295-2318: same name, argument
 // order, types and defaults — all fifty of them), voxel_downsample (:83), fast_ground_filter (:1658-1672),
-// classify_nground_pts (:2058-2081) and both sor_filter overloads (:204, :225) run on the GPU through the C-ABI.
-// Every other member (dist_filter, non_max_suppress, random_downsample, apply_motion_compensation, get_cloud_bbx, ...
+// classify_nground_pts (:2058-2081), both sor_filter overloads (:204, :225), vertical_intrinsic_calibration (:250),
+// get_pts_timestamp_ratio_in_frame (:412) and every overload of apply_motion_compensation (:470, :493) and
+// batch_apply_motion_compensation (:519, :534) run on the GPU through the C-ABI.
+// Every other member (dist_filter, non_max_suppress, random_downsample, get_cloud_bbx, ...
 // SURVEY.md section 8b) is inherited from the reference. test/mulls_slam.cpp:360-377, :1008-1009 and
 // test/mulls_reg.cpp:134-145 compile unchanged.
 #ifndef MULLS_B200_DROPIN_CFILTER_HPP
@@ -66,6 +68,39 @@ class CFilter : public CFilter_reference<PointT> {
         return b200::sor_filter<PointT>(cloud_in, cloud_out, mean_k, n_std);
     }
     bool sor_filter(CloudPtr &cloud_in_out, int mean_k, double n_std) { return b200::sor_filter<PointT>(cloud_in_out, mean_k, n_std); }
+    // cfilter.hpp:250 (test/mulls_slam.cpp:362, :407, :967)
+    bool vertical_intrinsic_calibration(CloudPtr &cloud_in_out, double var_vertical_ang_d = 0.0, bool inverse_z = false) {
+        return b200::vertical_intrinsic_calibration<PointT>(cloud_in_out, var_vertical_ang_d, inverse_z);
+    }
+    // cfilter.hpp:412 (test/mulls_slam.cpp:410-412, :972-974)
+    bool get_pts_timestamp_ratio_in_frame(CloudPtr &cloud_in_out, bool timestamp_availiable = true,
+                                          double scan_begin_ang_anticlock_x_positive_deg = 180.0, float scan_duration_ms = 100) {
+        return b200::get_pts_timestamp_ratio_in_frame<PointT>(cloud_in_out, timestamp_availiable,
+                                                              scan_begin_ang_anticlock_x_positive_deg, scan_duration_ms);
+    }
+    // cfilter.hpp:470 and :493 (test/mulls_slam.cpp:707, :980, :1001). Both overloads: declaring one hides the other.
+    void apply_motion_compensation(CloudPtr pc_in_out, Eigen::Matrix4d &Tran, float s_ambigous_thre = 0.000) {
+        b200::apply_motion_compensation<PointT>(pc_in_out, Tran, s_ambigous_thre);
+    }
+    void apply_motion_compensation(const CloudPtr pc_in, CloudPtr pc_out, Eigen::Matrix4d &Tran, float s_ambigous_thre = 0.0) {
+        b200::apply_motion_compensation<PointT>(pc_in, pc_out, Tran, s_ambigous_thre);
+    }
+    // cfilter.hpp:519 and :534 (test/mulls_slam.cpp:708-711): the five or six clouds in one device call
+    void batch_apply_motion_compensation(CloudPtr pc_ground, CloudPtr pc_pillar, CloudPtr pc_beam, CloudPtr pc_facade, CloudPtr pc_roof,
+                                         CloudPtr pc_vertex, Eigen::Matrix4d &Tran, bool undistort_keypoints_or_not = false) {
+        b200::batch_apply_motion_compensation<PointT>(pc_ground, pc_pillar, pc_beam, pc_facade, pc_roof, pc_vertex, Tran,
+                                                      undistort_keypoints_or_not);
+    }
+    void batch_apply_motion_compensation(const CloudPtr pc_ground, const CloudPtr pc_pillar, const CloudPtr pc_beam,
+                                         const CloudPtr pc_facade, const CloudPtr pc_roof, const CloudPtr pc_vertex,
+                                         CloudPtr pc_ground_undistort, CloudPtr pc_pillar_undistort, CloudPtr pc_beam_undistort,
+                                         CloudPtr pc_facade_undistort, CloudPtr pc_roof_undistort, CloudPtr pc_vertex_undistort,
+                                         Eigen::Matrix4d &Tran, bool undistort_keypoints_or_not = false) {
+        b200::batch_apply_motion_compensation<PointT>(pc_ground, pc_pillar, pc_beam, pc_facade, pc_roof, pc_vertex,
+                                                      pc_ground_undistort, pc_pillar_undistort, pc_beam_undistort,
+                                                      pc_facade_undistort, pc_roof_undistort, pc_vertex_undistort, Tran,
+                                                      undistort_keypoints_or_not);
+    }
 };
 
 } // namespace lo

@@ -32,6 +32,10 @@
  *   mulls_voxel_downsample   <- lo::CFilter<PointT>::voxel_downsample, include/common/cfilter.hpp:83-165
  *   mulls_extract_semantic_pts <- lo::CFilter<PointT>::extract_semantic_pts, include/common/cfilter.hpp:2295-2413
  *   mulls_sor_filter         <- lo::CFilter<PointT>::sor_filter, include/common/cfilter.hpp:203-247
+ *   mulls_vertical_intrinsic_calibration <- lo::CFilter<PointT>::vertical_intrinsic_calibration, cfilter.hpp:250-291
+ *   mulls_timestamp_ratio    <- lo::CFilter<PointT>::get_pts_timestamp_ratio_in_frame, cfilter.hpp:412-467
+ *   mulls_motion_compensation <- lo::CFilter<PointT>::apply_motion_compensation / batch_apply_motion_compensation,
+ *                               cfilter.hpp:470-549
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
  *
@@ -470,6 +474,45 @@ typedef struct mulls_sor_stats {
 int mulls_sor_filter(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double n_std,
                      uint8_t *keep_bits /* [(n+7)/8] */, float *mean_dist /* [n] or NULL */,
                      mulls_sor_stats *stats /* or NULL */);
+
+/* ---- Raw-scan corrections: the CFilter members test/mulls_slam.cpp runs on every raw scan (:406-412, :707-711,
+ * :967-980). Each call is stateless: the rows go to the device, the column the member changes comes back, nothing stays
+ * resident and the batch resident on the context is left alone. No multiply-add is contracted. A cloud (or, for
+ * mulls_motion_compensation, the clouds together) of more than the context's max_tgt_pts points: MULLS_E_CAPACITY. A NULL
+ * pointer where points are to be read or written: MULLS_E_ARG. An empty cloud does no device work. */
+
+/* vertical_intrinsic_calibration(cloud, var_vertical_ang_d, inverse_z), cfilter.hpp:250-291. xyz_out [n][3] receives the
+ * coordinates the member leaves, *applied what it returns:
+ *   - var_vertical_ang_d == 0: the input's coordinates, *applied = 0 (no device work)
+ *   - var_vertical_ang_d >= 180 or inverse_z: z negated, *applied = 0
+ *   - otherwise dist = (double)sqrtf(x*x + y*y + z*z) (float products and sum), v = asin(z / dist), v_c = v + var
+ *     (radians), x and y times cos(v_c) / cos(v), z = dist * sin(v_c), all in double, stored as float; *applied = 1.
+ *     A point at the origin becomes NaN, as in the reference.
+ * asin / cos / sin are CUDA's double functions, not the host's libm: a coordinate can differ from the host's in its
+ * last float bit. */
+int mulls_vertical_intrinsic_calibration(mulls_ctx *ctx, mulls_cloud_view cloud, double var_vertical_ang_d, int inverse_z,
+                                         float *xyz_out /* [n][3] */, int *applied);
+
+/* get_pts_timestamp_ratio_in_frame(cloud, timestamp_available, scan_begin_ang_deg, scan_duration_ms), cfilter.hpp:412-467:
+ * ratio_out [n] receives the new curvature column (the member always returns true).
+ *   - timestamp_available: last / first = the running max_ / min_ macros (utility.hpp:31-32) over the curvature column
+ *     in input order — a NaN timestamp resets both, so they are the extremes of the points after the last NaN (NaN when
+ *     the last point is NaN); if last - first < 0.75 * scan_duration_ms it becomes the (float) duration; ratio =
+ *     min_(1.0, max_(0.0, (last - curvature) / duration)) in double. Equal timestamps give 0 / 0 = NaN, as in the
+ *     reference. Bit-exact.
+ *   - otherwise: the float atan2(y, x), widened; + 2 pi when negative; + the begin angle; - 2 pi when >= 2 pi; ratio =
+ *     (2 pi - angle) / (2 pi), in double. The float atan2 is computed as the double one rounded to float. */
+int mulls_timestamp_ratio(mulls_ctx *ctx, mulls_cloud_view cloud, int timestamp_available, double scan_begin_ang_deg,
+                          float scan_duration_ms, float *ratio_out /* [n] */);
+
+/* apply_motion_compensation(cloud, T, s_ambiguous_thre), cfilter.hpp:470-516, over n_clouds (1..6) clouds in one upload
+ * and one launch: one cloud for apply_motion_compensation, five or six for batch_apply_motion_compensation (:519-549).
+ * q = Eigen::Quaterniond(T's rotation), computed once on the host; a point whose curvature s (the timestamp ratio) is
+ * < s_ambiguous_thre or > 1.0 - s_ambiguous_thre keeps its coordinates, every other point becomes
+ * Identity().slerp(s, q) * p + s * t in double, stored as float. xyz_out[c] [clouds[c].n][3] receives cloud c's
+ * coordinates. n_clouds outside 1..6: MULLS_E_ARG. */
+int mulls_motion_compensation(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, const double T[16] /* row-major */,
+                              float s_ambiguous_thre, float *const *xyz_out);
 
 /* The wire format the library ships host clouds in when the "host_pack" tunable is on (csrc/host_pack.h): the 28 of the
  * 48 bytes of a pcl::PointXYZINormal row (utility.hpp:40) that the path reads, repacked on the host cores into pinned

@@ -284,6 +284,9 @@ EXPORTED_SYMBOLS = (
     "mulls_voxel_downsample",
     "mulls_extract_semantic_pts",
     "mulls_sor_filter",
+    "mulls_vertical_intrinsic_calibration",
+    "mulls_timestamp_ratio",
+    "mulls_motion_compensation",
     "mulls_scan_probe",
     "mulls_scan_read",
     "mulls_pose_write",
@@ -353,6 +356,14 @@ def load_library() -> C.CDLL:
     lib.mulls_sor_filter.restype = C.c_int
     lib.mulls_sor_filter.argtypes = [vp, CloudView, C.c_int, C.c_double, C.POINTER(C.c_uint8), C.POINTER(C.c_float),
                                      C.POINTER(SorStats)]
+    lib.mulls_vertical_intrinsic_calibration.restype = C.c_int
+    lib.mulls_vertical_intrinsic_calibration.argtypes = [vp, CloudView, C.c_double, C.c_int, C.POINTER(C.c_float),
+                                                         C.POINTER(C.c_int)]
+    lib.mulls_timestamp_ratio.restype = C.c_int
+    lib.mulls_timestamp_ratio.argtypes = [vp, CloudView, C.c_int, C.c_double, C.c_float, C.POINTER(C.c_float)]
+    lib.mulls_motion_compensation.restype = C.c_int
+    lib.mulls_motion_compensation.argtypes = [vp, C.POINTER(CloudView), C.c_int, C.POINTER(C.c_double), C.c_float,
+                                              C.POINTER(C.POINTER(C.c_float))]
     lib.mulls_pack_rows.restype = C.c_int
     lib.mulls_pack_rows.argtypes = [C.POINTER(C.c_float), C.c_size_t, C.c_int, C.POINTER(C.c_float)]
     lib.mulls_scan_probe.restype = C.c_int

@@ -37,6 +37,38 @@ __device__ __forceinline__ float weight_by_residual(float res, float huber_thre)
     return 1.0f;
 }
 
+// cfilter.hpp:470-516 apply_motion_compensation, one point: p <- slerp(Identity, q, s) * p + s * t with s = the point's
+// timestamp ratio `curv` (widened) — Eigen's QuaternionBase::slerp from the identity (d = q.w: the `absD >= 1 - eps`
+// linear branch and the `d < 0` sign flip, constants from the host: linear, neg, theta = acos|d|, sin theta), then
+// Eigen's quaternion-vector product, in double, stored as float. A point with curv < thre or curv > 1.0 - thre is left
+// as it is (false). The ingest's undistortion (thre 0) and k_motion_compensation both run this text.
+// The constants are taken by reference: each is read where the reference's text reads it.
+MULLS_HD bool slerp_compensate(const double *q, const double *t, const int &linear, const int &neg, const double &theta,
+                               const double &sin_theta, float thre, float curv, float &x, float &y, float &z) {
+    if (curv < thre || (double)curv > 1.0 - (double)thre) return false;
+    const double s = (double)curv;
+    double scale0, scale1;
+    if (linear) {
+        scale0 = 1.0 - s;
+        scale1 = s;
+    } else {
+        scale0 = sin((1.0 - s) * theta) / sin_theta;
+        scale1 = sin(s * theta) / sin_theta;
+    }
+    if (neg) scale1 = -scale1;
+    const double qx = scale1 * q[0], qy = scale1 * q[1], qz = scale1 * q[2], qw = scale0 + scale1 * q[3];
+    const double vx = x, vy = y, vz = z;
+    double ux = qy * vz - qz * vy, uy = qz * vx - qx * vz, uz = qx * vy - qy * vx;
+    ux += ux, uy += uy, uz += uz;
+    const double rx = vx + qw * ux + (qy * uz - qz * uy);
+    const double ry = vy + qw * uy + (qz * ux - qx * uz);
+    const double rz = vz + qw * uz + (qx * uy - qy * ux);
+    x = (float)(rx + s * t[0]);
+    y = (float)(ry + s * t[1]);
+    z = (float)(rz + s * t[2]);
+    return true;
+}
+
 // 6x6 inverse by partial-pivot LU + identity solve (Eigen::PartialPivLU::inverse, Appendix B.9).
 // Executed by ONE thread on shared-memory matrices (dynamic indexing), ~1.5k flops.
 __device__ inline void inverse6(const double *A /*36 row-major*/, double *out /*36*/, double *lu /*36 scratch*/) {

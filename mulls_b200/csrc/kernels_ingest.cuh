@@ -56,31 +56,8 @@ __device__ __forceinline__ void load_input_point(const PairConst &pc, uint32_t s
         if (kUndistort && pc.undistort) {
             if (cls == MULLS_VERTEX) {
                 n_apply = 2; // not undistorted and not re-cloned: the initial guess lands twice (reference behaviour)
-            } else {
-                const float curv = curvature; // timestamp ratio of the point inside its frame
-                if (!(curv < 0.0f || (double)curv > 1.0)) {
-                    const double s = (double)curv;
-                    double scale0, scale1;
-                    if (pc.ud_linear) {
-                        scale0 = 1.0 - s;
-                        scale1 = s;
-                    } else {
-                        scale0 = sin((1.0 - s) * pc.ud_theta) / pc.ud_sin_theta;
-                        scale1 = sin(s * pc.ud_theta) / pc.ud_sin_theta;
-                    }
-                    if (pc.ud_neg) scale1 = -scale1;
-                    const double qx = scale1 * pc.ud_q[0], qy = scale1 * pc.ud_q[1], qz = scale1 * pc.ud_q[2],
-                                 qw = scale0 + scale1 * pc.ud_q[3];
-                    const double vx = x, vy = y, vz = z;
-                    double ux = qy * vz - qz * vy, uy = qz * vx - qx * vz, uz = qx * vy - qy * vx;
-                    ux += ux, uy += uy, uz += uz;
-                    const double rx = vx + qw * ux + (qy * uz - qz * uy);
-                    const double ry = vy + qw * uy + (qz * ux - qx * uz);
-                    const double rz = vz + qw * uz + (qx * uy - qy * ux);
-                    x = (float)(rx + s * pc.ud_t[0]);
-                    y = (float)(ry + s * pc.ud_t[1]);
-                    z = (float)(rz + s * pc.ud_t[2]);
-                }
+            } else { // curvature: the timestamp ratio of the point inside its frame
+                slerp_compensate(pc.ud_q, pc.ud_t, pc.ud_linear, pc.ud_neg, pc.ud_theta, pc.ud_sin_theta, 0.0f, curvature, x, y, z);
             }
         }
         for (int rep = 0; rep < n_apply; ++rep) {

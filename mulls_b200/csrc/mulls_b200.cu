@@ -26,6 +26,7 @@
 #include "kernels_classify.cuh"
 #include "kernels_ground.cuh"
 #include "kernels_sor.cuh"
+#include "kernels_rawscan.cuh"
 
 using namespace mulls;
 
@@ -151,6 +152,7 @@ struct mulls_ctx {
     Scratch gf_buf, gf_cell_buf; // ground filter (mulls_fast_ground_filter): per-point part and per-cell part
     Scratch vx_buf, ext_buf;     // voxel filter; clouds handed between the stages of extract_semantic_pts
     Scratch sor_buf;             // statistical outlier filter: mean distances, keep mask, statistics
+    Scratch raw_buf;             // raw-scan corrections: the rows of the call, the column it returns, timestamp state
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
     const mulls_map *tree_map = nullptr;
@@ -231,7 +233,7 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (void *p : ctx->allocs) cudaFree(p);
     if (ctx->cub_temp) cudaFree(ctx->cub_temp);
-    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf})
+    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf})
         if (s->p) cudaFree(s->p);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
     if (ctx->h_flags) cudaFreeHost(ctx->h_flags);
@@ -437,9 +439,43 @@ int mulls_get_stats(const mulls_ctx *ctx, mulls_run_stats *out) {
     return MULLS_OK;
 }
 
-// Inverse of the initial guess (Eigen Matrix4d::inverse: cofactors / determinant), its quaternion
-// (Eigen::Quaterniond(Matrix3d)) and the per-pair constants of Eigen's slerp(Identity -> q)
-// (cregistration.hpp:1248, cfilter.hpp:499-502).
+// Eigen::Quaterniond(T.block<3,3>(0,0)) of a row-major 4x4, its translation and the constants of Eigen's
+// slerp(Identity -> q): d = q.w, linear when |d| >= 1 - eps, neg when d < 0, theta = acos|d| (cfilter.hpp:472-475)
+static SlerpConst slerp_const_of(const double *T) {
+    SlerpConst sc;
+    double *q = sc.q; // x y z w
+    double t = T[0] + T[5] + T[10];
+    if (t > 0.0) {
+        t = std::sqrt(t + 1.0);
+        q[3] = 0.5 * t;
+        t = 0.5 / t;
+        q[0] = (T[9] - T[6]) * t;
+        q[1] = (T[2] - T[8]) * t;
+        q[2] = (T[4] - T[1]) * t;
+    } else {
+        int i = 0;
+        if (T[5] > T[0]) i = 1;
+        if (T[10] > T[5 * i]) i = 2;
+        const int j = (i + 1) % 3, k = (j + 1) % 3;
+        t = std::sqrt(T[5 * i] - T[5 * j] - T[5 * k] + 1.0);
+        q[i] = 0.5 * t;
+        t = 0.5 / t;
+        q[3] = (T[4 * k + j] - T[4 * j + k]) * t;
+        q[j] = (T[4 * j + i] + T[4 * i + j]) * t;
+        q[k] = (T[4 * k + i] + T[4 * i + k]) * t;
+    }
+    sc.t[0] = T[3], sc.t[1] = T[7], sc.t[2] = T[11];
+    const double one = 1.0 - 2.220446049250313e-16;
+    const double d = q[3], absD = std::fabs(d);
+    sc.linear = (absD >= one) ? 1 : 0;
+    sc.neg = (d < 0) ? 1 : 0;
+    sc.theta = sc.linear ? 0.0 : std::acos(absD);
+    sc.sin_theta = sc.linear ? 1.0 : std::sin(sc.theta);
+    return sc;
+}
+
+// Inverse of the initial guess (Eigen Matrix4d::inverse: cofactors / determinant) and the slerp constants of its
+// rotation (cregistration.hpp:1248, cfilter.hpp:499-502).
 static void setup_undistortion(const double *m, PairConst &pc) {
     double inv[16];
     inv[0] = m[5] * m[10] * m[15] - m[5] * m[11] * m[14] - m[9] * m[6] * m[15] + m[9] * m[7] * m[14] + m[13] * m[6] * m[11] - m[13] * m[7] * m[10];
@@ -461,35 +497,13 @@ static void setup_undistortion(const double *m, PairConst &pc) {
     const double det = m[0] * inv[0] + m[1] * inv[4] + m[2] * inv[8] + m[3] * inv[12];
     double T[16];
     for (int i = 0; i < 16; ++i) T[i] = inv[i] * (1.0 / det);
-    double q[4]; // x y z w
-    double t = T[0] + T[5] + T[10];
-    if (t > 0.0) {
-        t = std::sqrt(t + 1.0);
-        q[3] = 0.5 * t;
-        t = 0.5 / t;
-        q[0] = (T[9] - T[6]) * t;
-        q[1] = (T[2] - T[8]) * t;
-        q[2] = (T[4] - T[1]) * t;
-    } else {
-        int i = 0;
-        if (T[5] > T[0]) i = 1;
-        if (T[10] > T[5 * i]) i = 2;
-        const int j = (i + 1) % 3, k = (j + 1) % 3;
-        t = std::sqrt(T[5 * i] - T[5 * j] - T[5 * k] + 1.0);
-        q[i] = 0.5 * t;
-        t = 0.5 / t;
-        q[3] = (T[4 * k + j] - T[4 * j + k]) * t;
-        q[j] = (T[4 * j + i] + T[4 * i + j]) * t;
-        q[k] = (T[4 * k + i] + T[4 * i + k]) * t;
-    }
-    for (int i = 0; i < 4; ++i) pc.ud_q[i] = q[i];
-    pc.ud_t[0] = T[3], pc.ud_t[1] = T[7], pc.ud_t[2] = T[11];
-    const double one = 1.0 - 2.220446049250313e-16;
-    const double d = q[3], absD = std::fabs(d);
-    pc.ud_linear = (absD >= one) ? 1 : 0;
-    pc.ud_neg = (d < 0) ? 1 : 0;
-    pc.ud_theta = pc.ud_linear ? 0.0 : std::acos(absD);
-    pc.ud_sin_theta = pc.ud_linear ? 1.0 : std::sin(pc.ud_theta);
+    const SlerpConst sc = slerp_const_of(T);
+    for (int i = 0; i < 4; ++i) pc.ud_q[i] = sc.q[i];
+    for (int i = 0; i < 3; ++i) pc.ud_t[i] = sc.t[i];
+    pc.ud_linear = sc.linear;
+    pc.ud_neg = sc.neg;
+    pc.ud_theta = sc.theta;
+    pc.ud_sin_theta = sc.sin_theta;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1463,6 +1477,141 @@ int mulls_sor_filter(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double 
     // an error exit may leave the copy of the caller's cloud in flight: nothing is handed back before the stream drains
     if (rc != MULLS_OK && ctx && ctx->stream) cudaStreamSynchronize(ctx->stream);
     return rc;
+}
+
+// ================================================================================================
+// Raw-scan corrections (CFilter::vertical_intrinsic_calibration, get_pts_timestamp_ratio_in_frame,
+// apply_motion_compensation, cfilter.hpp:250-291, :412-549): kernels_rawscan.cuh. Stateless: the rows go up, the changed
+// column comes back, nothing stays resident.
+// ================================================================================================
+// raw_buf = [rows of the call, 48 B each][out_floats per point][TsState]; the rows of the n_clouds clouds are copied
+// one after the other
+static int raw_upload(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, size_t n_total, int out_floats,
+                      float **d_rows, float **d_out, TsState **d_st) {
+    const size_t off_out = n_total * 48, off_st = off_out + ceil_div(n_total * out_floats * sizeof(float), 16) * 16;
+    int rc = grow_scratch(ctx, ctx->raw_buf, off_st + sizeof(TsState));
+    if (rc != MULLS_OK) return rc;
+    char *base = (char *)ctx->raw_buf.p;
+    *d_rows = (float *)base, *d_out = (float *)(base + off_out), *d_st = (TsState *)(base + off_st);
+    size_t at = 0;
+    for (int c = 0; c < n_clouds; ++c) {
+        if (clouds[c].n) CK(cudaMemcpyAsync(base + at * 48, clouds[c].aos48, clouds[c].n * 48, cudaMemcpyHostToDevice, ctx->stream));
+        at += clouds[c].n;
+    }
+    return MULLS_OK;
+}
+
+static int raw_capacity(mulls_ctx *ctx, size_t n, const char *fn) {
+    if (n <= ctx->max_tgt) return MULLS_OK;
+    ctx->err = std::string(fn) + ": " + std::to_string(n) + " points exceed max_tgt_pts of the context";
+    return MULLS_E_CAPACITY;
+}
+
+static int raw_finish(mulls_ctx *ctx, uint64_t launches) {
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->stats = mulls_run_stats();
+    ctx->stats.kernel_launches = launches;
+    return MULLS_OK;
+}
+
+static int vertical_calib_impl(mulls_ctx *ctx, mulls_cloud_view cloud, double var_vertical_ang_d, int inverse_z, float *xyz_out,
+                               int *applied) {
+    if (!ctx || !applied || (cloud.n > 0 && (!cloud.aos48 || !xyz_out))) return MULLS_E_ARG;
+    int rc = raw_capacity(ctx, cloud.n, "mulls_vertical_intrinsic_calibration");
+    if (rc != MULLS_OK) return rc;
+    *applied = 0;
+    if (var_vertical_ang_d == 0) { // :252-253: the cloud is left as it is
+        for (size_t i = 0; i < cloud.n; ++i)
+            for (int d = 0; d < 3; ++d) xyz_out[3 * i + d] = cloud.aos48[12 * i + d];
+        return MULLS_OK;
+    }
+    const int negate_only = (var_vertical_ang_d >= 180.0 || inverse_z) ? 1 : 0; // :255-263
+    if (cloud.n > 0) {
+        float *d_rows, *d_out;
+        TsState *d_st;
+        if ((rc = raw_upload(ctx, &cloud, 1, cloud.n, 3, &d_rows, &d_out, &d_st)) != MULLS_OK) return rc;
+        const double var_rad = var_vertical_ang_d / 180.0 * M_PI;
+        k_vertical_calib<<<(unsigned)ceil_div(cloud.n, kRawBlock), kRawBlock, 0, ctx->stream>>>(d_rows, (uint32_t)cloud.n, var_rad,
+                                                                                                negate_only, d_out);
+        CK(cudaMemcpyAsync(xyz_out, d_out, cloud.n * 3 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+        if ((rc = raw_finish(ctx, 1)) != MULLS_OK) return rc;
+    }
+    *applied = negate_only ? 0 : 1;
+    return MULLS_OK;
+}
+
+static int timestamp_ratio_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int timestamp_available, double scan_begin_ang_deg,
+                                float scan_duration_ms, float *ratio_out) {
+    if (!ctx || (cloud.n > 0 && (!cloud.aos48 || !ratio_out))) return MULLS_E_ARG;
+    int rc = raw_capacity(ctx, cloud.n, "mulls_timestamp_ratio");
+    if (rc != MULLS_OK) return rc;
+    const size_t n = cloud.n;
+    if (n == 0) return MULLS_OK;
+    float *d_rows, *d_out;
+    TsState *d_st;
+    if ((rc = raw_upload(ctx, &cloud, 1, n, 1, &d_rows, &d_out, &d_st)) != MULLS_OK) return rc;
+    const unsigned nb = (unsigned)ceil_div(n, kRawBlock);
+    cudaStream_t st = ctx->stream;
+    uint64_t launches = 0;
+    if (timestamp_available) {
+        TsState init{};
+        init.min_key = ~0ull;
+        CK(cudaMemcpyAsync(d_st, &init, sizeof(init), cudaMemcpyHostToDevice, st));
+        k_ts_last_nan<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st);
+        k_ts_extremes<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st);
+        k_ts_setup<<<1, 32, 0, st>>>(d_rows, (uint32_t)n, scan_duration_ms, d_st);
+        k_ts_ratio<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st, d_out);
+        launches = 4;
+    } else {
+        k_azimuth_ratio<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, scan_begin_ang_deg / 180.0 * M_PI, d_out);
+        launches = 1;
+    }
+    CK(cudaMemcpyAsync(ratio_out, d_out, n * sizeof(float), cudaMemcpyDeviceToHost, st));
+    return raw_finish(ctx, launches);
+}
+
+static int motion_compensation_impl(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, const double *T,
+                                    float s_ambiguous_thre, float *const *xyz_out) {
+    if (!ctx || !clouds || !T || !xyz_out || n_clouds < 1 || n_clouds > MULLS_NUM_CLASSES) return MULLS_E_ARG;
+    size_t n = 0;
+    for (int c = 0; c < n_clouds; ++c) {
+        if (clouds[c].n > 0 && (!clouds[c].aos48 || !xyz_out[c])) return MULLS_E_ARG;
+        n += clouds[c].n;
+    }
+    int rc = raw_capacity(ctx, n, "mulls_motion_compensation");
+    if (rc != MULLS_OK || n == 0) return rc;
+    float *d_rows, *d_out;
+    TsState *d_st;
+    if ((rc = raw_upload(ctx, clouds, n_clouds, n, 3, &d_rows, &d_out, &d_st)) != MULLS_OK) return rc;
+    const SlerpConst sc = slerp_const_of(T);
+    k_motion_compensation<<<(unsigned)ceil_div(n, kRawBlock), kRawBlock, 0, ctx->stream>>>(d_rows, (uint32_t)n, sc, s_ambiguous_thre,
+                                                                                           d_out);
+    size_t at = 0;
+    for (int c = 0; c < n_clouds; ++c) {
+        if (clouds[c].n)
+            CK(cudaMemcpyAsync(xyz_out[c], d_out + 3 * at, clouds[c].n * 3 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+        at += clouds[c].n;
+    }
+    return raw_finish(ctx, 1);
+}
+
+// an error exit may leave a copy in flight: nothing is handed back before the stream drains
+static int raw_drain(mulls_ctx *ctx, int rc) {
+    if (rc != MULLS_OK && ctx && ctx->stream) cudaStreamSynchronize(ctx->stream);
+    return rc;
+}
+int mulls_vertical_intrinsic_calibration(mulls_ctx *ctx, mulls_cloud_view cloud, double var_vertical_ang_d, int inverse_z,
+                                         float *xyz_out, int *applied) {
+    return raw_drain(ctx, vertical_calib_impl(ctx, cloud, var_vertical_ang_d, inverse_z, xyz_out, applied));
+}
+int mulls_timestamp_ratio(mulls_ctx *ctx, mulls_cloud_view cloud, int timestamp_available, double scan_begin_ang_deg,
+                          float scan_duration_ms, float *ratio_out) {
+    return raw_drain(ctx, timestamp_ratio_impl(ctx, cloud, timestamp_available, scan_begin_ang_deg, scan_duration_ms, ratio_out));
+}
+int mulls_motion_compensation(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, const double T[16],
+                              float s_ambiguous_thre, float *const *xyz_out) {
+    return raw_drain(ctx, motion_compensation_impl(ctx, clouds, n_clouds, T, s_ambiguous_thre, xyz_out));
 }
 
 // ================================================================================================

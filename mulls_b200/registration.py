@@ -293,6 +293,43 @@ class Context:
         keep = np.unpackbits(bits, bitorder="little")[:n].astype(bool)
         return keep, dist[:n], {k: getattr(st, k) for k, _ in abi.SorStats._fields_}
 
+    def vertical_intrinsic_calibration(self, cloud: np.ndarray, var_vertical_ang_d: float, inverse_z: bool = False):
+        """CFilter::vertical_intrinsic_calibration (cfilter.hpp:250-291) on the GPU. Returns (xyz: float32[n, 3], the
+        member's return value)."""
+        c = abi.as_aos48(cloud)
+        xyz = np.zeros((max(len(c), 1), 3), np.float32)
+        applied = C.c_int(0)
+        self._check(self.lib.mulls_vertical_intrinsic_calibration(self.handle, abi.cloud_view(c), float(var_vertical_ang_d),
+                                                                  int(bool(inverse_z)), xyz.ctypes.data_as(C.POINTER(C.c_float)),
+                                                                  C.byref(applied)))
+        return xyz[: len(c)], bool(applied.value)
+
+    def timestamp_ratio(self, cloud: np.ndarray, timestamp_available: bool = True, scan_begin_ang_deg: float = 180.0,
+                        scan_duration_ms: float = 100.0) -> np.ndarray:
+        """CFilter::get_pts_timestamp_ratio_in_frame (cfilter.hpp:412-467) on the GPU: the new curvature column, float32[n]."""
+        c = abi.as_aos48(cloud)
+        ratio = np.zeros(max(len(c), 1), np.float32)
+        self._check(self.lib.mulls_timestamp_ratio(self.handle, abi.cloud_view(c), int(bool(timestamp_available)),
+                                                   float(scan_begin_ang_deg), float(scan_duration_ms),
+                                                   ratio.ctypes.data_as(C.POINTER(C.c_float))))
+        return ratio[: len(c)]
+
+    def motion_compensation(self, clouds, T, s_ambiguous_thre: float = 0.0):
+        """CFilter::apply_motion_compensation (cfilter.hpp:470-516) on the GPU for 1..6 clouds in one call (as
+        batch_apply_motion_compensation :519-549). `clouds`: one (n, 12) array or a list of them; T: 4x4. Returns the new
+        xyz (float32[n, 3]) of each cloud, in the same form."""
+        single = isinstance(clouds, np.ndarray)
+        cl = [abi.as_aos48(c) for c in ([clouds] if single else clouds)]
+        views = (abi.CloudView * max(len(cl), 1))(*[abi.cloud_view(c) for c in cl])
+        outs = [np.zeros((max(len(c), 1), 3), np.float32) for c in cl]
+        fp = C.POINTER(C.c_float)
+        ptrs = (fp * max(len(cl), 1))(*[o.ctypes.data_as(fp) for o in outs])
+        Td = np.ascontiguousarray(np.asarray(T, np.float64).reshape(16))
+        self._check(self.lib.mulls_motion_compensation(self.handle, views, len(cl), Td.ctypes.data_as(C.POINTER(C.c_double)),
+                                                       float(s_ambiguous_thre), ptrs))
+        res = [o[: len(c)] for o, c in zip(outs, cl)]
+        return res[0] if single else res
+
     def stats(self) -> dict:
         s = abi.RunStats()
         self._check(self.lib.mulls_get_stats(self.handle, C.byref(s)))
