@@ -218,6 +218,39 @@ bool mm_lls_icp_4dof_global(constraint_t &registration_con, float heading_step_d
     return successful_reg;
 }
 
+// lo::CRegistration<PointT>::find_feature_correspondence_ncc (cregistration.hpp:409-601), same arguments and defaults
+// (test/mulls_reg.cpp:173-174, test/mulls_slam.cpp:534-535): the keypoint matching runs on the device
+// (mulls_ncc_correspondences, readings in abi.h); the matched rows are appended to the output clouds here, as the
+// reference appends them. Returns false where the reference does (fewer than 10 keypoints in a cloud). A library error
+// is logged and also returns false, with both output clouds left as they were.
+template <typename PointT>
+bool find_feature_correspondence_ncc(const typename pcl::PointCloud<PointT>::Ptr &target_kpts,
+                                     const typename pcl::PointCloud<PointT>::Ptr &source_kpts,
+                                     typename pcl::PointCloud<PointT>::Ptr &target_corrs,
+                                     typename pcl::PointCloud<PointT>::Ptr &source_corrs, bool fixed_num_corr = false,
+                                     int corr_num = 2000, bool reciprocal_on = true) {
+    const size_t nt = target_kpts->points.size(), ns = source_kpts->points.size();
+    const size_t cap = fixed_num_corr ? 7 * (nt < ns ? nt : ns) : nt; // at most 7 pairs per keypoint / one per target row
+    std::vector<int32_t> ti(cap ? cap : 1), si(cap ? cap : 1);
+    size_t n = 0;
+    int performed = 0;
+    mulls_ctx *ctx = thread_context(0, nt > ns ? nt : ns);
+    if (!ctx || mulls_ncc_correspondences(ctx, view_of<PointT>(target_kpts), view_of<PointT>(source_kpts), fixed_num_corr ? 1 : 0,
+                                          corr_num, reciprocal_on ? 1 : 0, ti.data(), si.data(), cap, &n, &performed) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return false;
+    }
+    if (!performed) {
+        LOG(WARNING) << "Too few key points\n"; // :423
+        return false;
+    }
+    for (size_t k = 0; k < n; ++k) {
+        target_corrs->points.push_back(target_kpts->points[ti[k]]);
+        source_corrs->points.push_back(source_kpts->points[si[k]]);
+    }
+    return true;
+}
+
 } // namespace b200
 } // namespace lo
 #endif

@@ -11,8 +11,9 @@
 //     CRegistration_reference — every member the reference defines stays available, unchanged;
 //   * lo::CRegistration<PointT> is then defined HERE as a class derived from it whose mm_lls_icp
 //     (cregistration.hpp:1114-1123: same name, argument order, types and defaults) and mm_lls_icp_4dof_global
-//     (:1584-1592) run on the GPU through the C-ABI (include/mulls_b200/abi.h). All other public members the callers use
-//     — determine_source_target_cloud, assign_source_target_cloud, find_feature_correspondence_ncc, coarse_reg_teaser,
+//     (:1584-1592) and find_feature_correspondence_ncc (:409-411) run on the GPU through the C-ABI
+//     (include/mulls_b200/abi.h). All other public members the callers use
+//     — determine_source_target_cloud, assign_source_target_cloud, coarse_reg_teaser,
 //     coarse_reg_ransac, omp_ndt, omp_gicp, ... (SURVEY.md section 8b) — are inherited from the reference.
 // Differences in contract are listed in INTEGRATION.md (block1->tree_* are not populated: use mulls_nn_query or
 // the drop-in lo::MapManager of dropin/map_manager.h, which does not need them).
@@ -65,6 +66,15 @@ class CRegistration : public CRegistration_reference<PointT> {
                                 float dis_thre_update_rate = 1.05, float max_bearable_rotation_d = 15.0) {
         return b200::mm_lls_icp_4dof_global<PointT>(registration_con, heading_step_d, max_iter_num, dis_thre_unit, converge_translation,
                                                     converge_rotation_d, dis_thre_min, dis_thre_update_rate, max_bearable_rotation_d);
+    }
+    // cregistration.hpp:409-411
+    bool find_feature_correspondence_ncc(const typename pcl::PointCloud<PointT>::Ptr &target_kpts,
+                                         const typename pcl::PointCloud<PointT>::Ptr &source_kpts,
+                                         typename pcl::PointCloud<PointT>::Ptr &target_corrs,
+                                         typename pcl::PointCloud<PointT>::Ptr &source_corrs, bool fixed_num_corr = false,
+                                         int corr_num = 2000, bool reciprocal_on = true) {
+        return b200::find_feature_correspondence_ncc<PointT>(target_kpts, source_kpts, target_corrs, source_corrs, fixed_num_corr,
+                                                             corr_num, reciprocal_on);
     }
 };
 

@@ -36,6 +36,7 @@
  *   mulls_timestamp_ratio    <- lo::CFilter<PointT>::get_pts_timestamp_ratio_in_frame, cfilter.hpp:412-467
  *   mulls_motion_compensation <- lo::CFilter<PointT>::apply_motion_compensation / batch_apply_motion_compensation,
  *                               cfilter.hpp:470-549
+ *   mulls_ncc_correspondences <- lo::CRegistration<PointT>::find_feature_correspondence_ncc, cregistration.hpp:409-601
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
  *
@@ -513,6 +514,35 @@ int mulls_timestamp_ratio(mulls_ctx *ctx, mulls_cloud_view cloud, int timestamp_
  * coordinates. n_clouds outside 1..6: MULLS_E_ARG. */
 int mulls_motion_compensation(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, const double T[16] /* row-major */,
                               float s_ambiguous_thre, float *const *xyz_out);
+
+/* lo::CRegistration<PointT>::find_feature_correspondence_ncc(target_kpts, source_kpts, target_corrs, source_corrs,
+ * fixed_num_corr, corr_num, reciprocal_on), cregistration.hpp:409-601: the keypoint matching in front of the global
+ * registration (test/mulls_reg.cpp:173-174, test/mulls_slam.cpp:534-535). Stateless like the raw-scan corrections: the
+ * batch resident on the context and its grid are left alone. The keypoints are 48-byte pcl::PointXYZINormal rows
+ * (x y z data[3] | normal_x normal_y normal_z normal[3] | intensity curvature _ _). tgt_idx[k] / src_idx[k] (k < *n_out)
+ * receive the row indices of the k-th correspondence in the order the reference appends them; the caller appends
+ * target_kpts[tgt_idx[k]] to target_corrs and source_kpts[src_idx[k]] to source_corrs.
+ *   - fewer than 10 keypoints in either cloud (:421-425): *performed = 0, *n_out = 0 (the reference returns false and
+ *     leaves both output clouds as they are); otherwise *performed = 1 (it returns true)
+ *   - intensity range over the target only, with max_ / min_ (utility.hpp:31-32) started from 0 and FLT_MAX (not
+ *     -FLT_MAX); a NaN intensity becomes the running value and the next point replaces it
+ *   - descriptor (11 floats): the decimal digit pairs of (int)normal[0] and (int)normal[1] (/1000000, %1000000/10000,
+ *     %10000/100, %100, C++ integer semantics), (i - min) / (max - min) in float times the double 255.0,
+ *     normal[3] * 100 and data[3] * 30 in float; (int) of a NaN or out-of-range float is INT_MIN, the x86-64 result. A
+ *     constant target intensity gives NaN / infinite components, as in the reference
+ *   - distance: the float L1 sum over the 11 components, in component order, no contraction
+ *   - plain mode (!fixed_num_corr, !reciprocal_on): per target i in order, the first j with d < best from (FLT_MAX, 0);
+ *     NaN never wins, a row without a finite value below FLT_MAX pairs with source 0
+ *   - reciprocal mode: the same, target i dropped when best_i > d[r][j_i] for some target r (the non-NaN column minimum)
+ *   - fixed-number mode (reciprocal_on ignored): K = min_(corr_num, n_t * n_s) compared as size_t (negative corr_num:
+ *     every pair, 0: none); the first K pairs in ascending distance, ties in pair-index order (i * n_s + j), NaN after
+ *     every number (std::sort leaves that order open); walked in order, a pair is skipped when its target or its source
+ *     already holds 7 kept pairs. n_t * n_s > INT_MAX (the reference's int pair index): MULLS_E_ARG
+ * A cloud of more than the context's max_tgt_pts keypoints: MULLS_E_CAPACITY. More correspondences than cap: MULLS_E_ARG,
+ * with nothing written. Indices are int32_t like the reference's int keypoint counts; NULL index arrays need cap == 0. */
+int mulls_ncc_correspondences(mulls_ctx *ctx, mulls_cloud_view target_kpts, mulls_cloud_view source_kpts, int fixed_num_corr,
+                              int corr_num, int reciprocal_on, int32_t *tgt_idx, int32_t *src_idx, size_t cap, size_t *n_out,
+                              int *performed);
 
 /* The wire format the library ships host clouds in when the "host_pack" tunable is on (csrc/host_pack.h): the 28 of the
  * 48 bytes of a pcl::PointXYZINormal row (utility.hpp:40) that the path reads, repacked on the host cores into pinned

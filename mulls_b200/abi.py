@@ -287,6 +287,7 @@ EXPORTED_SYMBOLS = (
     "mulls_vertical_intrinsic_calibration",
     "mulls_timestamp_ratio",
     "mulls_motion_compensation",
+    "mulls_ncc_correspondences",
     "mulls_scan_probe",
     "mulls_scan_read",
     "mulls_pose_write",
@@ -364,6 +365,9 @@ def load_library() -> C.CDLL:
     lib.mulls_motion_compensation.restype = C.c_int
     lib.mulls_motion_compensation.argtypes = [vp, C.POINTER(CloudView), C.c_int, C.POINTER(C.c_double), C.c_float,
                                               C.POINTER(C.POINTER(C.c_float))]
+    lib.mulls_ncc_correspondences.restype = C.c_int
+    lib.mulls_ncc_correspondences.argtypes = [vp, CloudView, CloudView, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32),
+                                              C.POINTER(C.c_int32), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int)]
     lib.mulls_pack_rows.restype = C.c_int
     lib.mulls_pack_rows.argtypes = [C.POINTER(C.c_float), C.c_size_t, C.c_int, C.POINTER(C.c_float)]
     lib.mulls_scan_probe.restype = C.c_int

@@ -59,7 +59,8 @@ __global__ void __launch_bounds__(kRawBlock) k_azimuth_ratio(const float *rows, 
 // DBL_MAX only when there is no NaN at all. Equal values (+0 and -0) resolve to the later point. Here: the last NaN
 // index, then the extremes of the suffix as 64-bit keys (order-preserving value bits with -0 read as +0 | point index;
 // the min key holds the complemented index), so that one atomicMax / atomicMin per block picks the value and, among
-// equal values, the latest point.
+// equal values, the latest point. The two reductions take the column they fold as a template parameter: 9 (curvature)
+// here, 8 (intensity) for the NCC intensity range of kernels_ncc.cuh, whose folds start from FLT_MAX / 0.
 struct TsState {
     unsigned long long last_nan;      // index + 1 of the last NaN timestamp, 0: none
     unsigned long long max_key, min_key;
@@ -73,19 +74,23 @@ __device__ __forceinline__ uint32_t ts_value_bits(float c) {
     return (uint32_t)o ^ 0x80000000u;
 }
 __device__ __forceinline__ float ts_curvature(const float *rows, size_t i) { return rows[12 * i + 9]; }
+template <int kCol>
+__device__ __forceinline__ float row_column(const float *rows, size_t i) { return rows[12 * i + kCol]; }
 
+template <int kCol>
 __global__ void __launch_bounds__(kRawBlock) k_ts_last_nan(const float *rows, uint32_t n, TsState *st) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned long long v = (i < n && isnan(ts_curvature(rows, i))) ? (unsigned long long)i + 1 : 0ull;
+    const unsigned long long v = (i < n && isnan(row_column<kCol>(rows, i))) ? (unsigned long long)i + 1 : 0ull;
     const unsigned long long m = __reduce_max_sync(0xffffffffu, (unsigned)v); // n < 2^32 - 1
     if ((threadIdx.x & 31) == 0 && m) atomicMax(&st->last_nan, m);
 }
 
+template <int kCol>
 __global__ void __launch_bounds__(kRawBlock) k_ts_extremes(const float *rows, uint32_t n, TsState *st) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long kmax = 0ull, kmin = ~0ull;
     if (i < n && (unsigned long long)i >= st->last_nan) { // the suffix after the last NaN: no NaN in it
-        const unsigned long long vb = (unsigned long long)ts_value_bits(ts_curvature(rows, i)) << 32;
+        const unsigned long long vb = (unsigned long long)ts_value_bits(row_column<kCol>(rows, i)) << 32;
         kmax = vb | i;
         kmin = vb | (uint32_t)~i;
     }

@@ -12,6 +12,7 @@
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 
 #include <dlfcn.h>
 #include <mutex>
@@ -27,6 +28,7 @@
 #include "kernels_ground.cuh"
 #include "kernels_sor.cuh"
 #include "kernels_rawscan.cuh"
+#include "kernels_ncc.cuh"
 
 using namespace mulls;
 
@@ -153,6 +155,7 @@ struct mulls_ctx {
     Scratch vx_buf, ext_buf;     // voxel filter; clouds handed between the stages of extract_semantic_pts
     Scratch sor_buf;             // statistical outlier filter: mean distances, keep mask, statistics
     Scratch raw_buf;             // raw-scan corrections: the rows of the call, the column it returns, timestamp state
+    Scratch ncc_buf;             // NCC keypoint matching: rows, descriptors, row / column minima or select state, sort
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
     const mulls_map *tree_map = nullptr;
@@ -233,7 +236,7 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (void *p : ctx->allocs) cudaFree(p);
     if (ctx->cub_temp) cudaFree(ctx->cub_temp);
-    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf})
+    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf, &ctx->ncc_buf})
         if (s->p) cudaFree(s->p);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
     if (ctx->h_flags) cudaFreeHost(ctx->h_flags);
@@ -1558,8 +1561,8 @@ static int timestamp_ratio_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int time
         TsState init{};
         init.min_key = ~0ull;
         CK(cudaMemcpyAsync(d_st, &init, sizeof(init), cudaMemcpyHostToDevice, st));
-        k_ts_last_nan<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st);
-        k_ts_extremes<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st);
+        k_ts_last_nan<9><<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st);
+        k_ts_extremes<9><<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st);
         k_ts_setup<<<1, 32, 0, st>>>(d_rows, (uint32_t)n, scan_duration_ms, d_st);
         k_ts_ratio<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st, d_out);
         launches = 4;
@@ -1612,6 +1615,170 @@ int mulls_timestamp_ratio(mulls_ctx *ctx, mulls_cloud_view cloud, int timestamp_
 int mulls_motion_compensation(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, const double T[16],
                               float s_ambiguous_thre, float *const *xyz_out) {
     return raw_drain(ctx, motion_compensation_impl(ctx, clouds, n_clouds, T, s_ambiguous_thre, xyz_out));
+}
+
+// ================================================================================================
+// NCC keypoint matching (CRegistration::find_feature_correspondence_ncc, cregistration.hpp:409-601): kernels_ncc.cuh.
+// Stateless like the raw-scan corrections: the resident batch and its grid are left alone.
+// ================================================================================================
+static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, int fixed_num_corr, int corr_num, int reciprocal_on,
+                    int32_t *tgt_idx, int32_t *src_idx, size_t cap, size_t *n_out, int *performed) {
+    if (!ctx || !n_out || !performed || (tk.n && !tk.aos48) || (sk.n && !sk.aos48) || (cap && (!tgt_idx || !src_idx)))
+        return MULLS_E_ARG;
+    *n_out = 0;
+    *performed = 0;
+    const char *fn = "mulls_ncc_correspondences";
+    int rc;
+    if ((rc = raw_capacity(ctx, tk.n, fn)) != MULLS_OK || (rc = raw_capacity(ctx, sk.n, fn)) != MULLS_OK) return rc;
+    const size_t nt = tk.n, ns = sk.n, n_all = nt + ns;
+    if (nt < 10 || ns < 10) return MULLS_OK; // :421-425
+    const size_t M = nt * ns;
+    size_t K = 0;
+    if (fixed_num_corr) {
+        if (M > (size_t)INT_MAX) { // :559 forms the pair index in int
+            ctx->err = std::string(fn) + ": " + std::to_string(nt) + " x " + std::to_string(ns) +
+                       " pairs exceed INT_MAX in the fixed-number mode";
+            return MULLS_E_ARG;
+        }
+        K = ((size_t)corr_num < M) ? (size_t)corr_num : M; // :565 min_(corr_num, dist_array.size()): int vs size_t
+    }
+    const size_t gy = ceil_div(ns, kNccTileS);
+    if (gy > 65535) {
+        ctx->err = std::string(fn) + ": too many source keypoints for one grid";
+        return MULLS_E_CAPACITY;
+    }
+    cudaStream_t st = ctx->stream;
+    // ncc_buf, 256-byte aligned pieces
+    size_t off = 0;
+    auto piece = [&off](size_t bytes) {
+        const size_t o = off;
+        off += ceil_div(std::max<size_t>(bytes, 1), 256) * 256;
+        return o;
+    };
+    const size_t o_rows = piece(n_all * 48), o_desc = piece(n_all * kNccDim * sizeof(float)), o_ts = piece(sizeof(TsState)),
+                 o_range = piece(2 * sizeof(float));
+    size_t o_rowkey = 0, o_colmin = 0, o_cand = 0, o_keep = 0, o_sel = 0, o_out = 0, o_num = 0, o_gath = 0, o_sorted = 0, o_tmp = 0;
+    size_t tmp_bytes = 0;
+    if (!fixed_num_corr) {
+        o_rowkey = piece(nt * 8), o_colmin = piece(ns * 4), o_cand = piece(nt * 8), o_keep = piece(nt), o_out = piece(nt * 8);
+        o_num = piece(sizeof(int));
+        CK(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, (unsigned long long *)nullptr, (uint8_t *)nullptr,
+                                      (unsigned long long *)nullptr, (int *)nullptr, (int)nt, st));
+    } else {
+        o_sel = piece(sizeof(NccSelect)), o_gath = piece(K * 8), o_sorted = piece(K * 8);
+        CK(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr,
+                                          (int)std::max<size_t>(K, 1), 0, 64, st));
+    }
+    o_tmp = piece(tmp_bytes);
+    if ((rc = grow_scratch(ctx, ctx->ncc_buf, off)) != MULLS_OK) return rc;
+    char *base = (char *)ctx->ncc_buf.p;
+    float *d_rows = (float *)(base + o_rows), *d_desc = (float *)(base + o_desc), *d_range = (float *)(base + o_range);
+    TsState *d_ts = (TsState *)(base + o_ts);
+    CK(cudaMemcpyAsync(d_rows, tk.aos48, nt * 48, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync((char *)d_rows + nt * 48, sk.aos48, ns * 48, cudaMemcpyHostToDevice, st));
+    TsState ts0{};
+    ts0.min_key = ~0ull;
+    CK(cudaMemcpyAsync(d_ts, &ts0, sizeof(ts0), cudaMemcpyHostToDevice, st));
+    const unsigned nbt = (unsigned)ceil_div(nt, kRawBlock);
+    k_ts_last_nan<8><<<nbt, kRawBlock, 0, st>>>(d_rows, (uint32_t)nt, d_ts);
+    k_ts_extremes<8><<<nbt, kRawBlock, 0, st>>>(d_rows, (uint32_t)nt, d_ts);
+    k_ncc_range<<<1, 32, 0, st>>>(d_rows, (uint32_t)nt, d_ts, d_range);
+    k_ncc_descriptors<<<(unsigned)ceil_div(n_all, kRawBlock), kRawBlock, 0, st>>>(d_rows, (uint32_t)n_all, d_range, d_desc);
+    uint64_t launches = 4;
+    const NccPairs P{d_desc, (uint32_t)n_all, (uint32_t)nt, (uint32_t)ns};
+    const dim3 grid((unsigned)ceil_div(nt, kNccTileT), (unsigned)gy);
+    std::vector<std::pair<int32_t, int32_t>> res;
+    if (!fixed_num_corr) {
+        unsigned long long *d_rowkey = (unsigned long long *)(base + o_rowkey), *d_cand = (unsigned long long *)(base + o_cand),
+                           *d_out = (unsigned long long *)(base + o_out);
+        uint32_t *d_colmin = (uint32_t *)(base + o_colmin);
+        uint8_t *d_keep = (uint8_t *)(base + o_keep);
+        int *d_num = (int *)(base + o_num);
+        k_ncc_init<<<(unsigned)ceil_div(std::max(nt, ns), kRawBlock), kRawBlock, 0, st>>>(d_rowkey, (uint32_t)nt, d_colmin, (uint32_t)ns);
+        if (reciprocal_on)
+            k_ncc_pairs<kNccRowCol><<<grid, kNccBlock, 0, st>>>(P, d_rowkey, d_colmin, nullptr, 0, nullptr, 0);
+        else
+            k_ncc_pairs<kNccRow><<<grid, kNccBlock, 0, st>>>(P, d_rowkey, nullptr, nullptr, 0, nullptr, 0);
+        k_ncc_pick<<<nbt, kRawBlock, 0, st>>>(d_rowkey, d_colmin, (uint32_t)nt, reciprocal_on ? 1 : 0, d_cand, d_keep);
+        launches += 3;
+        size_t tb = tmp_bytes;
+        CK(cub::DeviceSelect::Flagged(base + o_tmp, tb, d_cand, d_keep, d_out, d_num, (int)nt, st));
+        std::vector<unsigned long long> h(nt);
+        int n_kept = 0;
+        CK(cudaMemcpyAsync(&n_kept, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(h.data(), d_out, nt * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaGetLastError());
+        CK(cudaStreamSynchronize(st));
+        res.reserve(n_kept);
+        for (int k = 0; k < n_kept; ++k) res.emplace_back((int32_t)(h[k] >> 32), (int32_t)(uint32_t)h[k]);
+    } else if (K > 0) {
+        NccSelect *d_sel = (NccSelect *)(base + o_sel);
+        unsigned long long *d_gath = (unsigned long long *)(base + o_gath), *d_sorted = (unsigned long long *)(base + o_sorted);
+        NccSelect s0{};
+        s0.rank = (uint32_t)(K - 1);
+        s0.E = 0xffffffffu;
+        if (K == M) s0.T = 0xffffffffu; // every pair: nothing to select
+        CK(cudaMemcpyAsync(d_sel, &s0, offsetof(NccSelect, hist), cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(d_sel->hist, 0, sizeof(s0.hist), st));
+        if (K < M) {
+            for (int shift = 24; shift >= 0; shift -= 8) { // the K-th smallest distance key T
+                k_ncc_pairs<kNccHistKey><<<grid, kNccBlock, 0, st>>>(P, nullptr, nullptr, d_sel, shift, nullptr, 0);
+                k_ncc_select_step<<<1, 32, 0, st>>>(d_sel, shift, 0);
+                launches += 2;
+            }
+            NccSelect h_sel;
+            CK(cudaMemcpyAsync(&h_sel, d_sel, offsetof(NccSelect, hist), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            if (h_sel.need_eq < h_sel.count_eq) { // ties at T: the need_eq lowest pair indices among them
+                for (int shift = 24; shift >= 0; shift -= 8) {
+                    k_ncc_pairs<kNccHistIdx><<<grid, kNccBlock, 0, st>>>(P, nullptr, nullptr, d_sel, shift, nullptr, 0);
+                    k_ncc_select_step<<<1, 32, 0, st>>>(d_sel, shift, 1);
+                    launches += 2;
+                }
+            }
+        }
+        k_ncc_pairs<kNccGather><<<grid, kNccBlock, 0, st>>>(P, nullptr, nullptr, d_sel, 0, d_gath, K);
+        size_t tb = tmp_bytes;
+        CK(cub::DeviceRadixSort::SortKeys(base + o_tmp, tb, d_gath, d_sorted, (int)K, 0, 64, st));
+        launches += 1;
+        std::vector<unsigned long long> h(K);
+        unsigned long long gathered = 0;
+        CK(cudaMemcpyAsync(&gathered, &d_sel->count, sizeof(gathered), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(h.data(), d_sorted, K * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaGetLastError());
+        CK(cudaStreamSynchronize(st));
+        if (gathered != K) {
+            ctx->err = std::string(fn) + ": the select gathered " + std::to_string(gathered) + " pairs for K = " + std::to_string(K);
+            return MULLS_E_CUDA;
+        }
+        // :567-586, the walk over the first K pairs in order: at most 7 pairs per target and per source
+        std::vector<int> count_target_kpt(nt, 0), count_source_kpt(ns, 0);
+        const int max_corr_num = 6;
+        for (size_t k = 0; k < K; ++k) {
+            const uint32_t index = (uint32_t)h[k];
+            const int i = (int)(index / ns), j = (int)(index % ns);
+            if (count_target_kpt[i] > max_corr_num || count_source_kpt[j] > max_corr_num) continue;
+            count_target_kpt[i]++;
+            count_source_kpt[j]++;
+            res.emplace_back(i, j);
+        }
+    }
+    if (res.size() > cap) {
+        ctx->err = std::string(fn) + ": " + std::to_string(res.size()) + " correspondences, room for " + std::to_string(cap);
+        return MULLS_E_ARG;
+    }
+    for (size_t k = 0; k < res.size(); ++k) tgt_idx[k] = res[k].first, src_idx[k] = res[k].second;
+    *n_out = res.size();
+    *performed = 1;
+    ctx->stats = mulls_run_stats();
+    ctx->stats.kernel_launches = launches;
+    return MULLS_OK;
+}
+int mulls_ncc_correspondences(mulls_ctx *ctx, mulls_cloud_view target_kpts, mulls_cloud_view source_kpts, int fixed_num_corr,
+                              int corr_num, int reciprocal_on, int32_t *tgt_idx, int32_t *src_idx, size_t cap, size_t *n_out,
+                              int *performed) {
+    return raw_drain(ctx, ncc_impl(ctx, target_kpts, source_kpts, fixed_num_corr, corr_num, reciprocal_on, tgt_idx, src_idx, cap,
+                                   n_out, performed));
 }
 
 // ================================================================================================

@@ -330,6 +330,25 @@ class Context:
         res = [o[: len(c)] for o, c in zip(outs, cl)]
         return res[0] if single else res
 
+    def ncc_correspondences(self, target_kpts: np.ndarray, source_kpts: np.ndarray, fixed_num_corr: bool = False,
+                            corr_num: int = 2000, reciprocal_on: bool = True):
+        """CRegistration::find_feature_correspondence_ncc (cregistration.hpp:409-601) on the GPU, as index pairs: returns
+        None where the reference returns false (fewer than 10 keypoints in a cloud), else (tgt_idx, src_idx), int32 arrays
+        of the rows the reference appends to target_corrs / source_corrs, in its order. The resident batch is untouched."""
+        t, s = abi.as_aos48(target_kpts), abi.as_aos48(source_kpts)
+        cap = 7 * min(len(t), len(s)) if fixed_num_corr else len(t)  # at most 7 pairs per keypoint / one per target row
+        ti = np.zeros(max(cap, 1), np.int32)
+        si = np.zeros(max(cap, 1), np.int32)
+        n = C.c_size_t(0)
+        performed = C.c_int(0)
+        ip = C.POINTER(C.c_int32)
+        self._check(self.lib.mulls_ncc_correspondences(self.handle, abi.cloud_view(t), abi.cloud_view(s), int(bool(fixed_num_corr)),
+                                                       int(corr_num), int(bool(reciprocal_on)), ti.ctypes.data_as(ip),
+                                                       si.ctypes.data_as(ip), cap, C.byref(n), C.byref(performed)))
+        if not performed.value:
+            return None
+        return ti[: n.value].copy(), si[: n.value].copy()
+
     def stats(self) -> dict:
         s = abi.RunStats()
         self._check(self.lib.mulls_get_stats(self.handle, C.byref(s)))
@@ -467,6 +486,21 @@ class CRegistration:
         self._ctx = Context(device, 1, max_src_pts, max_tgt_pts)
         self._batch_ctx = None
         self.last_trace = None
+
+    def find_feature_correspondence_ncc(self, target_kpts: np.ndarray, source_kpts: np.ndarray, target_corrs=None,
+                                        source_corrs=None, fixed_num_corr: bool = False, corr_num: int = 2000,
+                                        reciprocal_on: bool = True):
+        """lo::CRegistration::find_feature_correspondence_ncc (cregistration.hpp:409-601): returns (ok, target_corrs,
+        source_corrs). The matched keypoint rows are appended to the given (n, 12) clouds (empty when None), which come
+        back unchanged when ok is False (fewer than 10 keypoints in a cloud)."""
+        t, s = abi.as_aos48(target_kpts), abi.as_aos48(source_kpts)
+        tc = _empty() if target_corrs is None else abi.as_aos48(target_corrs)
+        sc = _empty() if source_corrs is None else abi.as_aos48(source_corrs)
+        got = self._ctx.ncc_correspondences(t, s, fixed_num_corr, corr_num, reciprocal_on)
+        if got is None:
+            return False, tc, sc
+        ti, si = got
+        return True, np.concatenate([tc, t[ti]]), np.concatenate([sc, s[si]])
 
     def mm_lls_icp_4dof_global(self, registration_con: Constraint, heading_step_d: float, max_iter_num: int = 20,
                                dis_thre_unit: float = 1.5, converge_translation: float = 0.005,
