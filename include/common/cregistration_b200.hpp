@@ -251,6 +251,33 @@ bool find_feature_correspondence_ncc(const typename pcl::PointCloud<PointT>::Ptr
     return true;
 }
 
+// lo::CRegistration<PointT>::coarse_reg_ransac (cregistration.hpp:604-661), same arguments and defaults
+// (test/mulls_reg.cpp:170-195, test/mulls_slam.cpp:532-560): the RANSAC rejector over the correspondences i <-> i runs on
+// the device (mulls_coarse_reg_ransac, readings in abi.h). Returns 1 (reliable), 0 (need check) or -1 (failed) as the
+// reference does, with tran_mat written only on 1 or 0. A library error is logged and returns -1 with tran_mat left as
+// it was, so the callers fall back to their odometry guess.
+template <typename PointT>
+int coarse_reg_ransac(const typename pcl::PointCloud<PointT>::Ptr &target_pts, const typename pcl::PointCloud<PointT>::Ptr &source_pts,
+                      Eigen::Matrix4d &tran_mat, float noise_bound = 0.2, int min_inlier_num = 8, int max_iter_num = 20000) {
+    const size_t n = target_pts->points.size();
+    double T[16];
+    int status = -1, n_inliers = 0, n_hypotheses = 0;
+    mulls_ctx *ctx = thread_context(0, n);
+    if (!ctx || mulls_coarse_reg_ransac(ctx, view_of<PointT>(target_pts), view_of<PointT>(source_pts), noise_bound, min_inlier_num,
+                                        max_iter_num, T, &status, &n_inliers, &n_hypotheses) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return -1;
+    }
+    LOG(INFO) << "[" << n_inliers << "] inlier correspondences found."; // :640
+    if (status < 0) {
+        LOG(WARNING) << "RANSAC failed"; // :658
+        return -1;
+    }
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) tran_mat(r, c) = T[4 * r + c];
+    return status;
+}
+
 } // namespace b200
 } // namespace lo
 #endif

@@ -11,10 +11,11 @@
 //     CRegistration_reference — every member the reference defines stays available, unchanged;
 //   * lo::CRegistration<PointT> is then defined HERE as a class derived from it whose mm_lls_icp
 //     (cregistration.hpp:1114-1123: same name, argument order, types and defaults) and mm_lls_icp_4dof_global
-//     (:1584-1592) and find_feature_correspondence_ncc (:409-411) run on the GPU through the C-ABI
-//     (include/mulls_b200/abi.h). All other public members the callers use
+//     (:1584-1592), find_feature_correspondence_ncc (:409-411) and coarse_reg_ransac (:605-607) run on the GPU through
+//     the C-ABI (include/mulls_b200/abi.h). All other public members the callers use
 //     — determine_source_target_cloud, assign_source_target_cloud, coarse_reg_teaser,
-//     coarse_reg_ransac, omp_ndt, omp_gicp, ... (SURVEY.md section 8b) — are inherited from the reference.
+//     omp_ndt, omp_gicp, ... (SURVEY.md section 8b) — are inherited from the reference; every overload of
+//     coarse_reg_ransac the reference class declares stays visible next to the device one.
 // Differences in contract are listed in INTEGRATION.md (block1->tree_* are not populated: use mulls_nn_query or
 // the drop-in lo::MapManager of dropin/map_manager.h, which does not need them).
 #ifndef MULLS_B200_DROPIN_CREGISTRATION_HPP
@@ -75,6 +76,12 @@ class CRegistration : public CRegistration_reference<PointT> {
                                          int corr_num = 2000, bool reciprocal_on = true) {
         return b200::find_feature_correspondence_ncc<PointT>(target_kpts, source_kpts, target_corrs, source_corrs, fixed_num_corr,
                                                              corr_num, reciprocal_on);
+    }
+    // cregistration.hpp:605-607
+    using CRegistration_reference<PointT>::coarse_reg_ransac;
+    int coarse_reg_ransac(const typename pcl::PointCloud<PointT>::Ptr &target_pts, const typename pcl::PointCloud<PointT>::Ptr &source_pts,
+                          Eigen::Matrix4d &tran_mat, float noise_bound = 0.2, int min_inlier_num = 8, int max_iter_num = 20000) {
+        return b200::coarse_reg_ransac<PointT>(target_pts, source_pts, tran_mat, noise_bound, min_inlier_num, max_iter_num);
     }
 };
 

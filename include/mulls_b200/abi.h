@@ -37,6 +37,7 @@
  *   mulls_motion_compensation <- lo::CFilter<PointT>::apply_motion_compensation / batch_apply_motion_compensation,
  *                               cfilter.hpp:470-549
  *   mulls_ncc_correspondences <- lo::CRegistration<PointT>::find_feature_correspondence_ncc, cregistration.hpp:409-601
+ *   mulls_coarse_reg_ransac  <- lo::CRegistration<PointT>::coarse_reg_ransac, cregistration.hpp:604-661
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
  *
@@ -543,6 +544,32 @@ int mulls_motion_compensation(mulls_ctx *ctx, const mulls_cloud_view *clouds, in
 int mulls_ncc_correspondences(mulls_ctx *ctx, mulls_cloud_view target_kpts, mulls_cloud_view source_kpts, int fixed_num_corr,
                               int corr_num, int reciprocal_on, int32_t *tgt_idx, int32_t *src_idx, size_t cap, size_t *n_out,
                               int *performed);
+
+/* lo::CRegistration<PointT>::coarse_reg_ransac(target_pts, source_pts, tran_mat, noise_bound, min_inlier_num,
+ * max_iter_num), cregistration.hpp:604-661: the coarse transform of the global registration (test/mulls_reg.cpp:170-195,
+ * test/mulls_slam.cpp:532-560), PCL 1.10's CorrespondenceRejectorSampleConsensus over the correspondences i <-> i,
+ * i < N = target_pts.n, with the inlier threshold noise_bound, max_iter_num iterations and the refinement on. Stateless
+ * like mulls_ncc_correspondences: the batch resident on the context and its grid are left alone. 48-byte rows as for
+ * the NCC matching; only x y z are read. Readings (ransac_core.cuh R1-R6 and C1-C2 state them in full):
+ *   - the sample stream is boost::mt19937(12345) with rnd() = mt() >> 1 on the model's persistent shuffle, a sample is
+ *     good when its three pairwise float squared source distances exceed the sample distance threshold (float
+ *     covariance of the N source points, pcl::eigen33); 1000 attempts per selection, an empty selection ends the search
+ *   - each hypothesis is pcl::umeyama in double (3x3 Jacobi SVD, sums in a fixed order) cast to float; a correspondence
+ *     is an inlier when the float squared error of T [s, 1] against t is < noise_bound^2 in double
+ *   - the adaptive k of RandomSampleConsensus (p = 0.99), at most max_iter_num + 1 hypotheses (max_iter_num == 0: none)
+ *   - refineModel(3, 1000): re-fit, re-select, threshold sqrt(min(noise_bound^2, 9 * 2.1981 * median)), stopping when
+ *     the inlier set repeats, the sizes oscillate, or after 1000 rounds
+ *   - the search finds no model (N < 3, no good sample, max_iter_num == 0), or fewer than 3 inliers survive: all N
+ *     correspondences remain, with the identity; a failed refinement leaves none and the identity (PCL's matrix would
+ *     be uninitialised; it is read only when min_inlier_num is 0)
+ * Outputs: *status is 1 when the remaining count is >= 2 * min_inlier_num, 0 when it is >= min_inlier_num, -1 otherwise
+ * (the comparisons are against size_t, so a negative min_inlier_num always gives -1); tran_mat (row-major) is written
+ * only when *status >= 0, with the float model widened; *n_inliers is the remaining count and *n_hypotheses the
+ * hypotheses scored. source_pts shorter than target_pts, or a NULL output: MULLS_E_ARG (nothing written). N above the
+ * context's max_tgt_pts: MULLS_E_CAPACITY. */
+int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_cloud_view source_pts, float noise_bound,
+                            int min_inlier_num, int max_iter_num, double tran_mat[16] /* row-major, written only when status >= 0 */,
+                            int *status, int *n_inliers, int *n_hypotheses);
 
 /* The wire format the library ships host clouds in when the "host_pack" tunable is on (csrc/host_pack.h): the 28 of the
  * 48 bytes of a pcl::PointXYZINormal row (utility.hpp:40) that the path reads, repacked on the host cores into pinned

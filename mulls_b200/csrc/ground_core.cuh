@@ -291,6 +291,23 @@ GF_HD void gf_high_emit(const GfArgs &A, uint32_t j) {
     o[0] = a, o[1] = r[1], o[2] = r[2];
 }
 
+// ---- pcl::computeMeanAndCovarianceMatrix (PCL 1.10): float accumulator xx xy xz yy yz zz x y z, in point order ----------
+GF_HD void gf_mean_cov_add(float accu[9], float x, float y, float z) {
+    accu[0] += x * x, accu[1] += x * y, accu[2] += x * z, accu[3] += y * y, accu[4] += y * z, accu[5] += z * z;
+    accu[6] += x, accu[7] += y, accu[8] += z;
+}
+// accu /= count; the centroid is accu[6..8] afterwards
+GF_HD void gf_mean_cov_finish(float accu[9], float count, float cov[3][3]) {
+    for (int i = 0; i < 9; ++i) accu[i] /= count;
+    cov[0][0] = accu[0] - accu[6] * accu[6];
+    cov[0][1] = accu[1] - accu[6] * accu[7];
+    cov[0][2] = accu[2] - accu[6] * accu[8];
+    cov[1][1] = accu[3] - accu[7] * accu[7];
+    cov[1][2] = accu[4] - accu[7] * accu[8];
+    cov[2][2] = accu[5] - accu[8] * accu[8];
+    cov[1][0] = cov[0][1], cov[2][0] = cov[0][2], cov[2][1] = cov[1][2];
+}
+
 // ---- pcl::SampleConsensusModelPlane pieces (PCL 1.10) ------------------------------------------------------------------
 // model_coefficients.dot(Vector4f(x, y, z, 1)): Eigen's 4-wide packet reduction (a0+a2)+(a1+a3)
 GF_HD float gf_plane_dot(const float c[4], float x, float y, float z) { return (c[0] * x + c[2] * z) + (c[1] * y + c[3] * 1.0f); }
@@ -365,15 +382,27 @@ GF_HD void gf_cross(const float a[3], const float b[3], float o[3]) {
     o[1] = a[2] * b[0] - a[0] * b[2];
     o[2] = a[0] * b[1] - a[1] * b[0];
 }
-// pcl::eigen33(mat, eigenvalue, eigenvector): eigenvector of the smallest eigenvalue
-GF_HD void gf_eigen33_smallest(const float mat[3][3], float evec[3]) {
+// pcl::eigen33's scaling: mat / max|mat_ij| (1 when that is at most FLT_MIN; a NaN entry does not raise it)
+GF_HD float gf_eigen33_scale(const float mat[3][3], float m[3][3]) {
     float scale = 0.0f;
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) scale = fmaxf(scale, fabsf(mat[i][j]));
     if (scale <= FLT_MIN) scale = 1.0f;
-    float m[3][3];
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) m[i][j] = mat[i][j] / scale;
+    return scale;
+}
+// pcl::eigen33(mat, eigenvalues): the roots of the scaled matrix, ascending, times the scale
+GF_HD void gf_eigen33_values(const float mat[3][3], float evals[3]) {
+    float m[3][3];
+    const float scale = gf_eigen33_scale(mat, m);
+    gf_roots(m, evals);
+    evals[0] *= scale, evals[1] *= scale, evals[2] *= scale;
+}
+// pcl::eigen33(mat, eigenvalue, eigenvector): eigenvector of the smallest eigenvalue
+GF_HD void gf_eigen33_smallest(const float mat[3][3], float evec[3]) {
+    float m[3][3];
+    gf_eigen33_scale(mat, m);
     float r[3];
     gf_roots(m, r);
     for (int i = 0; i < 3; ++i) m[i][i] -= r[0];
@@ -463,24 +492,14 @@ GF_HD bool gf_sac_plane(const float4 *cx, int n, double threshold, int max_itera
         const float4 p = cx[i];
         if ((double)fabsf(gf_plane_dot(best, p.x, p.y, p.z)) < threshold) {
             ++n_inl;
-            accu[0] += p.x * p.x, accu[1] += p.x * p.y, accu[2] += p.x * p.z, accu[3] += p.y * p.y, accu[4] += p.y * p.z,
-                accu[5] += p.z * p.z;
-            accu[6] += p.x, accu[7] += p.y, accu[8] += p.z;
+            gf_mean_cov_add(accu, p.x, p.y, p.z);
         }
     }
     if (n_inl == 0) return false;
     coeff[0] = best[0], coeff[1] = best[1], coeff[2] = best[2], coeff[3] = best[3];
     if (n_inl >= 4) {
-        const float cnt = (float)n_inl;
-        for (int i = 0; i < 9; ++i) accu[i] /= cnt;
         float cov[3][3];
-        cov[0][0] = accu[0] - accu[6] * accu[6];
-        cov[0][1] = accu[1] - accu[6] * accu[7];
-        cov[0][2] = accu[2] - accu[6] * accu[8];
-        cov[1][1] = accu[3] - accu[7] * accu[7];
-        cov[1][2] = accu[4] - accu[7] * accu[8];
-        cov[2][2] = accu[5] - accu[8] * accu[8];
-        cov[1][0] = cov[0][1], cov[2][0] = cov[0][2], cov[2][1] = cov[1][2];
+        gf_mean_cov_finish(accu, (float)n_inl, cov);
         float ev[3];
         gf_eigen33_smallest(cov, ev);
         coeff[0] = ev[0], coeff[1] = ev[1], coeff[2] = ev[2], coeff[3] = 0.0f;

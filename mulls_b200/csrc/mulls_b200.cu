@@ -29,6 +29,7 @@
 #include "kernels_sor.cuh"
 #include "kernels_rawscan.cuh"
 #include "kernels_ncc.cuh"
+#include "kernels_ransac.cuh"
 
 using namespace mulls;
 
@@ -156,6 +157,8 @@ struct mulls_ctx {
     Scratch sor_buf;             // statistical outlier filter: mean distances, keep mask, statistics
     Scratch raw_buf;             // raw-scan corrections: the rows of the call, the column it returns, timestamp state
     Scratch ncc_buf;             // NCC keypoint matching: rows, descriptors, row / column minima or select state, sort
+    Scratch rc_buf;              // RANSAC coarse registration: correspondences, hypotheses, counts, refinement state
+    void *rc_host = nullptr;     // pinned: two chunks of sample triples and their counts
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
     const mulls_map *tree_map = nullptr;
@@ -236,8 +239,9 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (void *p : ctx->allocs) cudaFree(p);
     if (ctx->cub_temp) cudaFree(ctx->cub_temp);
-    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf, &ctx->ncc_buf})
+    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf, &ctx->ncc_buf, &ctx->rc_buf})
         if (s->p) cudaFree(s->p);
+    if (ctx->rc_host) cudaFreeHost(ctx->rc_host);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
     if (ctx->h_flags) cudaFreeHost(ctx->h_flags);
     if (ctx->h_running) cudaFreeHost(ctx->h_running);
@@ -1782,6 +1786,164 @@ int mulls_ncc_correspondences(mulls_ctx *ctx, mulls_cloud_view target_kpts, mull
 }
 
 // ================================================================================================
+// RANSAC coarse registration (CRegistration::coarse_reg_ransac, cregistration.hpp:604-661): ransac_core.cuh,
+// kernels_ransac.cuh. Stateless like the NCC matching: the resident batch and its grid are left alone.
+// The sample stream is drawn here in chunks: kRcFirstChunk hypotheses, then up to kRcChunk. After each chunk the counts
+// come down and the adaptive-k walk is replayed over them. Once a k is known, the next chunk is drawn while the device
+// fits and scores the current one, never past ceil(k) hypotheses: a search that ends early draws little more than it uses.
+// ================================================================================================
+static constexpr int kRcFirstChunk = 64;
+static constexpr int kRcChunk = 4096;
+
+static int ransac_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, float noise_bound, int min_inlier_num,
+                       int max_iter_num, double *tran_mat, int *status, int *n_inliers, int *n_hypotheses) {
+    if (!ctx || !tran_mat || !status || !n_inliers || !n_hypotheses || (tv.n && !tv.aos48) || (sv.n && !sv.aos48))
+        return MULLS_E_ARG;
+    const char *fn = "mulls_coarse_reg_ransac";
+    const size_t N = tv.n;
+    if (sv.n < N) { // the reference would read source rows past the end
+        ctx->err = std::string(fn) + ": " + std::to_string(sv.n) + " source points for " + std::to_string(N) + " target points";
+        return MULLS_E_ARG;
+    }
+    int rc;
+    if ((rc = raw_capacity(ctx, N, fn)) != MULLS_OK) return rc;
+    if (N > (size_t)INT_MAX) {
+        ctx->err = std::string(fn) + ": more than INT_MAX correspondences";
+        return MULLS_E_ARG;
+    }
+    if (ceil_div(N, kRcTile) > 65535) { // k_ransac_count's grid.y
+        ctx->err = std::string(fn) + ": " + std::to_string(N) + " correspondences exceed one count grid (" +
+                   std::to_string((size_t)65535 * kRcTile) + ")";
+        return MULLS_E_CAPACITY;
+    }
+    float T[12] = {1.f, 0.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, 1.f, 0.f}; // identity
+    size_t n_final = 0;
+    int hyps = 0;
+    uint64_t launches = 0;
+    if (N > 0) { // an empty correspondence list returns before the rejector runs (getCorrespondences)
+        cudaStream_t st = ctx->stream;
+        size_t off = 0;
+        auto piece = [&off](size_t bytes) {
+            const size_t o = off;
+            off += ceil_div(std::max<size_t>(bytes, 1), 256) * 256;
+            return o;
+        };
+        const size_t o_corr = piece(N * 6 * sizeof(float)), o_samp = piece(2 * kRcChunk * 3 * sizeof(int)),
+                     o_T = piece(2 * (size_t)kRcChunk * 12 * sizeof(float)), o_cnt = piece(2 * kRcChunk * sizeof(int)),
+                     o_best = piece(12 * sizeof(float)), o_fa = piece(N), o_fb = piece(N), o_err = piece(N * sizeof(float)),
+                     o_out = piece(sizeof(RcRefineOut));
+        if ((rc = grow_scratch(ctx, ctx->rc_buf, off)) != MULLS_OK) return rc;
+        if (!ctx->rc_host) CK(cudaMallocHost(&ctx->rc_host, 2 * kRcChunk * 4 * sizeof(int)));
+        char *base = (char *)ctx->rc_buf.p;
+        float *d_corr = (float *)(base + o_corr), *d_best = (float *)(base + o_best);
+        int *h_samp[2] = {(int *)ctx->rc_host, (int *)ctx->rc_host + 3 * kRcChunk};
+        int *h_cnt[2] = {(int *)ctx->rc_host + 6 * kRcChunk, (int *)ctx->rc_host + 7 * kRcChunk};
+        int *d_samp[2] = {(int *)(base + o_samp), (int *)(base + o_samp) + 3 * kRcChunk};
+        float *d_T[2] = {(float *)(base + o_T), (float *)(base + o_T) + 12 * (size_t)kRcChunk};
+        int *d_cnt[2] = {(int *)(base + o_cnt), (int *)(base + o_cnt) + kRcChunk};
+        // the correspondences i <-> i: source x y z, target x y z
+        std::vector<float> c6(N * 6);
+        for (size_t i = 0; i < N; ++i)
+            for (int c = 0; c < 3; ++c) c6[6 * i + c] = sv.aos48[12 * i + c], c6[6 * i + 3 + c] = tv.aos48[12 * i + c];
+        CK(cudaMemcpyAsync(d_corr, c6.data(), N * 6 * sizeof(float), cudaMemcpyHostToDevice, st));
+        std::vector<int> shuf(N);
+        for (size_t i = 0; i < N; ++i) shuf[i] = (int)i;
+        SacSampler S{SacMt19937(), shuf.data(), N, sv.aos48, rc_sample_dist_threshold(sv.aos48, N)};
+        SacWalk W(N, max_iter_num);
+        // no more hypotheses than the walk can take: max_iterations + 1, or none when max_skip is 0
+        const int64_t cap_hyp = W.max_skip == 0 ? 0 : (max_iter_num < 0 ? 1 : (int64_t)max_iter_num + 1);
+        int64_t produced = 0;
+        bool exhausted = false;
+        // draws up to `want` samples, and never more hypotheses than the walk can take: cap_hyp, and once a count is in,
+        // ceil(k) (k only falls as the best count rises, so the k known now bounds the walk's end)
+        auto draw_chunk = [&](int *dst, int want) {
+            const int64_t lim = (W.best >= 0 && W.k < (double)cap_hyp) ? (int64_t)ceil(W.k) : cap_hyp;
+            int c = 0;
+            while (c < want && produced < lim && !exhausted) {
+                if (!S.draw(dst + 3 * c)) {
+                    exhausted = true;
+                    break;
+                }
+                ++c, ++produced;
+            }
+            return c;
+        };
+        const double thresh_sq = (double)noise_bound * (double)noise_bound;
+        int cnt[2] = {draw_chunk(h_samp[0], kRcFirstChunk), 0}, cur = 0;
+        bool done = !W.wants();
+        while (!done && cnt[cur] > 0) {
+            const int H = cnt[cur];
+            CK(cudaMemcpyAsync(d_samp[cur], h_samp[cur], (size_t)H * 3 * sizeof(int), cudaMemcpyHostToDevice, st));
+            CK(cudaMemsetAsync(d_cnt[cur], 0, (size_t)H * sizeof(int), st));
+            k_ransac_fit<<<(unsigned)ceil_div(H, kRcFitBlock), kRcFitBlock, 0, st>>>(d_corr, d_samp[cur], H, d_T[cur]);
+            const dim3 grid((unsigned)ceil_div(H, kRcCountBlock * kRcHypPerThread), (unsigned)ceil_div(N, kRcTile));
+            k_ransac_count<<<grid, kRcCountBlock, 0, st>>>(d_corr, (int)N, d_T[cur], H, thresh_sq, d_cnt[cur]);
+            CK(cudaMemcpyAsync(h_cnt[cur], d_cnt[cur], (size_t)H * sizeof(int), cudaMemcpyDeviceToHost, st));
+            launches += 2;
+            const int nxt = cur ^ 1;
+            // the next chunk is drawn while this one is scored, once a k is known to bound it
+            cnt[nxt] = W.best >= 0 ? draw_chunk(h_samp[nxt], kRcChunk) : 0;
+            CK(cudaGetLastError());
+            CK(cudaStreamSynchronize(st));
+            const int best_before = W.best;
+            for (int h = 0; h < H && !done; ++h) {
+                if (!W.wants()) done = true;
+                else W.take(h_cnt[cur][h]);
+            }
+            if (W.best != best_before) // keep the best model before its chunk buffer is reused
+                CK(cudaMemcpyAsync(d_best, d_T[cur] + 12 * (size_t)(W.best - hyps), 12 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            hyps += H;
+            if (!W.wants()) done = true;
+            else if (cnt[nxt] == 0) cnt[nxt] = draw_chunk(h_samp[nxt], kRcChunk); // after the first chunk
+            cur = nxt;
+        }
+        hyps = W.iterations;
+        if (W.best < 0) { // computeModel failed: every correspondence, identity
+            n_final = N;
+        } else {
+            RcRefineArgs A{d_corr, (int)N, d_best, (double)noise_bound, (uint8_t *)(base + o_fa), (uint8_t *)(base + o_fb),
+                           (float *)(base + o_err), (RcRefineOut *)(base + o_out)};
+            k_ransac_refine<<<1, kRcLanes, 0, st>>>(A);
+            launches += 1;
+            RcRefineOut o;
+            CK(cudaMemcpyAsync(&o, A.out, sizeof(o), cudaMemcpyDeviceToHost, st));
+            CK(cudaGetLastError());
+            CK(cudaStreamSynchronize(st));
+            if (!o.ok) {
+                n_final = 0; // refinement failed: no correspondences; T stays the identity (PCL's is uninitialised)
+            } else if (o.n_inliers < 3) {
+                n_final = N;
+            } else {
+                n_final = (size_t)o.n_inliers;
+                std::memcpy(T, o.T, sizeof(T));
+            }
+        }
+    }
+    // final_corres->size() >= min_inlier_num: int against size_t, so a negative minimum is never reached
+    const size_t lo = (size_t)(int64_t)min_inlier_num, hi = (size_t)(int64_t)(int32_t)((uint32_t)min_inlier_num * 2u);
+    int stat = -1;
+    if (n_final >= lo) {
+        stat = n_final >= hi ? 1 : 0;
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 4; ++c) tran_mat[4 * r + c] = (double)T[4 * r + c];
+        tran_mat[12] = tran_mat[13] = tran_mat[14] = 0.0;
+        tran_mat[15] = 1.0;
+    }
+    *status = stat;
+    *n_inliers = (int)n_final;
+    *n_hypotheses = hyps;
+    ctx->stats = mulls_run_stats();
+    ctx->stats.kernel_launches = launches;
+    return MULLS_OK;
+}
+int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_cloud_view source_pts, float noise_bound,
+                            int min_inlier_num, int max_iter_num, double tran_mat[16], int *status, int *n_inliers,
+                            int *n_hypotheses) {
+    return raw_drain(ctx, ransac_impl(ctx, target_pts, source_pts, noise_bound, min_inlier_num, max_iter_num, tran_mat, status,
+                                      n_inliers, n_hypotheses));
+}
+
+// ================================================================================================
 // Device-resident local map (MapManager::update_local_map, src/map_manager.cpp:17-145)
 // ================================================================================================
 } // extern "C"
@@ -2327,25 +2489,8 @@ const uint32_t *sac_draw_table() {
     static std::vector<uint32_t> tab;
     if (tab.empty()) {
         std::vector<uint32_t> t(kSacDraws);
-        uint32_t mt[624];
-        mt[0] = 12345u;
-        for (int i = 1; i < 624; ++i) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (uint32_t)i;
-        int idx = 624;
-        for (int k = 0; k < kSacDraws; ++k) {
-            if (idx >= 624) {
-                for (int i = 0; i < 624; ++i) {
-                    const uint32_t y = (mt[i] & 0x80000000u) | (mt[(i + 1) % 624] & 0x7fffffffu);
-                    mt[i] = mt[(i + 397) % 624] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
-                }
-                idx = 0;
-            }
-            uint32_t y = mt[idx++];
-            y ^= y >> 11;
-            y ^= (y << 7) & 0x9d2c5680u;
-            y ^= (y << 15) & 0xefc60000u;
-            y ^= y >> 18;
-            t[k] = y;
-        }
+        SacMt19937 mt;
+        for (int k = 0; k < kSacDraws; ++k) t[k] = mt.next();
         tab.swap(t);
     }
     return tab.data();

@@ -349,6 +349,22 @@ class Context:
             return None
         return ti[: n.value].copy(), si[: n.value].copy()
 
+    def coarse_reg_ransac(self, target_pts: np.ndarray, source_pts: np.ndarray, noise_bound: float = 0.2,
+                          min_inlier_num: int = 8, max_iter_num: int = 20000, tran_mat=None):
+        """CRegistration::coarse_reg_ransac (cregistration.hpp:604-661) on the GPU over the correspondences i <-> i,
+        i < len(target_pts). Returns (status, tran_mat, n_inliers, n_hypotheses): status 1 (reliable), 0 (need check) or
+        -1 (failed); tran_mat is a (4, 4) float64 copy of the given one (identity when None), replaced by the estimate
+        when status >= 0. The resident batch is untouched."""
+        t, s = abi.as_aos48(target_pts), abi.as_aos48(source_pts)
+        T = np.array(np.eye(4) if tran_mat is None else tran_mat, np.float64).reshape(4, 4).copy()
+        buf = np.ascontiguousarray(T.ravel())
+        st, ni, nh = C.c_int(0), C.c_int(0), C.c_int(0)
+        self._check(self.lib.mulls_coarse_reg_ransac(self.handle, abi.cloud_view(t), abi.cloud_view(s), float(noise_bound),
+                                                     int(min_inlier_num), int(max_iter_num),
+                                                     buf.ctypes.data_as(C.POINTER(C.c_double)), C.byref(st), C.byref(ni),
+                                                     C.byref(nh)))
+        return st.value, buf.reshape(4, 4), ni.value, nh.value
+
     def stats(self) -> dict:
         s = abi.RunStats()
         self._check(self.lib.mulls_get_stats(self.handle, C.byref(s)))
@@ -501,6 +517,13 @@ class CRegistration:
             return False, tc, sc
         ti, si = got
         return True, np.concatenate([tc, t[ti]]), np.concatenate([sc, s[si]])
+
+    def coarse_reg_ransac(self, target_pts: np.ndarray, source_pts: np.ndarray, tran_mat=None, noise_bound: float = 0.2,
+                          min_inlier_num: int = 8, max_iter_num: int = 20000):
+        """lo::CRegistration::coarse_reg_ransac (cregistration.hpp:604-661): returns (status, tran_mat). tran_mat is the
+        given (4, 4) matrix (identity when None), replaced by the estimate when status >= 0 and left as it was on -1."""
+        status, T, _, _ = self._ctx.coarse_reg_ransac(target_pts, source_pts, noise_bound, min_inlier_num, max_iter_num, tran_mat)
+        return status, T
 
     def mm_lls_icp_4dof_global(self, registration_con: Constraint, heading_step_d: float, max_iter_num: int = 20,
                                dis_thre_unit: float = 1.5, converge_translation: float = 0.005,
