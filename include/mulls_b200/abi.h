@@ -180,9 +180,11 @@ int mulls_batch_upload(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
 int mulls_batch_run_resident(mulls_ctx *ctx, mulls_icp_result *out /* [n_pairs] or NULL */,
                              mulls_icp_trace *trace /* [n_pairs] or NULL */);
 
-/* Statistics of the last run on this context (for bench.py). */
+/* Statistics of the last call on this context (for bench.py). A registration fills every field; a front-end call
+ * (PCA, SOR, raw-scan corrections, NCC, RANSAC, voxel / ground filter, classification, extract_semantic_pts) fills
+ * kernel_launches and ms_total and zeroes the rest, so a call that launches nothing reports zero launches. */
 typedef struct mulls_run_stats {
-    uint64_t kernel_launches;   /* kernels of this library launched by the last run */
+    uint64_t kernel_launches;   /* kernels of this library launched by the last call (library sorts and scans are not counted) */
     uint64_t algorithmic_bytes; /* sum over pairs and executed iterations of 28*(N_s,active + N_t) */
     uint64_t iterations;        /* sum over pairs of executed iterations */
     uint64_t search_launches;   /* launches of the search kernel (one per ICP iteration of the batch) */

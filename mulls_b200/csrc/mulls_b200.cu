@@ -97,7 +97,7 @@ struct mulls_ctx {
     size_t cub_temp_bytes = 0;
     mulls_icp_result *d_results = nullptr;
     mulls_icp_result *h_results = nullptr; // pinned
-    uint32_t *h_flags = nullptr;           // pinned copy of hash_used (3 words)
+    uint32_t *h_flags = nullptr;           // pinned copy of hash_used (3 words), then the target count of ingest_cloud
     int *h_running = nullptr;              // mapped pinned: pairs still iterating
     std::vector<cudaEvent_t> ev_done;      // one per iteration (launch-loop flow control)
     mulls_icp_trace *d_trace = nullptr;
@@ -201,6 +201,22 @@ static inline size_t ceil_div(size_t a, size_t b) { return (a + b - 1) / b; }
 static inline double wall_ms() {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
+
+// The device arrays of one call in one Scratch: take() hands out 256-byte aligned offsets, grow() makes the Scratch
+// hold them all and sets `base`, from which each array is at its offset.
+struct ScratchLayout {
+    size_t bytes = 0;
+    size_t take(size_t n) {
+        const size_t o = bytes;
+        bytes += ceil_div(std::max<size_t>(n, 1), 256) * 256;
+        return o;
+    }
+    int grow(mulls_ctx *ctx, Scratch &s, char *&base) const {
+        const int rc = grow_scratch(ctx, s, bytes);
+        base = (char *)s.p;
+        return rc;
+    }
+};
 
 extern "C" {
 
@@ -366,7 +382,7 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     A.trace = ctx->d_trace; // written only when LoopCtl::trace_on is set for the run
     if ((e = cudaMallocHost((void **)&ctx->h_results, max_pairs * (sizeof(mulls_icp_result) + sizeof(uint64_t)))) != cudaSuccess)
         return fail("pinned results", e);
-    if ((e = cudaMallocHost((void **)&ctx->h_flags, 3 * sizeof(uint32_t))) != cudaSuccess) return fail("pinned flags", e);
+    if ((e = cudaMallocHost((void **)&ctx->h_flags, 4 * sizeof(uint32_t))) != cudaSuccess) return fail("pinned flags", e);
     if ((e = cudaMallocHost((void **)&ctx->h_ctl, sizeof(LoopCtl))) != cudaSuccess) return fail("pinned control block", e);
     // radix-sort temp storage for the largest possible sort
     {
@@ -1296,55 +1312,114 @@ int mulls_icp_run_sharded(mulls_ctx *ctx, const mulls_cloud_view tgt[MULLS_NUM_C
 
 } // extern "C"
 
-// PCA features of one cloud (host rows, or rows already in HBM) into ctx->pca_buf; `args` receives the device arrays.
-// unit_dist > 0: distance-adaptive neighbourhoods (k_pca<true>). Nothing is synchronised: the caller consumes the arrays
-// on ctx->stream.
-static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_device, float radius, int k, int stride,
-                         PcaArgs &args, uint64_t &launches, uint32_t *nbr = nullptr, float unit_dist = 0.f) {
-    const bool adaptive = unit_dist > 0.f;
-    // the cloud becomes the only target class of a one-pair batch: same filter-less ingest, same grid
+// ================================================================================================
+// Stateless front-end calls: PCA, statistical outlier removal, raw-scan corrections, NCC matching, RANSAC, and the
+// chain of extract_semantic_pts (voxel filter, ground filter, non-ground classification)
+// ================================================================================================
+// The call frame of every public front-end entry point. The body enqueues the call on ctx->stream and counts the kernels
+// of this library it launches. An error exit may leave a copy from or into a caller's buffer in flight: nothing is
+// handed back before the stream drains. A call that succeeds leaves its launches and device span in ctx->stats.
+template <typename Body>
+static int front_call(mulls_ctx *ctx, Body &&body) {
+    if (!ctx) return MULLS_E_ARG;
+    ctx->stats = mulls_run_stats();
+    uint64_t launches = 0;
+    const int rc = [&]() -> int {
+        CK(cudaSetDevice(ctx->device));
+        CK(cudaEventRecord(ctx->ev_begin, ctx->stream));
+        if (const int rc = body(launches); rc != MULLS_OK) return rc;
+        CK(cudaEventRecord(ctx->ev_end, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        CK(cudaGetLastError());
+        return MULLS_OK;
+    }();
+    if (rc != MULLS_OK) {
+        cudaStreamSynchronize(ctx->stream);
+        return rc;
+    }
+    ctx->stats.kernel_launches = launches;
+    cudaEventElapsedTime(&ctx->stats.ms_total, ctx->ev_begin, ctx->ev_end);
+    return MULLS_OK;
+}
+
+// a front-end call takes no more points than the targets of a registration
+static int check_capacity(mulls_ctx *ctx, size_t n, const char *fn) {
+    if (n <= ctx->max_tgt) return MULLS_OK;
+    ctx->err = std::string(fn) + ": " + std::to_string(n) + " points exceed max_tgt_pts of the context";
+    return MULLS_E_CAPACITY;
+}
+
+// Uploads one cloud (host rows, or rows already in HBM) as the only target class of a one-pair batch and builds its
+// grid with the filter-less ingest of a registration; the resident batch is gone afterwards. radius > 0 becomes
+// dis_thre_unit (the grid's top level then covers 2.5 x radius), 0 keeps the default. full_pyramid sets
+// normal_shooting_on, which asks k_pair_setup for the full level pyramid, whose top block spans the whole grid.
+// finite_only keeps points with a non-finite coordinate out of the bbox and the grid. The grid must fit the hash pool
+// before a kernel reads it: else the pool grows and the grid is built again from the cloud already in HBM (it fits by
+// construction). `A` receives the device arrays, n_tgt the count of target points in the grid.
+static int ingest_cloud(mulls_ctx *ctx, mulls_cloud_view cloud, bool on_device, float radius, bool full_pyramid,
+                        bool finite_only, DeviceArrays &A, int &n_tgt, uint64_t &launches) {
     mulls_icp_params P;
     mulls_icp_default_params(&P);
     std::strcpy(P.used_feature_type, "100000");
     P.apply_intersection_filter = 0;
-    P.dis_thre_unit = radius; // the grid's top level then covers 2.5 x radius
-    // an adaptive radius grows without bound with the range: normal_shooting_on asks k_pair_setup for the full level
-    // pyramid, whose top block spans the whole grid
-    if (adaptive) P.normal_shooting_on = 1;
+    if (radius > 0.f) P.dis_thre_unit = radius;
+    if (full_pyramid) P.normal_shooting_on = 1;
     P.max_iter_num = 0;
     mulls_cloud_view tgt[MULLS_NUM_CLASSES] = {cloud, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
     mulls_cloud_view src[MULLS_NUM_CLASSES] = {{nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
     const double ident[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    int rc = upload_impl(ctx, 1, tgt, src, &P, ident, nullptr, nullptr, /*resident=*/false, cloud_on_device);
-    if (rc != MULLS_OK) return rc;
-    const size_t n = cloud.n;
-    const size_t bytes = n * (9 * sizeof(float) + sizeof(int));
-    rc = grow_scratch(ctx, ctx->pca_buf, bytes);
+    int rc = upload_impl(ctx, 1, tgt, src, &P, ident, nullptr, nullptr, /*resident=*/false, on_device);
+    ctx->uploaded = false;
     if (rc != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
-    DeviceArrays A = ctx->A;
+    A = ctx->A;
     A.trace = nullptr;
-    rc = launch_ingest(ctx, A, false, launches);
-    if (rc != MULLS_OK) return rc;
-    // the grid must fit the hash pool before k_pca reads it: else grow the pool and build the grid again from the
-    // cloud already in HBM (it fits by construction)
+    if ((rc = launch_ingest(ctx, A, false, launches, nullptr, nullptr, finite_only)) != MULLS_OK) return rc;
     CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(ctx->h_flags + 3, (const char *)A.ps + offsetof(PairState, n_tgt), sizeof(int), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    n_tgt = (int)ctx->h_flags[3];
     if (ctx->h_flags[1]) {
         if ((rc = grow_hash_pool(ctx)) != MULLS_OK) return rc;
         A.hash = ctx->A.hash, A.hash_pool_entries = ctx->A.hash_pool_entries;
-        if ((rc = launch_ingest(ctx, A, false, launches)) != MULLS_OK) return rc;
+        if ((rc = launch_ingest(ctx, A, false, launches, nullptr, nullptr, finite_only)) != MULLS_OK) return rc;
     }
+    return MULLS_OK;
+}
+
+// PCA features of one cloud (host rows, or rows already in HBM) into ctx->pca_buf; `args` receives the device arrays.
+// unit_dist > 0: distance-adaptive neighbourhoods (k_pca<true>). The PCA is not waited for: the caller consumes the
+// arrays on ctx->stream.
+static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_device, float radius, int k, int stride,
+                         PcaArgs &args, uint64_t &launches, float unit_dist = 0.f) {
+    const bool adaptive = unit_dist > 0.f;
+    // an adaptive radius grows without bound with the range: it needs the full level pyramid
+    DeviceArrays A;
+    int n_tgt = 0;
+    int rc = ingest_cloud(ctx, cloud, cloud_on_device, radius, adaptive, false, A, n_tgt, launches);
+    if (rc != MULLS_OK) return rc;
+    const size_t n = cloud.n;
+    ScratchLayout L;
+    const size_t o_ev = L.take(3 * n * sizeof(float)), o_pr = L.take(3 * n * sizeof(float)),
+                 o_nr = L.take(3 * n * sizeof(float)), o_num = L.take(n * sizeof(int)), outputs = L.bytes;
+    // k within the list capacity (the reference uses 20..50): the neighbour lists, and with them pcl::PCA's float mean /
+    // covariance accumulated in radiusSearch order — bit-reproducible against the CPU path; larger or unlimited k: fp64
+    // warp reduction
+    const bool lists = k >= 1 && k <= kPcaListCap;
+    const size_t o_nbr = lists ? L.take(n * (size_t)k * sizeof(uint32_t)) : 0;
+    char *base;
+    if ((rc = L.grow(ctx, ctx->pca_buf, base)) != MULLS_OK) return rc;
     args.radius = radius;
     args.r2 = (float)((double)radius * (double)radius);
     args.k = k;
     args.stride = stride;
-    args.eigenvalues = (float *)ctx->pca_buf.p;
-    args.principal = args.eigenvalues + 3 * n;
-    args.normal = args.principal + 3 * n;
-    args.pt_num = (int *)(args.normal + 3 * n);
-    args.nbr = nbr;
-    CK(cudaMemsetAsync(ctx->pca_buf.p, 0, std::max<size_t>(bytes, 16), st));
+    args.eigenvalues = (float *)(base + o_ev);
+    args.principal = (float *)(base + o_pr);
+    args.normal = (float *)(base + o_nr);
+    args.pt_num = (int *)(base + o_num);
+    args.nbr = lists ? (uint32_t *)(base + o_nbr) : nullptr;
+    cudaStream_t st = ctx->stream;
+    CK(cudaMemsetAsync(base, 0, outputs, st));
     if (n && adaptive) {
         PcaAdaptiveArgs aa;
         static_cast<PcaArgs &>(aa) = args;
@@ -1355,27 +1430,17 @@ static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_d
         k_pca<false><<<(unsigned)ceil_div(n, kPcaWarps), kPcaWarps * 32, 0, st>>>(A, args);
         ++launches;
     }
-    ctx->uploaded = false; // the resident batch was replaced by the PCA cloud
     return MULLS_OK;
 }
 
 // mulls_pca_features / mulls_pca_features_adaptive (unit_dist > 0)
 static int pca_features_impl(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int k, int stride, float unit_dist,
-                             mulls_pca_out *out) {
-    if (!ctx || !out || !out->eigenvalues || !out->principal || !out->normal || !out->pt_num || stride < 1 ||
-        !(radius > 0.f))
+                             mulls_pca_out *out, uint64_t &launches) {
+    if (!out || !out->eigenvalues || !out->principal || !out->normal || !out->pt_num || stride < 1 || !(radius > 0.f))
         return MULLS_E_ARG;
     PcaArgs args;
-    uint64_t launches = 0;
     const size_t n = cloud.n;
-    // k within the list capacity (the reference uses 20..50): pcl::PCA's float mean / covariance accumulated in
-    // radiusSearch order — bit-reproducible against the CPU path; larger or unlimited k: fp64 warp reduction
-    uint32_t *nbr = nullptr;
-    if (k >= 1 && k <= kPcaListCap && n > 0) {
-        if (const int rc = grow_scratch(ctx, ctx->cls_buf, n * (size_t)k * sizeof(uint32_t)); rc != MULLS_OK) return rc;
-        nbr = (uint32_t *)ctx->cls_buf.p;
-    }
-    int rc = pca_on_device(ctx, cloud, false, radius, k, stride, args, launches, nbr, unit_dist);
+    int rc = pca_on_device(ctx, cloud, false, radius, k, stride, args, launches, unit_dist);
     if (rc != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
     if (n) {
@@ -1384,81 +1449,52 @@ static int pca_features_impl(mulls_ctx *ctx, mulls_cloud_view cloud, float radiu
         CK(cudaMemcpyAsync(out->normal, args.normal, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(out->pt_num, args.pt_num, n * sizeof(int), cudaMemcpyDeviceToHost, st));
     }
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
-    ctx->stats = mulls_run_stats();
-    ctx->stats.kernel_launches = launches;
     return MULLS_OK;
 }
 
 extern "C" {
 
 int mulls_pca_features(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int k, int stride, mulls_pca_out *out) {
-    return pca_features_impl(ctx, cloud, radius, k, stride, 0.f, out);
+    return front_call(ctx, [&](uint64_t &launches) { return pca_features_impl(ctx, cloud, radius, k, stride, 0.f, out, launches); });
 }
 
 int mulls_pca_features_adaptive(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int k, int stride, float unit_dist,
                                 mulls_pca_out *out) {
-    if (!(unit_dist > 0.f)) return MULLS_E_ARG;
-    return pca_features_impl(ctx, cloud, radius, k, stride, unit_dist, out);
+    return front_call(ctx, [&](uint64_t &launches) {
+        return unit_dist > 0.f ? pca_features_impl(ctx, cloud, radius, k, stride, unit_dist, out, launches) : MULLS_E_ARG;
+    });
 }
 
 // ================================================================================================
 // Statistical outlier removal (CFilter::sor_filter, cfilter.hpp:203-247): kernels_sor.cuh
 // ================================================================================================
 static int sor_filter_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double n_std, uint8_t *keep_bits, float *mean_dist,
-                           mulls_sor_stats *stats) {
-    if (!ctx || mean_k < 1 || mean_k > kSorMaxMeanK || (cloud.n > 0 && (!cloud.aos48 || !keep_bits))) return MULLS_E_ARG;
+                           mulls_sor_stats *stats, uint64_t &launches) {
+    if (mean_k < 1 || mean_k > kSorMaxMeanK || (cloud.n > 0 && (!cloud.aos48 || !keep_bits))) return MULLS_E_ARG;
     const size_t n = cloud.n;
-    if (n > ctx->max_tgt) {
-        ctx->err = "mulls_sor_filter: the cloud exceeds max_tgt_pts of the context";
-        return MULLS_E_CAPACITY;
-    }
+    int rc = check_capacity(ctx, n, "mulls_sor_filter");
+    if (rc != MULLS_OK) return rc;
     if (n <= (size_t)mean_k) { // (checked again on the finite points after the ingest)
         ctx->err = "mulls_sor_filter: the cloud needs more than mean_k finite points";
         return MULLS_E_ARG;
     }
-    // the cloud becomes the only target class of a one-pair batch; normal_shooting_on asks k_pair_setup for the full
-    // level pyramid, whose top block spans the whole grid (the search has no radius)
-    mulls_icp_params P;
-    mulls_icp_default_params(&P);
-    std::strcpy(P.used_feature_type, "100000");
-    P.apply_intersection_filter = 0;
-    P.normal_shooting_on = 1;
-    P.max_iter_num = 0;
-    mulls_cloud_view tgt[MULLS_NUM_CLASSES] = {cloud, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
-    mulls_cloud_view src[MULLS_NUM_CLASSES] = {{nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
-    const double ident[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    int rc = upload_impl(ctx, 1, tgt, src, &P, ident, nullptr, nullptr, /*resident=*/false);
-    ctx->uploaded = false; // the resident batch is replaced by the cloud
-    if (rc != MULLS_OK) return rc;
-    const size_t words = ceil_div(n, 32);
-    const size_t off_bits = ceil_div(n * sizeof(float), 16) * 16, off_stats = off_bits + ceil_div(words * 4, 16) * 16;
-    if ((rc = grow_scratch(ctx, ctx->sor_buf, off_stats + sizeof(mulls_sor_stats))) != MULLS_OK) return rc;
-    float *d_dist = (float *)ctx->sor_buf.p;
-    uint32_t *d_keep = (uint32_t *)((char *)ctx->sor_buf.p + off_bits);
-    mulls_sor_stats *d_stats = (mulls_sor_stats *)((char *)ctx->sor_buf.p + off_stats);
-    cudaStream_t st = ctx->stream;
-    DeviceArrays A = ctx->A;
-    A.trace = nullptr;
-    uint64_t launches = 0;
-    if ((rc = launch_ingest(ctx, A, false, launches, nullptr, nullptr, /*finite_only=*/true)) != MULLS_OK) return rc;
-    // the grid must fit the hash pool before the search reads it (else grow the pool and build the grid again from the
-    // cloud already in HBM), and the finite points must be more than mean_k
+    // the search has no radius: the full level pyramid; the finite points must be more than mean_k
+    DeviceArrays A;
     int n_valid = 0;
-    CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&n_valid, (const char *)A.ps + offsetof(PairState, n_tgt), sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (ctx->h_flags[1]) {
-        if ((rc = grow_hash_pool(ctx)) != MULLS_OK) return rc;
-        A.hash = ctx->A.hash, A.hash_pool_entries = ctx->A.hash_pool_entries;
-        if ((rc = launch_ingest(ctx, A, false, launches, nullptr, nullptr, true)) != MULLS_OK) return rc;
-    }
+    if ((rc = ingest_cloud(ctx, cloud, false, 0.f, true, /*finite_only=*/true, A, n_valid, launches)) != MULLS_OK) return rc;
     if (n_valid <= mean_k) {
         ctx->err = "mulls_sor_filter: " + std::to_string(n_valid) + " finite points, mean_k + 1 = " + std::to_string(mean_k + 1) +
                    " neighbours wanted per point";
         return MULLS_E_ARG;
     }
+    ScratchLayout L;
+    const size_t o_dist = L.take(n * sizeof(float)), o_keep = L.take(ceil_div(n, 32) * 4), o_stats = L.take(sizeof(mulls_sor_stats));
+    char *base;
+    if ((rc = L.grow(ctx, ctx->sor_buf, base)) != MULLS_OK) return rc;
+    float *d_dist = (float *)(base + o_dist);
+    uint32_t *d_keep = (uint32_t *)(base + o_keep);
+    mulls_sor_stats *d_stats = (mulls_sor_stats *)(base + o_stats);
+    cudaStream_t st = ctx->stream;
     CK(cudaMemsetAsync(d_dist, 0, n * sizeof(float), st)); // non-finite points: distance 0, as PCL
     const unsigned nb = (unsigned)ceil_div((size_t)n_valid, kSorBlock);
     if (mean_k + 1 <= 16) k_sor_dist<16><<<nb, kSorBlock, 0, st>>>(A, mean_k, d_dist);
@@ -1467,23 +1503,16 @@ static int sor_filter_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, d
     k_sor_stats<<<1, 32, 0, st>>>(A, d_dist, (uint32_t)n, n_std, d_stats);
     k_sor_mark<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(d_dist, (uint32_t)n, d_stats, d_keep);
     launches += 3;
-    CK(cudaGetLastError());
-    mulls_sor_stats h_stats;
     CK(cudaMemcpyAsync(keep_bits, d_keep, (n + 7) / 8, cudaMemcpyDeviceToHost, st));
     if (mean_dist) CK(cudaMemcpyAsync(mean_dist, d_dist, n * sizeof(float), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&h_stats, d_stats, sizeof(h_stats), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (stats) *stats = h_stats;
-    ctx->stats = mulls_run_stats();
-    ctx->stats.kernel_launches = launches;
+    if (stats) CK(cudaMemcpyAsync(stats, d_stats, sizeof(*stats), cudaMemcpyDeviceToHost, st));
     return MULLS_OK;
 }
 int mulls_sor_filter(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double n_std, uint8_t *keep_bits, float *mean_dist,
                      mulls_sor_stats *stats) {
-    const int rc = sor_filter_impl(ctx, cloud, mean_k, n_std, keep_bits, mean_dist, stats);
-    // an error exit may leave the copy of the caller's cloud in flight: nothing is handed back before the stream drains
-    if (rc != MULLS_OK && ctx && ctx->stream) cudaStreamSynchronize(ctx->stream);
-    return rc;
+    return front_call(ctx, [&](uint64_t &launches) {
+        return sor_filter_impl(ctx, cloud, mean_k, n_std, keep_bits, mean_dist, stats, launches);
+    });
 }
 
 // ================================================================================================
@@ -1495,37 +1524,25 @@ int mulls_sor_filter(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double 
 // one after the other
 static int raw_upload(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, size_t n_total, int out_floats,
                       float **d_rows, float **d_out, TsState **d_st) {
-    const size_t off_out = n_total * 48, off_st = off_out + ceil_div(n_total * out_floats * sizeof(float), 16) * 16;
-    int rc = grow_scratch(ctx, ctx->raw_buf, off_st + sizeof(TsState));
+    ScratchLayout L;
+    const size_t o_rows = L.take(n_total * 48), o_out = L.take(n_total * out_floats * sizeof(float)), o_st = L.take(sizeof(TsState));
+    char *base;
+    int rc = L.grow(ctx, ctx->raw_buf, base);
     if (rc != MULLS_OK) return rc;
-    char *base = (char *)ctx->raw_buf.p;
-    *d_rows = (float *)base, *d_out = (float *)(base + off_out), *d_st = (TsState *)(base + off_st);
+    *d_rows = (float *)(base + o_rows), *d_out = (float *)(base + o_out), *d_st = (TsState *)(base + o_st);
     size_t at = 0;
     for (int c = 0; c < n_clouds; ++c) {
-        if (clouds[c].n) CK(cudaMemcpyAsync(base + at * 48, clouds[c].aos48, clouds[c].n * 48, cudaMemcpyHostToDevice, ctx->stream));
+        if (clouds[c].n)
+            CK(cudaMemcpyAsync(*d_rows + at * 12, clouds[c].aos48, clouds[c].n * 48, cudaMemcpyHostToDevice, ctx->stream));
         at += clouds[c].n;
     }
     return MULLS_OK;
 }
 
-static int raw_capacity(mulls_ctx *ctx, size_t n, const char *fn) {
-    if (n <= ctx->max_tgt) return MULLS_OK;
-    ctx->err = std::string(fn) + ": " + std::to_string(n) + " points exceed max_tgt_pts of the context";
-    return MULLS_E_CAPACITY;
-}
-
-static int raw_finish(mulls_ctx *ctx, uint64_t launches) {
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(ctx->stream));
-    ctx->stats = mulls_run_stats();
-    ctx->stats.kernel_launches = launches;
-    return MULLS_OK;
-}
-
 static int vertical_calib_impl(mulls_ctx *ctx, mulls_cloud_view cloud, double var_vertical_ang_d, int inverse_z, float *xyz_out,
-                               int *applied) {
-    if (!ctx || !applied || (cloud.n > 0 && (!cloud.aos48 || !xyz_out))) return MULLS_E_ARG;
-    int rc = raw_capacity(ctx, cloud.n, "mulls_vertical_intrinsic_calibration");
+                               int *applied, uint64_t &launches) {
+    if (!applied || (cloud.n > 0 && (!cloud.aos48 || !xyz_out))) return MULLS_E_ARG;
+    int rc = check_capacity(ctx, cloud.n, "mulls_vertical_intrinsic_calibration");
     if (rc != MULLS_OK) return rc;
     *applied = 0;
     if (var_vertical_ang_d == 0) { // :252-253: the cloud is left as it is
@@ -1541,17 +1558,17 @@ static int vertical_calib_impl(mulls_ctx *ctx, mulls_cloud_view cloud, double va
         const double var_rad = var_vertical_ang_d / 180.0 * M_PI;
         k_vertical_calib<<<(unsigned)ceil_div(cloud.n, kRawBlock), kRawBlock, 0, ctx->stream>>>(d_rows, (uint32_t)cloud.n, var_rad,
                                                                                                 negate_only, d_out);
+        ++launches;
         CK(cudaMemcpyAsync(xyz_out, d_out, cloud.n * 3 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-        if ((rc = raw_finish(ctx, 1)) != MULLS_OK) return rc;
     }
     *applied = negate_only ? 0 : 1;
     return MULLS_OK;
 }
 
 static int timestamp_ratio_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int timestamp_available, double scan_begin_ang_deg,
-                                float scan_duration_ms, float *ratio_out) {
-    if (!ctx || (cloud.n > 0 && (!cloud.aos48 || !ratio_out))) return MULLS_E_ARG;
-    int rc = raw_capacity(ctx, cloud.n, "mulls_timestamp_ratio");
+                                float scan_duration_ms, float *ratio_out, uint64_t &launches) {
+    if (cloud.n > 0 && (!cloud.aos48 || !ratio_out)) return MULLS_E_ARG;
+    int rc = check_capacity(ctx, cloud.n, "mulls_timestamp_ratio");
     if (rc != MULLS_OK) return rc;
     const size_t n = cloud.n;
     if (n == 0) return MULLS_OK;
@@ -1560,7 +1577,6 @@ static int timestamp_ratio_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int time
     if ((rc = raw_upload(ctx, &cloud, 1, n, 1, &d_rows, &d_out, &d_st)) != MULLS_OK) return rc;
     const unsigned nb = (unsigned)ceil_div(n, kRawBlock);
     cudaStream_t st = ctx->stream;
-    uint64_t launches = 0;
     if (timestamp_available) {
         TsState init{};
         init.min_key = ~0ull;
@@ -1569,24 +1585,24 @@ static int timestamp_ratio_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int time
         k_ts_extremes<9><<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st);
         k_ts_setup<<<1, 32, 0, st>>>(d_rows, (uint32_t)n, scan_duration_ms, d_st);
         k_ts_ratio<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, d_st, d_out);
-        launches = 4;
+        launches += 4;
     } else {
         k_azimuth_ratio<<<nb, kRawBlock, 0, st>>>(d_rows, (uint32_t)n, scan_begin_ang_deg / 180.0 * M_PI, d_out);
-        launches = 1;
+        launches += 1;
     }
     CK(cudaMemcpyAsync(ratio_out, d_out, n * sizeof(float), cudaMemcpyDeviceToHost, st));
-    return raw_finish(ctx, launches);
+    return MULLS_OK;
 }
 
 static int motion_compensation_impl(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, const double *T,
-                                    float s_ambiguous_thre, float *const *xyz_out) {
-    if (!ctx || !clouds || !T || !xyz_out || n_clouds < 1 || n_clouds > MULLS_NUM_CLASSES) return MULLS_E_ARG;
+                                    float s_ambiguous_thre, float *const *xyz_out, uint64_t &launches) {
+    if (!clouds || !T || !xyz_out || n_clouds < 1 || n_clouds > MULLS_NUM_CLASSES) return MULLS_E_ARG;
     size_t n = 0;
     for (int c = 0; c < n_clouds; ++c) {
         if (clouds[c].n > 0 && (!clouds[c].aos48 || !xyz_out[c])) return MULLS_E_ARG;
         n += clouds[c].n;
     }
-    int rc = raw_capacity(ctx, n, "mulls_motion_compensation");
+    int rc = check_capacity(ctx, n, "mulls_motion_compensation");
     if (rc != MULLS_OK || n == 0) return rc;
     float *d_rows, *d_out;
     TsState *d_st;
@@ -1594,31 +1610,33 @@ static int motion_compensation_impl(mulls_ctx *ctx, const mulls_cloud_view *clou
     const SlerpConst sc = slerp_const_of(T);
     k_motion_compensation<<<(unsigned)ceil_div(n, kRawBlock), kRawBlock, 0, ctx->stream>>>(d_rows, (uint32_t)n, sc, s_ambiguous_thre,
                                                                                            d_out);
+    ++launches;
     size_t at = 0;
     for (int c = 0; c < n_clouds; ++c) {
         if (clouds[c].n)
             CK(cudaMemcpyAsync(xyz_out[c], d_out + 3 * at, clouds[c].n * 3 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
         at += clouds[c].n;
     }
-    return raw_finish(ctx, 1);
+    return MULLS_OK;
 }
 
-// an error exit may leave a copy in flight: nothing is handed back before the stream drains
-static int raw_drain(mulls_ctx *ctx, int rc) {
-    if (rc != MULLS_OK && ctx && ctx->stream) cudaStreamSynchronize(ctx->stream);
-    return rc;
-}
 int mulls_vertical_intrinsic_calibration(mulls_ctx *ctx, mulls_cloud_view cloud, double var_vertical_ang_d, int inverse_z,
                                          float *xyz_out, int *applied) {
-    return raw_drain(ctx, vertical_calib_impl(ctx, cloud, var_vertical_ang_d, inverse_z, xyz_out, applied));
+    return front_call(ctx, [&](uint64_t &launches) {
+        return vertical_calib_impl(ctx, cloud, var_vertical_ang_d, inverse_z, xyz_out, applied, launches);
+    });
 }
 int mulls_timestamp_ratio(mulls_ctx *ctx, mulls_cloud_view cloud, int timestamp_available, double scan_begin_ang_deg,
                           float scan_duration_ms, float *ratio_out) {
-    return raw_drain(ctx, timestamp_ratio_impl(ctx, cloud, timestamp_available, scan_begin_ang_deg, scan_duration_ms, ratio_out));
+    return front_call(ctx, [&](uint64_t &launches) {
+        return timestamp_ratio_impl(ctx, cloud, timestamp_available, scan_begin_ang_deg, scan_duration_ms, ratio_out, launches);
+    });
 }
 int mulls_motion_compensation(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, const double T[16],
                               float s_ambiguous_thre, float *const *xyz_out) {
-    return raw_drain(ctx, motion_compensation_impl(ctx, clouds, n_clouds, T, s_ambiguous_thre, xyz_out));
+    return front_call(ctx, [&](uint64_t &launches) {
+        return motion_compensation_impl(ctx, clouds, n_clouds, T, s_ambiguous_thre, xyz_out, launches);
+    });
 }
 
 // ================================================================================================
@@ -1626,14 +1644,14 @@ int mulls_motion_compensation(mulls_ctx *ctx, const mulls_cloud_view *clouds, in
 // Stateless like the raw-scan corrections: the resident batch and its grid are left alone.
 // ================================================================================================
 static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, int fixed_num_corr, int corr_num, int reciprocal_on,
-                    int32_t *tgt_idx, int32_t *src_idx, size_t cap, size_t *n_out, int *performed) {
-    if (!ctx || !n_out || !performed || (tk.n && !tk.aos48) || (sk.n && !sk.aos48) || (cap && (!tgt_idx || !src_idx)))
+                    int32_t *tgt_idx, int32_t *src_idx, size_t cap, size_t *n_out, int *performed, uint64_t &launches) {
+    if (!n_out || !performed || (tk.n && !tk.aos48) || (sk.n && !sk.aos48) || (cap && (!tgt_idx || !src_idx)))
         return MULLS_E_ARG;
     *n_out = 0;
     *performed = 0;
     const char *fn = "mulls_ncc_correspondences";
     int rc;
-    if ((rc = raw_capacity(ctx, tk.n, fn)) != MULLS_OK || (rc = raw_capacity(ctx, sk.n, fn)) != MULLS_OK) return rc;
+    if ((rc = check_capacity(ctx, tk.n, fn)) != MULLS_OK || (rc = check_capacity(ctx, sk.n, fn)) != MULLS_OK) return rc;
     const size_t nt = tk.n, ns = sk.n, n_all = nt + ns;
     if (nt < 10 || ns < 10) return MULLS_OK; // :421-425
     const size_t M = nt * ns;
@@ -1652,30 +1670,24 @@ static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, in
         return MULLS_E_CAPACITY;
     }
     cudaStream_t st = ctx->stream;
-    // ncc_buf, 256-byte aligned pieces
-    size_t off = 0;
-    auto piece = [&off](size_t bytes) {
-        const size_t o = off;
-        off += ceil_div(std::max<size_t>(bytes, 1), 256) * 256;
-        return o;
-    };
-    const size_t o_rows = piece(n_all * 48), o_desc = piece(n_all * kNccDim * sizeof(float)), o_ts = piece(sizeof(TsState)),
-                 o_range = piece(2 * sizeof(float));
+    ScratchLayout L;
+    const size_t o_rows = L.take(n_all * 48), o_desc = L.take(n_all * kNccDim * sizeof(float)), o_ts = L.take(sizeof(TsState)),
+                 o_range = L.take(2 * sizeof(float));
     size_t o_rowkey = 0, o_colmin = 0, o_cand = 0, o_keep = 0, o_sel = 0, o_out = 0, o_num = 0, o_gath = 0, o_sorted = 0, o_tmp = 0;
     size_t tmp_bytes = 0;
     if (!fixed_num_corr) {
-        o_rowkey = piece(nt * 8), o_colmin = piece(ns * 4), o_cand = piece(nt * 8), o_keep = piece(nt), o_out = piece(nt * 8);
-        o_num = piece(sizeof(int));
+        o_rowkey = L.take(nt * 8), o_colmin = L.take(ns * 4), o_cand = L.take(nt * 8), o_keep = L.take(nt), o_out = L.take(nt * 8);
+        o_num = L.take(sizeof(int));
         CK(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, (unsigned long long *)nullptr, (uint8_t *)nullptr,
                                       (unsigned long long *)nullptr, (int *)nullptr, (int)nt, st));
     } else {
-        o_sel = piece(sizeof(NccSelect)), o_gath = piece(K * 8), o_sorted = piece(K * 8);
+        o_sel = L.take(sizeof(NccSelect)), o_gath = L.take(K * 8), o_sorted = L.take(K * 8);
         CK(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr,
                                           (int)std::max<size_t>(K, 1), 0, 64, st));
     }
-    o_tmp = piece(tmp_bytes);
-    if ((rc = grow_scratch(ctx, ctx->ncc_buf, off)) != MULLS_OK) return rc;
-    char *base = (char *)ctx->ncc_buf.p;
+    o_tmp = L.take(tmp_bytes);
+    char *base;
+    if ((rc = L.grow(ctx, ctx->ncc_buf, base)) != MULLS_OK) return rc;
     float *d_rows = (float *)(base + o_rows), *d_desc = (float *)(base + o_desc), *d_range = (float *)(base + o_range);
     TsState *d_ts = (TsState *)(base + o_ts);
     CK(cudaMemcpyAsync(d_rows, tk.aos48, nt * 48, cudaMemcpyHostToDevice, st));
@@ -1688,7 +1700,7 @@ static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, in
     k_ts_extremes<8><<<nbt, kRawBlock, 0, st>>>(d_rows, (uint32_t)nt, d_ts);
     k_ncc_range<<<1, 32, 0, st>>>(d_rows, (uint32_t)nt, d_ts, d_range);
     k_ncc_descriptors<<<(unsigned)ceil_div(n_all, kRawBlock), kRawBlock, 0, st>>>(d_rows, (uint32_t)n_all, d_range, d_desc);
-    uint64_t launches = 4;
+    launches += 4;
     const NccPairs P{d_desc, (uint32_t)n_all, (uint32_t)nt, (uint32_t)ns};
     const dim3 grid((unsigned)ceil_div(nt, kNccTileT), (unsigned)gy);
     std::vector<std::pair<int32_t, int32_t>> res;
@@ -1774,15 +1786,15 @@ static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, in
     for (size_t k = 0; k < res.size(); ++k) tgt_idx[k] = res[k].first, src_idx[k] = res[k].second;
     *n_out = res.size();
     *performed = 1;
-    ctx->stats = mulls_run_stats();
-    ctx->stats.kernel_launches = launches;
     return MULLS_OK;
 }
 int mulls_ncc_correspondences(mulls_ctx *ctx, mulls_cloud_view target_kpts, mulls_cloud_view source_kpts, int fixed_num_corr,
                               int corr_num, int reciprocal_on, int32_t *tgt_idx, int32_t *src_idx, size_t cap, size_t *n_out,
                               int *performed) {
-    return raw_drain(ctx, ncc_impl(ctx, target_kpts, source_kpts, fixed_num_corr, corr_num, reciprocal_on, tgt_idx, src_idx, cap,
-                                   n_out, performed));
+    return front_call(ctx, [&](uint64_t &launches) {
+        return ncc_impl(ctx, target_kpts, source_kpts, fixed_num_corr, corr_num, reciprocal_on, tgt_idx, src_idx, cap, n_out,
+                        performed, launches);
+    });
 }
 
 // ================================================================================================
@@ -1796,8 +1808,8 @@ static constexpr int kRcFirstChunk = 64;
 static constexpr int kRcChunk = 4096;
 
 static int ransac_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, float noise_bound, int min_inlier_num,
-                       int max_iter_num, double *tran_mat, int *status, int *n_inliers, int *n_hypotheses) {
-    if (!ctx || !tran_mat || !status || !n_inliers || !n_hypotheses || (tv.n && !tv.aos48) || (sv.n && !sv.aos48))
+                       int max_iter_num, double *tran_mat, int *status, int *n_inliers, int *n_hypotheses, uint64_t &launches) {
+    if (!tran_mat || !status || !n_inliers || !n_hypotheses || (tv.n && !tv.aos48) || (sv.n && !sv.aos48))
         return MULLS_E_ARG;
     const char *fn = "mulls_coarse_reg_ransac";
     const size_t N = tv.n;
@@ -1806,7 +1818,7 @@ static int ransac_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv,
         return MULLS_E_ARG;
     }
     int rc;
-    if ((rc = raw_capacity(ctx, N, fn)) != MULLS_OK) return rc;
+    if ((rc = check_capacity(ctx, N, fn)) != MULLS_OK) return rc;
     if (N > (size_t)INT_MAX) {
         ctx->err = std::string(fn) + ": more than INT_MAX correspondences";
         return MULLS_E_ARG;
@@ -1819,22 +1831,16 @@ static int ransac_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv,
     float T[12] = {1.f, 0.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, 1.f, 0.f}; // identity
     size_t n_final = 0;
     int hyps = 0;
-    uint64_t launches = 0;
     if (N > 0) { // an empty correspondence list returns before the rejector runs (getCorrespondences)
         cudaStream_t st = ctx->stream;
-        size_t off = 0;
-        auto piece = [&off](size_t bytes) {
-            const size_t o = off;
-            off += ceil_div(std::max<size_t>(bytes, 1), 256) * 256;
-            return o;
-        };
-        const size_t o_corr = piece(N * 6 * sizeof(float)), o_samp = piece(2 * kRcChunk * 3 * sizeof(int)),
-                     o_T = piece(2 * (size_t)kRcChunk * 12 * sizeof(float)), o_cnt = piece(2 * kRcChunk * sizeof(int)),
-                     o_best = piece(12 * sizeof(float)), o_fa = piece(N), o_fb = piece(N), o_err = piece(N * sizeof(float)),
-                     o_out = piece(sizeof(RcRefineOut));
-        if ((rc = grow_scratch(ctx, ctx->rc_buf, off)) != MULLS_OK) return rc;
+        ScratchLayout L;
+        const size_t o_corr = L.take(N * 6 * sizeof(float)), o_samp = L.take(2 * kRcChunk * 3 * sizeof(int)),
+                     o_T = L.take(2 * (size_t)kRcChunk * 12 * sizeof(float)), o_cnt = L.take(2 * kRcChunk * sizeof(int)),
+                     o_best = L.take(12 * sizeof(float)), o_fa = L.take(N), o_fb = L.take(N), o_err = L.take(N * sizeof(float)),
+                     o_out = L.take(sizeof(RcRefineOut));
+        char *base;
+        if ((rc = L.grow(ctx, ctx->rc_buf, base)) != MULLS_OK) return rc;
         if (!ctx->rc_host) CK(cudaMallocHost(&ctx->rc_host, 2 * kRcChunk * 4 * sizeof(int)));
-        char *base = (char *)ctx->rc_buf.p;
         float *d_corr = (float *)(base + o_corr), *d_best = (float *)(base + o_best);
         int *h_samp[2] = {(int *)ctx->rc_host, (int *)ctx->rc_host + 3 * kRcChunk};
         int *h_cnt[2] = {(int *)ctx->rc_host + 6 * kRcChunk, (int *)ctx->rc_host + 7 * kRcChunk};
@@ -1932,15 +1938,15 @@ static int ransac_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv,
     *status = stat;
     *n_inliers = (int)n_final;
     *n_hypotheses = hyps;
-    ctx->stats = mulls_run_stats();
-    ctx->stats.kernel_launches = launches;
     return MULLS_OK;
 }
 int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_cloud_view source_pts, float noise_bound,
                             int min_inlier_num, int max_iter_num, double tran_mat[16], int *status, int *n_inliers,
                             int *n_hypotheses) {
-    return raw_drain(ctx, ransac_impl(ctx, target_pts, source_pts, noise_bound, min_inlier_num, max_iter_num, tran_mat, status,
-                                      n_inliers, n_hypotheses));
+    return front_call(ctx, [&](uint64_t &launches) {
+        return ransac_impl(ctx, target_pts, source_pts, noise_bound, min_inlier_num, max_iter_num, tran_mat, status, n_inliers,
+                           n_hypotheses, launches);
+    });
 }
 
 // ================================================================================================
@@ -2252,9 +2258,7 @@ int mulls_map_update(mulls_map *m, const mulls_cloud_view scan_down[MULLS_NUM_CL
             mulls_cloud_view v{(const float *)m->buf[m->cur][c], m->n[c]};
             PcaArgs args;
             uint64_t launches = 0;
-            if (const int rc = grow_scratch(ctx, ctx->cls_buf, (size_t)m->n[c] * pca_max_k * sizeof(uint32_t)); rc != MULLS_OK)
-                return rc;
-            const int rc = pca_on_device(ctx, v, true, pca_radius, pca_max_k, 1, args, launches, (uint32_t *)ctx->cls_buf.p);
+            const int rc = pca_on_device(ctx, v, true, pca_radius, pca_max_k, 1, args, launches);
             if (rc != MULLS_OK) return rc;
             k_map_revector<<<1, kMapBlock, 0, st>>>(m->buf[m->cur][c], m->n[c], args, pca_min_k, lo[k], hi[k], min_linearity,
                                                    m->mid[c], &m->d_state->n_out[c]);
@@ -2335,9 +2339,9 @@ void mulls_classify_default_params(mulls_classify_params *p) {
     p->pca_unit_distance = 0.f;
 }
 
-int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_classify_params *params,
-                           mulls_classify_out *out) {
-    if (!ctx || !params || !out || (cloud_in.n > 0 && !cloud_in.aos48)) return MULLS_E_ARG;
+static int classify_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_classify_params *params, mulls_classify_out *out,
+                         uint64_t &launches) {
+    if (!params || !out || (cloud_in.n > 0 && !cloud_in.aos48)) return MULLS_E_ARG;
     const mulls_classify_params &P = *params;
     // the reference names two units (30 at cfilter.hpp:2093, 35 as get_pc_pca_feature's default): the caller picks one
     if (P.use_distance_adaptive_pca && !(P.pca_unit_distance > 0.f)) {
@@ -2352,33 +2356,25 @@ int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mull
     for (int k = 0; k < MULLS_OUT_COUNT; ++k) out->n[k] = 0;
     const size_t n0 = cloud_in.n;
     if (n0 == 0) return MULLS_OK;
-    if (n0 > ctx->max_tgt) {
-        ctx->err = "mulls_classify_nground: cloud exceeds max_tgt_pts of the context";
-        return MULLS_E_CAPACITY;
-    }
-    CK(cudaSetDevice(ctx->device));
+    if (const int rc = check_capacity(ctx, n0, "mulls_classify_nground"); rc != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
     // :2086-2087 random_downsample_pcl(cloud_in, unground_down_fixed_num): the size it leaves is known up front
     size_t n = n0;
     const bool sample_in = P.fixed_num_downsampling && P.unground_down_fixed_num >= 0 && n0 > (size_t)P.unground_down_fixed_num;
     if (sample_in) n = (size_t)P.unground_down_fixed_num;
     const int stride = P.pca_down_rate > 0 ? P.pca_down_rate : 1;
-    // scratch layout
     const size_t row_b = 48;
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        const size_t o = off;
-        off += (bytes + 255) / 256 * 256;
-        return o;
-    };
-    const size_t o_in = take(n0 * row_b), o_rows = take(n0 * row_b);
+    ScratchLayout L;
+    const size_t o_in = L.take(n0 * row_b), o_rows = L.take(n0 * row_b);
     size_t o_cls[4], o_srt[4], o_dn[4], o_dn2[4];
-    for (int c = 0; c < 4; ++c) o_cls[c] = take(n0 * row_b), o_srt[c] = take(n0 * row_b), o_dn[c] = take(n0 * row_b), o_dn2[c] = take(n0 * row_b);
-    const size_t o_sect = take(2 * n0 * row_b), o_vrows = take(n0 * row_b), o_vertex = take(n0 * row_b);
-    const size_t o_sel = take(4 * n0 * sizeof(float4)), o_nbr = take(n0 * (size_t)P.neighbor_k * sizeof(uint32_t));
-    const size_t o_l0 = take(n0), o_l = take(n0), o_df = take(n0), o_s4 = take(n0), o_vf = take(n0), o_st = take(sizeof(ClsState));
-    if (const int rc = grow_scratch(ctx, ctx->cls_buf, off); rc != MULLS_OK) return rc;
-    char *base = (char *)ctx->cls_buf.p;
+    for (int c = 0; c < 4; ++c)
+        o_cls[c] = L.take(n0 * row_b), o_srt[c] = L.take(n0 * row_b), o_dn[c] = L.take(n0 * row_b), o_dn2[c] = L.take(n0 * row_b);
+    const size_t o_sect = L.take(2 * n0 * row_b), o_vrows = L.take(n0 * row_b), o_vertex = L.take(n0 * row_b);
+    const size_t o_sel = L.take(4 * n0 * sizeof(float4));
+    const size_t o_l0 = L.take(n0), o_l = L.take(n0), o_df = L.take(n0), o_s4 = L.take(n0), o_vf = L.take(n0),
+                 o_st = L.take(sizeof(ClsState));
+    char *base;
+    if (const int rc = L.grow(ctx, ctx->cls_buf, base); rc != MULLS_OK) return rc;
     ClsArgs C;
     std::memset(&C, 0, sizeof(C));
     C.P = P;
@@ -2401,10 +2397,7 @@ int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mull
     C.st4 = (uint8_t *)(base + o_s4);
     C.vflag = (uint8_t *)(base + o_vf);
     C.st = (ClsState *)(base + o_st);
-    uint32_t *nbr = (uint32_t *)(base + o_nbr);
-    CK(cudaEventRecord(ctx->ev_begin, st));
     CK(cudaMemsetAsync(C.st, 0, sizeof(ClsState), st));
-    uint64_t launches = 0;
     if (sample_in) {
         CK(cudaMemcpyAsync(base + o_in, cloud_in.aos48, n0 * row_b, cudaMemcpyDefault, st)); // host or device rows
         k_rows_sample<<<1, kClsBlock, 0, st>>>((const float4 *)(base + o_in), (uint32_t)n0, P.unground_down_fixed_num, P.random_seed,
@@ -2418,8 +2411,7 @@ int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mull
     if (n > 0) {
         // :2089-2097 PCA of every pca_down_rate-th point, with the neighbour lists
         mulls_cloud_view v{(const float *)C.rows, n};
-        const int rc = pca_on_device(ctx, v, true, P.neighbor_searching_radius, P.neighbor_k, stride, C.F, launches, nbr,
-                                     unit_dist);
+        const int rc = pca_on_device(ctx, v, true, P.neighbor_searching_radius, P.neighbor_k, stride, C.F, launches, unit_dist);
         if (rc != MULLS_OK) return rc;
         C.keys_a = ctx->A.keys_a;
         C.keys_b = ctx->A.keys_b;
@@ -2470,12 +2462,12 @@ int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mull
         }
         CK(cudaMemcpyAsync(out->rows[k], src[k], cnt[k] * row_b, cudaMemcpyDefault, st));
     }
-    CK(cudaEventRecord(ctx->ev_end, st));
-    CK(cudaStreamSynchronize(st));
-    ctx->stats = mulls_run_stats();
-    ctx->stats.kernel_launches = launches;
-    cudaEventElapsedTime(&ctx->stats.ms_total, ctx->ev_begin, ctx->ev_end);
     return MULLS_OK;
+}
+
+int mulls_classify_nground(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_classify_params *params,
+                           mulls_classify_out *out) {
+    return front_call(ctx, [&](uint64_t &launches) { return classify_impl(ctx, cloud_in, params, out, launches); });
 }
 
 } // extern "C"
@@ -2528,9 +2520,9 @@ void mulls_ground_default_params(mulls_ground_params *p) { // extract_semantic_p
     p->random_seed = 0;
 }
 
-int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_ground_params *params,
-                             mulls_ground_out *out) {
-    if (!ctx || !params || !out || (cloud_in.n > 0 && !cloud_in.aos48)) return MULLS_E_ARG;
+static int ground_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_ground_params *params, mulls_ground_out *out,
+                       uint64_t &launches) {
+    if (!params || !out || (cloud_in.n > 0 && !cloud_in.aos48)) return MULLS_E_ARG;
     const mulls_ground_params &P = *params;
     if (P.estimate_ground_normal_method != 0 && P.estimate_ground_normal_method != 3) {
         ctx->err = "mulls_fast_ground_filter: estimate_ground_normal_method 1 / 2 (pcl::NormalEstimation) are not implemented";
@@ -2544,11 +2536,7 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
     out->n_ground = out->n_ground_down = out->n_unground = 0;
     const size_t n = cloud_in.n;
     if (n == 0) return MULLS_OK;
-    if (n > ctx->max_tgt || n >= (1ull << 31)) {
-        ctx->err = "mulls_fast_ground_filter: cloud exceeds max_tgt_pts of the context";
-        return MULLS_E_CAPACITY;
-    }
-    CK(cudaSetDevice(ctx->device));
+    if (const int rc = check_capacity(ctx, n, "mulls_fast_ground_filter"); rc != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
     // temporary storage of the library sort / scans
     size_t sort_bytes = 0, scan_bytes = 0;
@@ -2557,19 +2545,16 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
     cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, st);
     // per-point scratch
     const size_t row_b = 48;
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        const size_t o = off;
-        off += (bytes + 255) / 256 * 256;
-        return o;
-    };
-    const size_t o_rows = take(n * row_b), o_g = take(n * row_b), o_gd = take(n * row_b), o_u = take(n * row_b);
-    const size_t o_key = take(4 * n), o_idx = take(4 * n), o_keys = take(4 * n), o_idxs = take(4 * n), o_call = take(4 * n);
-    const size_t o_hf = take(4 * n), o_hp = take(4 * n), o_dec = take(n), o_cand = take(16 * n), o_shuf = take(4 * n), o_inl = take(n);
-    const size_t o_st = take(sizeof(GfState)), o_draws = take(kSacDraws * sizeof(uint32_t));
-    const size_t o_tmp = take(std::max(sort_bytes, scan_bytes));
-    if (const int rc = grow_scratch(ctx, ctx->gf_buf, off); rc != MULLS_OK) return rc;
-    char *base = (char *)ctx->gf_buf.p;
+    ScratchLayout L;
+    const size_t o_rows = L.take(n * row_b), o_g = L.take(n * row_b), o_gd = L.take(n * row_b), o_u = L.take(n * row_b);
+    const size_t o_key = L.take(4 * n), o_idx = L.take(4 * n), o_keys = L.take(4 * n), o_idxs = L.take(4 * n),
+                 o_call = L.take(4 * n);
+    const size_t o_hf = L.take(4 * n), o_hp = L.take(4 * n), o_dec = L.take(n), o_cand = L.take(16 * n), o_shuf = L.take(4 * n),
+                 o_inl = L.take(n);
+    const size_t o_st = L.take(sizeof(GfState)), o_draws = L.take(kSacDraws * sizeof(uint32_t));
+    const size_t o_tmp = L.take(std::max(sort_bytes, scan_bytes));
+    char *base;
+    if (const int rc = L.grow(ctx, ctx->gf_buf, base); rc != MULLS_OK) return rc;
     GfArgs A;
     std::memset(&A, 0, sizeof(A));
     A.P = P;
@@ -2590,7 +2575,6 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
     A.draws = (const uint32_t *)(base + o_draws);
     void *tmp = base + o_tmp;
     size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
-    CK(cudaEventRecord(ctx->ev_begin, st));
     CK(cudaMemcpyAsync((void *)A.rows, cloud_in.aos48, n * row_b, cudaMemcpyDefault, st)); // host or device rows
     CK(cudaMemcpyAsync((void *)A.draws, sac_draw_table(), kSacDraws * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     GfState hs;
@@ -2598,7 +2582,6 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
     hs.bb[0] = hs.bb[1] = host_ord(FLT_MAX);
     hs.bb[2] = hs.bb[3] = host_ord(-FLT_MAX);
     CK(cudaMemcpyAsync(A.st, &hs, sizeof(GfState), cudaMemcpyHostToDevice, st));
-    uint64_t launches = 0;
     const unsigned pb = (unsigned)ceil_div(n, kGfBlock);
     k_gf_bbox<<<pb, kGfBlock, 0, st>>>(A);
     k_gf_setup<<<1, 32, 0, st>>>(A);
@@ -2613,20 +2596,16 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
     const int num_grid = hs.num_grid;
     if (num_grid > 0) { // (a degenerate cloud with zero extent along x or y has no cell: every point fails the id test)
         const size_t g = (size_t)num_grid;
-        size_t coff = 0;
-        auto ctake = [&](size_t bytes) {
-            const size_t o = coff;
-            coff += (bytes + 255) / 256 * 256;
-            return o;
-        };
-        const size_t c_start = ctake(4 * g), c_end = ctake(4 * g), c_minz = ctake(4 * g), c_nb = ctake(4 * g), c_oth = ctake(4 * g);
-        const size_t c_rel = ctake(4 * g), c_nrm = ctake(16 * g), c_ng = ctake(4 * g), c_nu = ctake(4 * g), c_og = ctake(4 * g),
-                     c_ou = ctake(4 * g);
+        ScratchLayout CL;
+        const size_t c_start = CL.take(4 * g), c_end = CL.take(4 * g), c_minz = CL.take(4 * g), c_nb = CL.take(4 * g),
+                     c_oth = CL.take(4 * g);
+        const size_t c_rel = CL.take(4 * g), c_nrm = CL.take(16 * g), c_ng = CL.take(4 * g), c_nu = CL.take(4 * g),
+                     c_og = CL.take(4 * g), c_ou = CL.take(4 * g);
         size_t cscan = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, cscan, (uint32_t *)nullptr, (uint32_t *)nullptr, num_grid, st);
-        const size_t c_tmp = ctake(cscan);
-        if (const int rc = grow_scratch(ctx, ctx->gf_cell_buf, coff); rc != MULLS_OK) return rc;
-        char *cb = (char *)ctx->gf_cell_buf.p;
+        const size_t c_tmp = CL.take(cscan);
+        char *cb;
+        if (const int rc = CL.grow(ctx, ctx->gf_cell_buf, cb); rc != MULLS_OK) return rc;
         A.cell_start = (uint32_t *)(cb + c_start), A.cell_end = (uint32_t *)(cb + c_end);
         A.min_z = (float *)(cb + c_minz), A.neighbor_min_z = (float *)(cb + c_nb), A.outlier_thre = (float *)(cb + c_oth);
         A.reliable = (int *)(cb + c_rel);
@@ -2655,7 +2634,7 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
         k_gf_totals<<<1, 1, 0, st>>>(A, num_grid);
         k_gf_cell_emit<<<wb, kGfBlock, 0, st>>>(A, num_grid);
         k_gf_down<<<1, kClsBlock, 0, st>>>(A);
-        launches += 11;
+        launches += 10;
         CK(cudaMemcpyAsync(&hs, A.st, sizeof(GfState), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         CK(cudaGetLastError());
@@ -2671,12 +2650,12 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
         if (out->unground && hs.n_unground)
             CK(cudaMemcpyAsync(out->unground, A.out_unground, hs.n_unground * row_b, cudaMemcpyDefault, st));
     }
-    CK(cudaEventRecord(ctx->ev_end, st));
-    CK(cudaStreamSynchronize(st));
-    ctx->stats = mulls_run_stats();
-    ctx->stats.kernel_launches = launches;
-    cudaEventElapsedTime(&ctx->stats.ms_total, ctx->ev_begin, ctx->ev_end);
     return MULLS_OK;
+}
+
+int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_ground_params *params,
+                             mulls_ground_out *out) {
+    return front_call(ctx, [&](uint64_t &launches) { return ground_impl(ctx, cloud_in, params, out, launches); });
 }
 
 } // extern "C"
@@ -2686,16 +2665,13 @@ int mulls_fast_ground_filter(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mu
 // ------------------------------------------------------------------------------------------------
 extern "C" {
 
-int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxel_size, float *out, size_t cap, size_t *n_out) {
-    if (!ctx || !n_out || (cloud_in.n > 0 && (!cloud_in.aos48 || !out))) return MULLS_E_ARG;
+static int voxel_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxel_size, float *out, size_t cap, size_t *n_out,
+                      uint64_t &launches) {
+    if (!n_out || (cloud_in.n > 0 && (!cloud_in.aos48 || !out))) return MULLS_E_ARG;
     *n_out = 0;
     const size_t n = cloud_in.n;
     if (n == 0) return MULLS_OK;
-    if (n > ctx->max_tgt || n >= (1ull << 31)) {
-        ctx->err = "mulls_voxel_downsample: cloud exceeds max_tgt_pts of the context";
-        return MULLS_E_CAPACITY;
-    }
-    CK(cudaSetDevice(ctx->device));
+    if (const int rc = check_capacity(ctx, n, "mulls_voxel_downsample"); rc != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
     const size_t row_b = 48;
     if (voxel_size < 0.001) { // :89-97 disabled: cloud_out = cloud_in
@@ -2704,7 +2680,6 @@ int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxe
             return MULLS_E_CAPACITY;
         }
         CK(cudaMemcpyAsync(out, cloud_in.aos48, n * row_b, cudaMemcpyDefault, st));
-        CK(cudaStreamSynchronize(st));
         *n_out = n;
         return MULLS_OK;
     }
@@ -2712,17 +2687,13 @@ int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxe
     cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr,
                                     (uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, 0, 64, st);
     cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, st);
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        const size_t o = off;
-        off += (bytes + 255) / 256 * 256;
-        return o;
-    };
-    const size_t o_rows = take(n * row_b), o_out = take(n * row_b), o_key = take(8 * n), o_keys = take(8 * n);
-    const size_t o_idx = take(4 * n), o_idxs = take(4 * n), o_head = take(4 * n), o_pos = take(4 * n), o_st = take(sizeof(VxState));
-    const size_t o_tmp = take(std::max(sort_bytes, scan_bytes));
-    if (const int rc = grow_scratch(ctx, ctx->vx_buf, off); rc != MULLS_OK) return rc;
-    char *base = (char *)ctx->vx_buf.p;
+    ScratchLayout L;
+    const size_t o_rows = L.take(n * row_b), o_out = L.take(n * row_b), o_key = L.take(8 * n), o_keys = L.take(8 * n);
+    const size_t o_idx = L.take(4 * n), o_idxs = L.take(4 * n), o_head = L.take(4 * n), o_pos = L.take(4 * n),
+                 o_st = L.take(sizeof(VxState));
+    const size_t o_tmp = L.take(std::max(sort_bytes, scan_bytes));
+    char *base;
+    if (const int rc = L.grow(ctx, ctx->vx_buf, base); rc != MULLS_OK) return rc;
     VxArgs V;
     V.n = (uint32_t)n;
     V.voxel_size = voxel_size;
@@ -2737,7 +2708,6 @@ int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxe
     VxState hs;
     std::memset(&hs, 0, sizeof(hs));
     for (int d = 0; d < 3; ++d) hs.bb[d] = host_ord(FLT_MAX), hs.bb[3 + d] = host_ord(-FLT_MAX);
-    CK(cudaEventRecord(ctx->ev_begin, st));
     CK(cudaMemcpyAsync((void *)V.rows, cloud_in.aos48, n * row_b, cudaMemcpyDefault, st));
     CK(cudaMemcpyAsync(V.st, &hs, sizeof(VxState), cudaMemcpyHostToDevice, st));
     const unsigned pb = (unsigned)ceil_div(n, kGfBlock);
@@ -2750,6 +2720,7 @@ int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxe
     size_t b2 = tmp_bytes;
     CK(cub::DeviceScan::ExclusiveSum(tmp, b2, V.head, V.pos, (int)n, st));
     k_vx_gather<<<pb, kGfBlock, 0, st>>>(V);
+    launches += 5;
     CK(cudaMemcpyAsync(&hs, V.st, sizeof(VxState), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     CK(cudaGetLastError());
@@ -2759,17 +2730,17 @@ int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxe
         return MULLS_E_CAPACITY;
     }
     CK(cudaMemcpyAsync(out, V.out, (size_t)hs.n_out * row_b, cudaMemcpyDefault, st));
-    CK(cudaEventRecord(ctx->ev_end, st));
-    CK(cudaStreamSynchronize(st));
-    ctx->stats = mulls_run_stats();
-    ctx->stats.kernel_launches = 5;
-    cudaEventElapsedTime(&ctx->stats.ms_total, ctx->ev_begin, ctx->ev_end);
     return MULLS_OK;
 }
 
-int mulls_extract_semantic_pts(mulls_ctx *ctx, mulls_cloud_view pc_raw, const mulls_extract_params *params,
-                               mulls_extract_out *out) {
-    if (!ctx || !params || !out || (pc_raw.n > 0 && !pc_raw.aos48)) return MULLS_E_ARG;
+int mulls_voxel_downsample(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxel_size, float *out, size_t cap, size_t *n_out) {
+    return front_call(ctx, [&](uint64_t &launches) { return voxel_impl(ctx, cloud_in, voxel_size, out, cap, n_out, launches); });
+}
+
+// the three stages in one call frame: one launch count, one device span
+static int extract_impl(mulls_ctx *ctx, mulls_cloud_view pc_raw, const mulls_extract_params *params, mulls_extract_out *out,
+                        uint64_t &launches) {
+    if (!params || !out || (pc_raw.n > 0 && !pc_raw.aos48)) return MULLS_E_ARG;
     out->n_down = out->n_ground = out->n_ground_down = 0;
     for (int k = 0; k < MULLS_OUT_COUNT; ++k) out->cls.n[k] = 0;
     const size_t n = pc_raw.n;
@@ -2778,40 +2749,32 @@ int mulls_extract_semantic_pts(mulls_ctx *ctx, mulls_cloud_view pc_raw, const mu
         ctx->err = "mulls_extract_semantic_pts: the output buffers must hold pc_raw.n rows";
         return MULLS_E_ARG;
     }
-    CK(cudaSetDevice(ctx->device));
     // the clouds handed from stage to stage stay in HBM: pc_down and the ground filter's cloud_unground
     const size_t row_b = 48;
     int rc = grow_scratch(ctx, ctx->ext_buf, 2 * n * row_b);
     if (rc != MULLS_OK) return rc;
     float *d_down = (float *)ctx->ext_buf.p, *d_ung = (float *)((char *)ctx->ext_buf.p + n * row_b);
-    float ms = 0.f;
-    uint64_t launches = 0;
     // :2346 voxel_downsample(pc_raw, pc_down) (pc_sketch, :2348, is not a feature cloud and is not produced)
     size_t n_down = 0;
-    rc = mulls_voxel_downsample(ctx, pc_raw, params->vf_downsample_resolution, d_down, n, &n_down);
+    rc = voxel_impl(ctx, pc_raw, params->vf_downsample_resolution, d_down, n, &n_down, launches);
     if (rc != MULLS_OK) return rc;
-    ms += ctx->stats.ms_total, launches += ctx->stats.kernel_launches;
     out->n_down = n_down;
-    if (out->pc_down && n_down) {
-        CK(cudaMemcpyAsync(out->pc_down, d_down, n_down * row_b, cudaMemcpyDefault, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
+    if (out->pc_down && n_down) CK(cudaMemcpyAsync(out->pc_down, d_down, n_down * row_b, cudaMemcpyDefault, ctx->stream));
     // :2355-2361 fast_ground_filter(pc_down -> pc_ground, pc_ground_down, pc_unground)
     mulls_ground_out g;
     std::memset(&g, 0, sizeof(g));
     g.ground = out->pc_ground, g.ground_down = out->pc_ground_down, g.unground = d_ung;
     g.cap = n;
-    rc = mulls_fast_ground_filter(ctx, mulls_cloud_view{d_down, n_down}, &params->ground, &g);
+    rc = ground_impl(ctx, mulls_cloud_view{d_down, n_down}, &params->ground, &g, launches);
     if (rc != MULLS_OK) return rc;
-    ms += ctx->stats.ms_total, launches += ctx->stats.kernel_launches;
     out->n_ground = g.n_ground, out->n_ground_down = g.n_ground_down;
     // :2378-2391 classify_nground_pts(pc_unground -> pillar, beam, facade, roof, their down clouds, vertex)
-    rc = mulls_classify_nground(ctx, mulls_cloud_view{d_ung, g.n_unground}, &params->classify, &out->cls);
-    if (rc != MULLS_OK) return rc;
-    ms += ctx->stats.ms_total, launches += ctx->stats.kernel_launches;
-    ctx->stats.ms_total = ms;
-    ctx->stats.kernel_launches = launches;
-    return MULLS_OK;
+    return classify_impl(ctx, mulls_cloud_view{d_ung, g.n_unground}, &params->classify, &out->cls, launches);
+}
+
+int mulls_extract_semantic_pts(mulls_ctx *ctx, mulls_cloud_view pc_raw, const mulls_extract_params *params,
+                               mulls_extract_out *out) {
+    return front_call(ctx, [&](uint64_t &launches) { return extract_impl(ctx, pc_raw, params, out, launches); });
 }
 
 } // extern "C"
