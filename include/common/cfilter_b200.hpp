@@ -1,5 +1,6 @@
 // Drop-in shims: lo::CFilter<PointT>::classify_nground_pts (include/common/cfilter.hpp:2058-2290), fast_ground_filter
-// (:1658-2036), voxel_downsample (:83-165), sor_filter (:203-247), scanner_filter (:914-929) and the raw-scan corrections
+// (:1658-2036), voxel_downsample (:83-165), sor_filter (:203-247), non_max_suppress (:1183-1240), scanner_filter
+// (:914-929) and the raw-scan corrections
 // vertical_intrinsic_calibration (:250-291), get_pts_timestamp_ratio_in_frame (:412-467), apply_motion_compensation and
 // batch_apply_motion_compensation (:470-549) over the mulls_b200 C-ABI. A MULLS maintainer replaces the BODY of classify_nground_pts by
 //
@@ -196,6 +197,31 @@ bool sor_filter(typename pcl::PointCloud<PointT>::Ptr &cloud_in, typename pcl::P
 template <typename PointT>
 bool sor_filter(typename pcl::PointCloud<PointT>::Ptr &cloud_in_out, int mean_k, double n_std) {
     return sor_filter<PointT>(cloud_in_out, cloud_in_out, mean_k, n_std);
+}
+
+// lo::CFilter<PointT>::non_max_suppress, the in-place overload (include/common/cfilter.hpp:1183-1240) with
+// kd_tree_already_built = false (mulls_non_max_suppress): the cloud's points become its kept rows, all 48 bytes of each,
+// in the reference's order (score descending; abi.h states the readings). width and height are not touched, as in the
+// reference. Returns false with the cloud untouched for fewer than 10 points, as the reference, or when the call is
+// refused (no device).
+template <typename PointT>
+bool non_max_suppress(typename pcl::PointCloud<PointT>::Ptr &cloud_in_out, float non_max_radius) {
+    static_assert(sizeof(PointT) == 48, "the C-ABI consumes pcl::PointXYZINormal rows (48 bytes)");
+    const size_t n = cloud_in_out->points.size();
+    if (n < 10) return false;
+    mulls_ctx *ctx = thread_context(1, n);
+    std::vector<int32_t> idx(n);
+    size_t n_kept = 0;
+    int performed = 0;
+    if (!ctx || mulls_non_max_suppress(ctx, view_of<PointT>(cloud_in_out), non_max_radius, idx.data(), &n_kept, &performed) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return false;
+    }
+    std::vector<PointT> kept;
+    kept.reserve(n_kept);
+    for (size_t k = 0; k < n_kept; ++k) kept.push_back(cloud_in_out->points[idx[k]]);
+    cloud_in_out->points.swap(kept);
+    return performed != 0;
 }
 
 // lo::CFilter<PointT>::scanner_filter (include/common/cfilter.hpp:914-929) in float, on the host: drops the points within

@@ -38,6 +38,7 @@
  *                               cfilter.hpp:470-549
  *   mulls_ncc_correspondences <- lo::CRegistration<PointT>::find_feature_correspondence_ncc, cregistration.hpp:409-601
  *   mulls_coarse_reg_ransac  <- lo::CRegistration<PointT>::coarse_reg_ransac, cregistration.hpp:604-661
+ *   mulls_non_max_suppress   <- lo::CFilter<PointT>::non_max_suppress(cloud_in_out, non_max_radius), cfilter.hpp:1183-1240
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
  *
@@ -572,6 +573,28 @@ int mulls_ncc_correspondences(mulls_ctx *ctx, mulls_cloud_view target_kpts, mull
 int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_cloud_view source_pts, float noise_bound,
                             int min_inlier_num, int max_iter_num, double tran_mat[16] /* row-major, written only when status >= 0 */,
                             int *status, int *n_inliers, int *n_hypotheses);
+
+/* lo::CFilter<PointT>::non_max_suppress(cloud_in_out, non_max_radius, kd_tree_already_built = false), cfilter.hpp:1183-1240:
+ * the keypoint suppression in front of the NCC matching (test/mulls_reg.cpp:145-149, test/mulls_slam.cpp:462). Stateless
+ * like mulls_ncc_correspondences: the batch resident on the context and its grid are left alone. 48-byte rows as for the
+ * NCC matching; x y z and the score normal[3] (float 7 of the row) are read. The reference sorts the cloud by score,
+ * descending, then walks it: the first point not yet visited is kept and every point within the radius of it is
+ * visited; the cloud becomes the kept points in that order. kept_idx[k] (k < *n_kept) receives the input row index of
+ * the k-th kept point; the entries past *n_kept are unspecified. Readings:
+ *   - fewer than 10 points (:1189-1191): *performed = 0, *n_kept = 0, kept_idx untouched (the reference returns false
+ *     and leaves the cloud unsorted); otherwise *performed = 1 (it returns true)
+ *   - order: descending score; equal scores keep input order (std::sort leaves it open), +0 and -0 are equal, NaN scores
+ *     come after every number, in input order (std::sort with > is undefined on NaN)
+ *   - neighbour test: FLANN's float L2_Simple distance flann_l2(kept, p) < r2, r2 = (float)((double)r * r): a negative
+ *     radius acts as its absolute value, a zero or NaN radius suppresses nothing
+ *   - a point with a non-finite coordinate is within the radius of no point (its FLANN distances are NaN or inf): it is
+ *     kept when the walk reaches it and suppresses nothing, as PCL does on a cloud that is not dense
+ *   - kd_tree_already_built = true (a tree built on the cloud before the sort) is not served here; the drop-in forwards
+ *     it to the reference member
+ * A cloud of more than the context's max_tgt_pts points: MULLS_E_CAPACITY. A NULL output, or NULL rows with n > 0:
+ * MULLS_E_ARG. */
+int mulls_non_max_suppress(mulls_ctx *ctx, mulls_cloud_view cloud, float non_max_radius, int32_t *kept_idx /* [cloud.n] */,
+                           size_t *n_kept, int *performed);
 
 /* The wire format the library ships host clouds in when the "host_pack" tunable is on (csrc/host_pack.h): the 28 of the
  * 48 bytes of a pcl::PointXYZINormal row (utility.hpp:40) that the path reads, repacked on the host cores into pinned

@@ -289,6 +289,7 @@ EXPORTED_SYMBOLS = (
     "mulls_motion_compensation",
     "mulls_ncc_correspondences",
     "mulls_coarse_reg_ransac",
+    "mulls_non_max_suppress",
     "mulls_scan_probe",
     "mulls_scan_read",
     "mulls_pose_write",
@@ -372,6 +373,9 @@ def load_library() -> C.CDLL:
     lib.mulls_coarse_reg_ransac.restype = C.c_int
     lib.mulls_coarse_reg_ransac.argtypes = [vp, CloudView, CloudView, C.c_float, C.c_int, C.c_int, C.POINTER(C.c_double),
                                             C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    lib.mulls_non_max_suppress.restype = C.c_int
+    lib.mulls_non_max_suppress.argtypes = [vp, CloudView, C.c_float, C.POINTER(C.c_int32), C.POINTER(C.c_size_t),
+                                           C.POINTER(C.c_int)]
     lib.mulls_pack_rows.restype = C.c_int
     lib.mulls_pack_rows.argtypes = [C.POINTER(C.c_float), C.c_size_t, C.c_int, C.POINTER(C.c_float)]
     lib.mulls_scan_probe.restype = C.c_int

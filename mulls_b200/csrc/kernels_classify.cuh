@@ -5,12 +5,13 @@
 // order-dependent step reproduces the sequential result exactly:
 //   * vertex-neighbourhood promotion (:2169-2210) reads labels that the same loop has just written for smaller
 //     indices: resolved by monotone rounds (a candidate waits while an earlier undecided candidate could still tip it);
-//   * non_max_suppress (:1243-1312) is the greedy maximal independent set in score order: resolved chunk by chunk
-//     against the already selected points, then by monotone rounds inside the chunk.
+//   * non_max_suppress (:1243-1312) is the greedy maximal independent set in score order: kernels_nms.cuh, shared
+//     with mulls_non_max_suppress.
 #pragma once
 #include "device_math.cuh"
 #include "device_types.cuh"
 #include "kernels_map.cuh"
+#include "kernels_nms.cuh"
 #include "kernels_pca.cuh"
 
 namespace mulls {
@@ -23,7 +24,7 @@ struct ClsState {
     uint32_t n_down[4];  // *_down after the thresholds / the NMS
     uint32_t n_down2[4]; // ... after the fixed-number down-sampling
     uint32_t n_vertex;
-    uint32_t nms_ran[4]; // the class cloud was sorted by non_max_suppress
+    uint32_t nms_ran[4]; // the class cloud was sorted by non_max_suppress (NmsArgs::ran)
 };
 
 struct ClsArgs {
@@ -44,8 +45,6 @@ struct ClsArgs {
     float4 *sect;      // one sector of xy_normal_balanced_downsample (n rows)
     float4 *vrows;     // keypoint rows by point index (n rows)
     float4 *vertex;
-    float4 *sel_pos;   // NMS: positions selected so far, 4 x n
-    uint64_t *keys_a, *keys_b;
     ClsState *st;
 };
 
@@ -308,141 +307,6 @@ __global__ void __launch_bounds__(kClsBlock) k_cls_compact_vertex(ClsArgs C) {
     }
     __syncthreads();
     if (threadIdx.x == 0) C.st->n_vertex = s_total;
-}
-
-// ---- non_max_suppress (:1243-1312) -------------------------------------------------------------------------------
-__device__ __forceinline__ bool nms_active(const ClsArgs &C, int c) {
-    const int fixed[4] = {C.P.pillar_down_fixed_num, C.P.beam_down_fixed_num, C.P.facade_down_fixed_num, C.P.roof_down_fixed_num};
-    return C.P.sharpen_with_nms && fixed[c] > 0 && C.st->n_cls2[c] >= 10;
-}
-__device__ __forceinline__ uint32_t nms_offset(const ClsArgs &C, int c) {
-    uint32_t off = 0;
-    for (int k = 0; k < c; ++k)
-        if (nms_active(C, k)) off += C.st->n_cls2[k];
-    return off;
-}
-
-// sort key of a class-cloud entry: class | descending score (normal[3]) | position in the class cloud (std::sort is
-// not stable; ties keep their order here and in the CPU restatement)
-__global__ void __launch_bounds__(256) k_nms_keys(ClsArgs C) {
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    const int c = blockIdx.y;
-    if (!nms_active(C, c) || t >= C.st->n_cls2[c]) return;
-    const float score = C.cls[c][3 * (size_t)t + 1].w;
-    const uint32_t ord = (uint32_t)float_to_ordered(score) ^ 0x80000000u; // ascending unsigned order of the float
-    C.keys_a[nms_offset(C, c) + t] = ((uint64_t)c << 61) | ((uint64_t)(~ord) << 29) | (uint64_t)t;
-}
-
-__global__ void __launch_bounds__(256) k_nms_gather(ClsArgs C) {
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= C.n) return;
-    const uint64_t key = C.keys_b[r];
-    if (key == ~0ull) return;
-    const int c = (int)(key >> 61);
-    const uint32_t slot = (uint32_t)(key & ((1u << 29) - 1u));
-    const float4 *in = C.cls[c] + 3 * (size_t)slot;
-    float4 *o = C.cls_sorted[c] + 3 * (size_t)(r - nms_offset(C, c));
-    o[0] = in[0], o[1] = in[1], o[2] = in[2];
-}
-
-// one block per class: greedy selection in score order, 1024 points at a time. Inside a chunk every thread first
-// builds the bit mask of the EARLIER chunk points within the radius (32 words), then the rounds are pure bit tests
-// against two shared masks (selected / suppressed) that only ever gain bits.
-__global__ void __launch_bounds__(kClsBlock) k_nms_select(ClsArgs C) {
-    const int c = blockIdx.x;
-    __shared__ uint32_t s_warp[kClsBlock / 32];
-    __shared__ uint32_t s_total;
-    __shared__ float s_x[kClsBlock], s_y[kClsBlock], s_z[kClsBlock];
-    __shared__ uint32_t s_sel[kClsBlock / 32], s_sup[kClsBlock / 32];
-    if (!nms_active(C, c)) {
-        if (threadIdx.x == 0) C.st->nms_ran[c] = 0; // n_down stays what the threshold loop left (0 when sharpening)
-        return;
-    }
-    const uint32_t n = C.st->n_cls2[c];
-    const float nms_radius = (float)(0.25 * (double)C.P.neighbor_searching_radius);
-    const float r2 = (float)((double)nms_radius * (double)nms_radius);
-    const float4 *pts = C.cls_sorted[c];
-    float4 *sel = C.sel_pos + (size_t)c * C.n;
-    const uint32_t tid = threadIdx.x, myw = tid >> 5, mybit = 1u << (tid & 31);
-    if (tid == 0) s_total = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < n; base += kClsBlock) {
-        const uint32_t i = base + tid;
-        const bool valid = i < n;
-        float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (valid) p = pts[3 * (size_t)i];
-        s_x[tid] = p.x, s_y[tid] = p.y, s_z[tid] = p.z;
-        if (tid < kClsBlock / 32) s_sel[tid] = 0, s_sup[tid] = 0;
-        // (1) against the points selected in the earlier chunks
-        bool open = valid;
-        const uint32_t n_sel = s_total;
-        if (valid)
-            for (uint32_t t = 0; t < n_sel; ++t) {
-                const float4 q = sel[t];
-                if (flann_l2(q.x, q.y, q.z, p.x, p.y, p.z) < r2) {
-                    open = false;
-                    break;
-                }
-            }
-        __syncthreads();
-        if (!open) atomicOr(&s_sup[myw], mybit);
-        // (2) near mask over the earlier points of the chunk
-        uint32_t near[kClsBlock / 32];
-#pragma unroll
-        for (int w = 0; w < kClsBlock / 32; ++w) {
-            uint32_t mk = 0;
-            if (open && (uint32_t)(w * 32) < tid) {
-                const uint32_t lim = min(32u, tid - (uint32_t)(w * 32));
-                for (uint32_t b = 0; b < lim; ++b) {
-                    const uint32_t t = (uint32_t)(w * 32) + b;
-                    if (flann_l2(s_x[t], s_y[t], s_z[t], p.x, p.y, p.z) < r2) mk |= 1u << b;
-                }
-            }
-            near[w] = mk;
-        }
-        __syncthreads();
-        // (3) a point is selected once every earlier point within the radius is suppressed
-        while (true) {
-            int pending = 0;
-            if (open) {
-                bool hit = false, blocked = false;
-#pragma unroll
-                for (int w = 0; w < kClsBlock / 32; ++w) {
-                    const uint32_t nm = near[w];
-                    if (nm) {
-                        const uint32_t se = ((volatile uint32_t *)s_sel)[w];
-                        const uint32_t su = ((volatile uint32_t *)s_sup)[w];
-                        if (nm & se) hit = true;
-                        if (nm & ~(se | su)) blocked = true;
-                    }
-                }
-                if (hit) {
-                    atomicOr(&s_sup[myw], mybit);
-                    open = false;
-                } else if (!blocked) {
-                    atomicOr(&s_sel[myw], mybit);
-                    open = false;
-                } else {
-                    pending = 1;
-                }
-            }
-            if (!__syncthreads_or(pending)) break;
-        }
-        // (4) append the chunk's selected points, in order
-        const bool keep = valid && (s_sel[myw] & mybit);
-        const uint32_t slot = map_tile_slot(keep, s_warp, &s_total);
-        if (keep) {
-            const float4 *r = pts + 3 * (size_t)i;
-            float4 *o = C.down[c] + 3 * (size_t)slot;
-            o[0] = r[0], o[1] = r[1], o[2] = r[2];
-            sel[slot] = p;
-        }
-        __syncthreads();
-    }
-    if (tid == 0) {
-        C.st->n_down[c] = s_total;
-        C.st->nms_ran[c] = 1;
-    }
 }
 
 // ---- fixed-number down-sampling (:2257-2267) -----------------------------------------------------------------------

@@ -158,6 +158,7 @@ struct mulls_ctx {
     Scratch raw_buf;             // raw-scan corrections: the rows of the call, the column it returns, timestamp state
     Scratch ncc_buf;             // NCC keypoint matching: rows, descriptors, row / column minima or select state, sort
     Scratch rc_buf;              // RANSAC coarse registration: correspondences, hypotheses, counts, refinement state
+    Scratch nms_buf;             // keypoint NMS: rows, sorted rows, keys, sort scratch, cell hash, kept indices
     void *rc_host = nullptr;     // pinned: two chunks of sample triples and their counts
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
@@ -255,7 +256,7 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (void *p : ctx->allocs) cudaFree(p);
     if (ctx->cub_temp) cudaFree(ctx->cub_temp);
-    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf, &ctx->ncc_buf, &ctx->rc_buf})
+    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf, &ctx->ncc_buf, &ctx->rc_buf, &ctx->nms_buf})
         if (s->p) cudaFree(s->p);
     if (ctx->rc_host) cudaFreeHost(ctx->rc_host);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
@@ -2305,6 +2306,113 @@ int mulls_icp_run_to_map(mulls_ctx *ctx, mulls_map *m, const mulls_cloud_view sr
 }
 
 // ================================================================================================
+// Keypoint non-maximum suppression (CFilter::non_max_suppress, cfilter.hpp:1183-1312): kernels_nms.cuh. One device NMS
+// for classify_nground_pts' four class clouds and for mulls_non_max_suppress' one cloud.
+// ================================================================================================
+// Slots of the cell hash of k_nms_select for clouds of at most `cap` points, 0 for none: a cloud of at most one chunk
+// never looks back at earlier chunks, and a radius whose square is not > 0 suppresses nothing. Load factor <= 1/2.
+static uint32_t nms_hash_slots(size_t cap, float r2) {
+    if (cap <= (size_t)kNmsBlock || !(r2 > 0.f)) return 0;
+    uint32_t h = 1;
+    while (h < 2 * cap) h <<= 1;
+    return h;
+}
+// 1 / the cell edge. The edge exceeds every per-axis |dx| of a pair whose float flann_l2 is < r2: such a |dx| is below
+// sqrt(r2) (1 + 2^-22), the margin here is 2^-10 and also covers the double rounding of x * (1 / edge). The floor keeps the edge
+// above the distances a flushed product could hide. DESIGN §16.
+static double nms_inv_cell(float r2) { return 1.0 / std::max(std::sqrt((double)r2) * (1.0 + 1.0 / 1024), 1e-18); }
+
+// sorts the active clouds of N by score and runs the greedy walk: 3 kernels of this library and one radix sort. N's hash
+// slots, when it has them, are contiguous from hash[0].
+static int launch_nms(mulls_ctx *ctx, const NmsArgs &N, void *cub_temp, size_t cub_bytes, uint64_t &launches) {
+    cudaStream_t st = ctx->stream;
+    const unsigned gb = (unsigned)ceil_div(N.total, 256);
+    CK(cudaMemsetAsync(N.keys_a, 0xff, N.total * sizeof(uint64_t), st));
+    if (N.hash[0]) CK(cudaMemsetAsync(N.hash[0], 0xff, (size_t)N.n_clouds * (N.hash_mask + 1ull) * sizeof(NmsSlot), st));
+    k_nms_keys<<<dim3(gb, N.n_clouds), 256, 0, st>>>(N);
+    CK(cub::DeviceRadixSort::SortKeys(cub_temp, cub_bytes, N.keys_a, N.keys_b, (int)N.total, 0, 64, st));
+    k_nms_gather<<<gb, 256, 0, st>>>(N);
+    k_nms_select<<<N.n_clouds, kNmsBlock, 0, st>>>(N);
+    launches += 3;
+    return MULLS_OK;
+}
+
+struct NmsCounts { // device-side n / n_kept / ran of the one cloud of mulls_non_max_suppress, and its host copy
+    uint32_t n, n_kept, ran, pad;
+};
+
+static int nms_impl(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int32_t *kept_idx, size_t *n_kept, int *performed,
+                    NmsCounts &hc, uint64_t &launches) {
+    if (!kept_idx || !n_kept || !performed || (cloud.n > 0 && !cloud.aos48)) {
+        ctx->err = "mulls_non_max_suppress: NULL cloud rows or output";
+        return MULLS_E_ARG;
+    }
+    const size_t n = cloud.n;
+    int rc = check_capacity(ctx, n, "mulls_non_max_suppress");
+    if (rc != MULLS_OK) return rc;
+    if (n < 10) return MULLS_OK; // cfilter.hpp:1189-1191: no sort, no device work
+    if (n >= kNmsMaxPoints) {
+        ctx->err = "mulls_non_max_suppress: at most 2^29 - 1 points";
+        return MULLS_E_CAPACITY;
+    }
+    cudaStream_t st = ctx->stream;
+    const float r2 = (float)((double)radius * (double)radius);
+    const uint32_t slots = nms_hash_slots(n, r2);
+    size_t cub_bytes = 0;
+    CK(cub::DeviceRadixSort::SortKeys(nullptr, cub_bytes, (uint64_t *)nullptr, (uint64_t *)nullptr, (int)n, 0, 64, st));
+    ScratchLayout L;
+    const size_t o_in = L.take(n * 48), o_srt = L.take(n * 48), o_sel = L.take(n * sizeof(float4)), o_idx = L.take(n * sizeof(int32_t)),
+                 o_ord = L.take(n * sizeof(uint32_t)), o_ka = L.take(n * sizeof(uint64_t)), o_kb = L.take(n * sizeof(uint64_t)),
+                 o_hash = L.take((size_t)slots * sizeof(NmsSlot)), o_next = L.take(slots ? n * sizeof(int32_t) : 0),
+                 o_cnt = L.take(sizeof(NmsCounts)), o_cub = L.take(cub_bytes);
+    char *base;
+    if ((rc = L.grow(ctx, ctx->nms_buf, base)) != MULLS_OK) return rc;
+    NmsCounts *d_cnt = (NmsCounts *)(base + o_cnt);
+    hc = NmsCounts{(uint32_t)n, 0, 0, 0};
+    CK(cudaMemcpyAsync(d_cnt, &hc, sizeof(hc), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(base + o_in, cloud.aos48, n * 48, cudaMemcpyDefault, st));
+    NmsArgs N;
+    std::memset(&N, 0, sizeof(N));
+    N.n_clouds = 1;
+    N.on_mask = 1;
+    N.n = &d_cnt->n;
+    N.n_kept = &d_cnt->n_kept;
+    N.ran = &d_cnt->ran;
+    N.r2 = r2;
+    N.inv_cell = nms_inv_cell(r2);
+    N.in[0] = (const float4 *)(base + o_in);
+    N.sorted[0] = (float4 *)(base + o_srt);
+    N.kept_idx[0] = (int32_t *)(base + o_idx);
+    N.sel[0] = (float4 *)(base + o_sel);
+    if (slots) {
+        N.hash[0] = (NmsSlot *)(base + o_hash);
+        N.next[0] = (int32_t *)(base + o_next);
+    }
+    N.hash_mask = slots - 1;
+    N.total = (uint32_t)n;
+    N.keys_a = (uint64_t *)(base + o_ka);
+    N.keys_b = (uint64_t *)(base + o_kb);
+    N.order = (uint32_t *)(base + o_ord);
+    if ((rc = launch_nms(ctx, N, base + o_cub, cub_bytes, launches)) != MULLS_OK) return rc;
+    // all n entries: one copy instead of a count read-back first; the ones past the kept count are unspecified
+    CK(cudaMemcpyAsync(kept_idx, N.kept_idx[0], n * sizeof(int32_t), cudaMemcpyDefault, st));
+    CK(cudaMemcpyAsync(&hc, d_cnt, sizeof(hc), cudaMemcpyDeviceToHost, st));
+    return MULLS_OK;
+}
+
+int mulls_non_max_suppress(mulls_ctx *ctx, mulls_cloud_view cloud, float non_max_radius, int32_t *kept_idx, size_t *n_kept,
+                           int *performed) {
+    NmsCounts hc{0, 0, 0, 0};
+    const int rc = front_call(ctx, [&](uint64_t &launches) {
+        return nms_impl(ctx, cloud, non_max_radius, kept_idx, n_kept, performed, hc, launches);
+    });
+    if (rc != MULLS_OK) return rc;
+    *n_kept = hc.n_kept;
+    *performed = hc.ran ? 1 : 0;
+    return MULLS_OK;
+}
+
+// ================================================================================================
 // Non-ground feature classification (CFilter::classify_nground_pts, cfilter.hpp:2058-2290)
 // ================================================================================================
 void mulls_classify_default_params(mulls_classify_params *p) {
@@ -2370,7 +2478,12 @@ static int classify_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_
     for (int c = 0; c < 4; ++c)
         o_cls[c] = L.take(n0 * row_b), o_srt[c] = L.take(n0 * row_b), o_dn[c] = L.take(n0 * row_b), o_dn2[c] = L.take(n0 * row_b);
     const size_t o_sect = L.take(2 * n0 * row_b), o_vrows = L.take(n0 * row_b), o_vertex = L.take(n0 * row_b);
-    const size_t o_sel = L.take(4 * n0 * sizeof(float4));
+    const size_t o_sel = L.take(4 * n0 * sizeof(float4)), o_ord = L.take(n0 * sizeof(uint32_t));
+    // non_max_suppress(cloud, cloud_down, 0.25 * neighbor_searching_radius) (:2236-2255) on the four class clouds
+    const float nms_radius = (float)(0.25 * (double)P.neighbor_searching_radius);
+    const float nms_r2 = (float)((double)nms_radius * (double)nms_radius);
+    const uint32_t nms_slots = nms_hash_slots(n, nms_r2);
+    const size_t o_hash = L.take(4 * (size_t)nms_slots * sizeof(NmsSlot)), o_next = L.take(nms_slots ? 4 * n0 * sizeof(int32_t) : 0);
     const size_t o_l0 = L.take(n0), o_l = L.take(n0), o_df = L.take(n0), o_s4 = L.take(n0), o_vf = L.take(n0),
                  o_st = L.take(sizeof(ClsState));
     char *base;
@@ -2390,7 +2503,6 @@ static int classify_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_
     C.sect = (float4 *)(base + o_sect);
     C.vrows = (float4 *)(base + o_vrows);
     C.vertex = (float4 *)(base + o_vertex);
-    C.sel_pos = (float4 *)(base + o_sel);
     C.label0 = (uint8_t *)(base + o_l0);
     C.label = (uint8_t *)(base + o_l);
     C.downflag = (uint8_t *)(base + o_df);
@@ -2413,8 +2525,6 @@ static int classify_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_
         mulls_cloud_view v{(const float *)C.rows, n};
         const int rc = pca_on_device(ctx, v, true, P.neighbor_searching_radius, P.neighbor_k, stride, C.F, launches, unit_dist);
         if (rc != MULLS_OK) return rc;
-        C.keys_a = ctx->A.keys_a;
-        C.keys_b = ctx->A.keys_b;
         const unsigned gb = (unsigned)ceil_div(n, 256);
         k_cls_label<<<gb, 256, 0, st>>>(C);
         k_cls_compact<<<8, kClsBlock, 0, st>>>(C);
@@ -2426,13 +2536,32 @@ static int classify_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_
         k_cls_compact_vertex<<<1, kClsBlock, 0, st>>>(C);
         launches += 8;
         if (P.sharpen_with_nms) {
-            CK(cudaMemsetAsync(C.keys_a, 0xff, n * sizeof(uint64_t), st));
-            k_nms_keys<<<dim3(gb, 4), 256, 0, st>>>(C);
-            size_t bytes = ctx->cub_temp_bytes;
-            CK(cub::DeviceRadixSort::SortKeys(ctx->cub_temp, bytes, C.keys_a, C.keys_b, (int)n, 0, 64, st));
-            k_nms_gather<<<gb, 256, 0, st>>>(C);
-            k_nms_select<<<4, kClsBlock, 0, st>>>(C);
-            launches += 3;
+            const int fixed[4] = {P.pillar_down_fixed_num, P.beam_down_fixed_num, P.facade_down_fixed_num, P.roof_down_fixed_num};
+            NmsArgs N;
+            std::memset(&N, 0, sizeof(N));
+            N.n_clouds = 4;
+            N.n = C.st->n_cls2;
+            N.n_kept = C.st->n_down; // n_down stays what the threshold loop left (0 when sharpening) where NMS does not run
+            N.ran = C.st->nms_ran;
+            N.r2 = nms_r2;
+            N.inv_cell = nms_inv_cell(nms_r2);
+            N.hash_mask = nms_slots - 1;
+            N.total = (uint32_t)n;
+            N.keys_a = ctx->A.keys_a;
+            N.keys_b = ctx->A.keys_b;
+            N.order = (uint32_t *)(base + o_ord);
+            for (int c = 0; c < 4; ++c) {
+                if (fixed[c] > 0) N.on_mask |= 1u << c;
+                N.in[c] = C.cls[c];
+                N.sorted[c] = C.cls_sorted[c];
+                N.kept_rows[c] = C.down[c];
+                N.sel[c] = (float4 *)(base + o_sel) + (size_t)c * n0;
+                if (nms_slots) {
+                    N.hash[c] = (NmsSlot *)(base + o_hash) + (size_t)c * nms_slots;
+                    N.next[c] = (int32_t *)(base + o_next) + (size_t)c * n0;
+                }
+            }
+            if (const int rc = launch_nms(ctx, N, ctx->cub_temp, ctx->cub_temp_bytes, launches); rc != MULLS_OK) return rc;
         }
         if (P.fixed_num_downsampling) {
             k_cls_fixed<<<4, kClsBlock, 0, st>>>(C);

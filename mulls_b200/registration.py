@@ -365,6 +365,19 @@ class Context:
                                                      C.byref(nh)))
         return st.value, buf.reshape(4, 4), ni.value, nh.value
 
+    def non_max_suppress(self, cloud: np.ndarray, non_max_radius: float):
+        """CFilter::non_max_suppress(cloud_in_out, non_max_radius) (cfilter.hpp:1183-1240) on the GPU. Returns
+        (kept_idx, performed): kept_idx is an int32 array of the input rows the reference leaves in the cloud, in its
+        order (cloud[kept_idx] is that cloud); performed is False, with kept_idx empty, where the reference returns false
+        and leaves the cloud as it was (fewer than 10 points). The resident batch is untouched."""
+        c = abi.as_aos48(cloud)
+        idx = np.zeros(max(len(c), 1), np.int32)
+        n = C.c_size_t(0)
+        performed = C.c_int(0)
+        self._check(self.lib.mulls_non_max_suppress(self.handle, abi.cloud_view(c), float(non_max_radius),
+                                                    idx.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(n), C.byref(performed)))
+        return idx[: n.value].copy(), bool(performed.value)
+
     def stats(self) -> dict:
         s = abi.RunStats()
         self._check(self.lib.mulls_get_stats(self.handle, C.byref(s)))
