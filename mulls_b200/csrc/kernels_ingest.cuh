@@ -453,8 +453,8 @@ __global__ void __launch_bounds__(256) k_gather(DeviceArrays A, const uint64_t *
         if (pc.sharded) nrm.w = __int_as_float(__float_as_int(nrm.w) + (int)pc.src_index_base[seg - kNumClasses]);
         A.src_pos[0][d] = pos;
         A.src_nrm[0][d] = nrm;
-        A.src_prevj[0][d] = -1;
-        A.src_cert[0][d] = make_float4(0.f, 0.f, 0.f, 0.f);
+        // (src_prevj and src_cert need no initial value: iteration 0 reads no previous match, and a certificate is read
+        // only after k_search<1> has written it, kernels_iterate.cuh)
     }
 }
 

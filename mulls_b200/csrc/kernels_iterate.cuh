@@ -101,25 +101,31 @@ __device__ __forceinline__ GridView grid_of(const DeviceArrays &A, const PairCon
 // ------------------------------------------------------------------------------------------------
 constexpr int kShootK = 10;
 
-// ---- k_search ----------------------------------------------------------------------------------
-// what every search kernel does first: cregistration.hpp:1260 — incremental in-place update of the float source
-// cloud by the previous iteration's TempTran (double math, float store, as pcl::transformPointCloudWithNormals)
-__device__ __forceinline__ void load_and_advance(DeviceArrays &A, const PairState &ps, int buf, uint32_t gi, bool valid,
-                                                 float4 &p, float4 &n) {
-    p = A.src_pos[buf][gi];
-    n = A.src_nrm[buf][gi];
-    if (valid && ps.iter > 0) {
+// ---- the moved source --------------------------------------------------------------------------
+// cregistration.hpp:1260 — the float source cloud moved by the previous iteration's TempTran (double math, float
+// result, as pcl::transformPointCloudWithNormals). src_pos / src_nrm[buf] hold the cloud as the iteration found it and
+// are never written back: each kernel of the iteration that needs a moved point or normal recomputes it from ps.T_inc,
+// which solve_and_advance replaces only after k_accumulate. Built with -fmad=false, the same double expressions give
+// the same bits in every kernel; the moved cloud is stored once, by k_accumulate's compaction into buf ^ 1.
+__device__ __forceinline__ float4 advanced_pos(const PairState &ps, float4 p) {
+    if (ps.iter > 0) {
         const double *t = ps.T_inc;
-        const double px = p.x, py = p.y, pz = p.z, qx = n.x, qy = n.y, qz = n.z;
+        const double px = p.x, py = p.y, pz = p.z;
         p.x = (float)(t[0] * px + t[1] * py + t[2] * pz + t[3]);
         p.y = (float)(t[4] * px + t[5] * py + t[6] * pz + t[7]);
         p.z = (float)(t[8] * px + t[9] * py + t[10] * pz + t[11]);
+    }
+    return p;
+}
+__device__ __forceinline__ float4 advanced_nrm(const PairState &ps, float4 n) { // n.w (the original index) stays
+    if (ps.iter > 0) {
+        const double *t = ps.T_inc;
+        const double qx = n.x, qy = n.y, qz = n.z;
         n.x = (float)(t[0] * qx + t[1] * qy + t[2] * qz);
         n.y = (float)(t[4] * qx + t[5] * qy + t[6] * qz);
         n.z = (float)(t[8] * qx + t[9] * qy + t[10] * qz);
-        A.src_pos[buf][gi] = p;
-        A.src_nrm[buf][gi] = n;
     }
+    return n;
 }
 
 // shoot = 0: every class except the normal-shooting ones; shoot = 1 (k_search_shoot): only those
@@ -127,17 +133,23 @@ __device__ __forceinline__ bool shoots(const PairConst &pc, int c) {
     return pc.normal_shooting && (c == MULLS_GROUND || c == MULLS_FACADE || c == MULLS_ROOF);
 }
 
-// ---- k_search: I1 + I2a of the iteration — apply the previous increment to the source (:1260), exact
-//      radius-bounded 1-NN on the hashed multi-level grid (nn_search_walk, search_core.cuh — replaces the kd-tree query
-//      of :1745), claim the target for the duplicate check. Resident blocks fetch their work from the live list.
+// ---- k_search: I1 + I2a of the iteration — apply the previous increment to the source (:1260, in registers),
+//      exact radius-bounded 1-NN on the hashed multi-level grid (nn_search_walk, search_core.cuh — replaces the kd-tree
+//      query of :1745), claim the target for the duplicate check. Resident blocks fetch their work from the live list.
+//      Per active source it reads the stored position and original index and the previous match (not in iteration 0,
+//      which has none), and writes the match and its distance: the moved source is not stored.
 // Iterations 0 .. kKeepFromIter-1 ("direct"): work unit = a quarter chunk (32 sources) per WARP, one query per lane,
 //   no cooperation and no barrier; the last of them also leaves a certificate per query (src_cert: where the query
 //   stood, and a radius inside which its match is the only target).
 // From iteration kKeepFromIter on ("keep"): work unit = a chunk per BLOCK, two passes:
 //   A  every source: transform, then try to KEEP the previous match without a search: if |p - q| + |p - p_ref| stays
 //      below the certificate radius, q is still the unique nearest target and its distance is computed directly (the
-//      result a search would return, bit for bit). Queries that cannot be kept are listed in shared memory;
+//      result a search would return, bit for bit). Queries that cannot be kept are listed in shared memory, with their
+//      moved position and original index;
 //   B  the listed queries, densely packed into the first threads of the block: seeded exact search, new certificate.
+//   Every source a keep test reads a certificate of was searched with one in iteration kKeepFromIter-1 or in a later
+//   pass B: `active` can only turn from true to false (n_src_g only shrinks), and pass A reads src_cert of active
+//   classes only.
 //   Late iterations keep most matches (measured on the C2 pair: 41 / 54 / 86 % in iterations 3 / 4 / 5; ~100 % once
 //   converged), and what is kept costs the streaming pass A only. (A variant with pass B fed from ONE queue in HBM —
 //   dense warps whatever chunk a source comes from, no barrier — was slower in iterations 3 / 4 / 5: the queue
@@ -176,13 +188,14 @@ __device__ __forceinline__ void search_finish(DeviceArrays &A, const PairConst &
 // seeded exact search of one query (p already advanced). Seeds: the previous iteration's match (a real candidate, so
 // the box-distance pruning bites from the first cell on and the search only has to prove that nothing is closer); a
 // match that the last increment left far away (the big first corrections) is challenged by a fresh greedy descent.
+// seeded = false (iteration 0): there is no previous match, and src_prevj is not read.
 template <class Bounds>
 __device__ __forceinline__ void search_one(DeviceArrays &A, const PairConst &pc, int c, int buf, uint32_t gi, const float4 p,
-                                           float orig_bits, const SearchFrame &f, bool write_cert) {
+                                           float orig_bits, const SearchFrame &f, bool write_cert, bool seeded) {
     NoStats st;
     int best_j = -1;
     float best_d2 = INFINITY;
-    const int pj = A.src_prevj[buf][gi];
+    const int pj = seeded ? A.src_prevj[buf][gi] : -1;
     if (pj >= 0) {
         const float4 q = __ldg(&f.g.pos[pj]);
         best_d2 = flann_l2(p.x, p.y, p.z, q.x, q.y, q.z);
@@ -214,23 +227,23 @@ __device__ __forceinline__ void search_quarter(DeviceArrays &A, int buf, uint32_
     if ((int)cd.first >= ns) return; // warp-uniform
     if (shoots(pc, c)) return;       // warp-uniform: k_search_shoot's work
     const uint32_t local = cd.first + 32u * sub + (threadIdx.x & 31u);
-    const bool valid = (int)local < ns;
-    const uint32_t gi = pc.src_base[c] + (valid ? local : 0);
-    float4 p, n;
-    load_and_advance(A, ps, buf, gi, valid, p, n);
-    if (!valid) return;
+    if ((int)local >= ns) return;
+    const uint32_t gi = pc.src_base[c] + local;
     // determine_corres needs >= 3 points on both sides (:1727-1728)
     if (!(pc.used[c] && nsg >= 3 && nt >= 3)) {
         A.nn_idx[gi] = -1;
         A.nn_d2[gi] = INFINITY;
         return;
     }
+    const float4 p = advanced_pos(ps, A.src_pos[buf][gi]);
     const SearchFrame f = search_frame(A, pc, ps, c);
-    search_one<Bounds>(A, pc, c, buf, gi, p, n.w, f, write_cert);
+    search_one<Bounds>(A, pc, c, buf, gi, p, A.src_nrm[buf][gi].w, f, write_cert, ps.iter > 0);
 }
 
-// keep mode: one block, one chunk. need_list / n_need live in shared memory.
-__device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint32_t chunk, uint8_t *need_list, uint32_t *n_need) {
+// keep mode: one block, one chunk. need_list / carry / n_need live in shared memory; carry[k] = the moved position of
+// the k-th listed query, its original index in .w.
+__device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint32_t chunk, uint8_t *need_list, float4 *carry,
+                                                  uint32_t *n_need) {
     const ChunkDesc cd = A.it_chunks[chunk];
     const PairConst &pc = A.pc[cd.pair];
     const PairState &ps = A.ps[cd.pair];
@@ -249,8 +262,7 @@ __device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint
         const uint32_t local = cd.first + threadIdx.x;
         const bool valid = (int)local < ns;
         const uint32_t gi = pc.src_base[c] + (valid ? local : 0);
-        float4 p, n;
-        load_and_advance(A, ps, buf, gi, valid, p, n);
+        float4 p = make_float4(0.f, 0.f, 0.f, 0.f); // (moved position; .w = original index)
         bool need = false;
         if (valid) {
             if (!active) {
@@ -258,6 +270,8 @@ __device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint
                 A.nn_d2[gi] = INFINITY;
             } else {
                 need = true;
+                p = advanced_pos(ps, A.src_pos[buf][gi]);
+                p.w = A.src_nrm[buf][gi].w;
                 const int pj = A.src_prevj[buf][gi];
                 const float4 ce = A.src_cert[buf][gi]; // p_ref, certificate radius (0: none)
                 if (pj >= 0 && ce.w > 0.0f) {
@@ -267,7 +281,7 @@ __device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint
                     // every other target t: |p - t| >= |p_ref - t| - |p - p_ref| >= radius - moved. The factors and the
                     // 3e-5 m absorb the float evaluation of all the distances involved (coordinates < 1 km)
                     if ((sqrtf(d1) + sqrtf(mv)) * 1.0001f + 3e-5f < ce.w * 0.9999f) {
-                        search_finish(A, pc, c, gi, pj, d1, f.max_dist_sqr, n.w);
+                        search_finish(A, pc, c, gi, pj, d1, f.max_dist_sqr, p.w);
                         need = false;
                     }
                 }
@@ -277,14 +291,18 @@ __device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint
         uint32_t base = 0;
         if (lane == 0 && m) base = atomicAdd(n_need, (uint32_t)__popc(m));
         base = __shfl_sync(0xffffffffu, base, 0);
-        if (need) need_list[base + __popc(m & ((1u << lane) - 1u))] = (uint8_t)threadIdx.x;
+        if (need) {
+            const uint32_t k = base + __popc(m & ((1u << lane) - 1u));
+            need_list[k] = (uint8_t)threadIdx.x;
+            carry[k] = p;
+        }
     }
     __syncthreads();
     // ---- pass B: the listed queries fill the first threads (whole warps stay out when few are left)
     if (threadIdx.x < *n_need) {
         const uint32_t gi = pc.src_base[c] + cd.first + need_list[threadIdx.x];
-        const float4 p = A.src_pos[buf][gi]; // (advanced by pass A)
-        search_one<WalkBounds>(A, pc, c, buf, gi, p, A.src_nrm[buf][gi].w, f, true);
+        const float4 p = carry[threadIdx.x];
+        search_one<WalkBounds>(A, pc, c, buf, gi, p, p.w, f, true, true);
     }
 }
 
@@ -305,8 +323,9 @@ __global__ void __launch_bounds__(kIterBlock, kSearchBlocksPerSm) k_search(Devic
     if (search_mode_of(it) != kMode) return;
     if (kMode == 2) {
         __shared__ uint8_t s_need[kIterBlock];
+        __shared__ float4 s_carry[kIterBlock];
         __shared__ uint32_t s_n_need;
-        for_each_live_chunk(A, buf, 0, [&](uint32_t chunk) { search_keep_chunk(A, buf, chunk, s_need, &s_n_need); });
+        for_each_live_chunk(A, buf, 0, [&](uint32_t chunk) { search_keep_chunk(A, buf, chunk, s_need, s_carry, &s_n_need); });
     } else {
         const uint32_t n_units = (kIterBlock / 32) * A.ctl->n_live[buf];
         const uint32_t *list = A.live_chunks + (size_t)buf * A.live_stride;
@@ -335,16 +354,14 @@ __device__ __forceinline__ void search_shoot_chunk(DeviceArrays &A, int buf, uin
     const int ns = ps.n_src[c], nt = ps.n_tgt[c], nsg = ps.n_src_g[c];
     if ((int)cd.first >= ns || !shoots(pc, c)) return; // block-uniform
     const uint32_t local = cd.first + threadIdx.x;
-    const bool valid = (int)local < ns;
-    const uint32_t gi = pc.src_base[c] + (valid ? local : 0);
-    float4 p, n;
-    load_and_advance(A, ps, buf, gi, valid, p, n);
-    if (!valid) return;
+    if ((int)local >= ns) return;
+    const uint32_t gi = pc.src_base[c] + local;
     if (!(pc.used[c] && nsg >= 3 && nt >= 3)) {
         A.nn_idx[gi] = -1;
         A.nn_d2[gi] = INFINITY;
         return;
     }
+    const float4 p = advanced_pos(ps, A.src_pos[buf][gi]), n = advanced_nrm(ps, A.src_nrm[buf][gi]);
     const GridView g = grid_of(A, pc, ps, c);
     const float max_distance_f = 2.5f * ps.thre;
     int sj = -1;
@@ -394,8 +411,8 @@ __device__ __forceinline__ void resolve_body(DeviceArrays &A, int buf, uint32_t 
         bool corr = matched;
         kept = true;
         if (dedup) {
-            const float4 n = A.src_nrm[buf][gi];
-            const bool winner = matched && A.claim[pc.tgt_base[c] + j] == (unsigned)__float_as_int(n.w);
+            const float orig = A.src_nrm[buf][gi].w;
+            const bool winner = matched && A.claim[pc.tgt_base[c] + j] == (unsigned)__float_as_int(orig);
             kept = winner;
             corr = winner;
         }
@@ -404,7 +421,7 @@ __device__ __forceinline__ void resolve_body(DeviceArrays &A, int buf, uint32_t 
             const float d2 = A.nn_d2[gi];
             pass = d2 < ps.thre * ps.thre;
             if (pass && c != MULLS_VERTEX) {
-                const float4 n = A.src_nrm[buf][gi];
+                const float4 n = advanced_nrm(ps, A.src_nrm[buf][gi]);
                 const float4 m = A.tgt_nrm[pc.tgt_base[c] + j];
                 const double dot = (double)n.x * (double)m.x + (double)n.y * (double)m.y + (double)n.z * (double)m.z;
                 const float cos_angle = (float)fabs(dot);
@@ -431,7 +448,9 @@ __device__ __forceinline__ void resolve_body(DeviceArrays &A, int buf, uint32_t 
         if (p) atomicAdd(&ps.n_corr[c], p);
     }
 }
-__global__ void __launch_bounds__(kIterBlock) k_resolve(DeviceArrays A, int buf) {
+// 16 resident blocks per SM fill it (2048 threads); the bound holds the kernel to the 32 registers that allows
+constexpr int kResolveBlocksPerSm = 16;
+__global__ void __launch_bounds__(kIterBlock, kResolveBlocksPerSm) k_resolve(DeviceArrays A, int buf) {
     buf = loop_buf(A, buf);
     for_each_live_chunk(A, buf, 1, [&](uint32_t chunk) { resolve_body(A, buf, chunk); });
 }
@@ -803,18 +822,28 @@ __device__ __forceinline__ void accumulate_body(DeviceArrays &A, int buf, uint32
     __syncthreads();
     dst_local = s_base + s_off[warp] + __popc(kb & ((1u << lane) - 1u));
 
-    // (2) terms of the surviving correspondences
-    float w_store = 0.0f;
+    // (2) compaction into the other buffer (order preserved: :1776-1789), of the moved source: a source that is not kept
+    // is never read again
+    float4 p = make_float4(0, 0, 0, 0);
     int j = -1;
-    float4 p = make_float4(0, 0, 0, 0), n = make_float4(0, 0, 0, 0);
     float d2 = 0.0f;
-    if (valid) {
-        p = A.src_pos[buf][gi];
-        n = A.src_nrm[buf][gi];
+    const uint32_t gd = pc.src_base[c] + dst_local;
+    if (kept) {
+        p = advanced_pos(ps, A.src_pos[buf][gi]);
         j = A.nn_idx[gi];
         d2 = A.nn_d2[gi];
-        if (j >= 0) A.claim[pc.tgt_base[c] + j] = kClaimFree; // reset the table for the next iteration
+        // reset the claim table for the next iteration: where k_resolve checked duplicates, a claimed target was claimed
+        // by its winner, the one matched source that is kept; elsewhere every matched source is kept and resets its own.
+        // (Sharded runs clear the whole table before each search: a winner may belong to another rank.)
+        if (j >= 0) A.claim[pc.tgt_base[c] + j] = kClaimFree;
+        A.src_pos[buf ^ 1][gd] = p;
+        A.src_nrm[buf ^ 1][gd] = advanced_nrm(ps, A.src_nrm[buf][gi]);
+        A.src_prevj[buf ^ 1][gd] = j;
+        // certificates exist from the iteration before the first keep test on (k_search<1>)
+        if (ps.iter >= kKeepFromIter - 1) A.src_cert[buf ^ 1][gd] = A.src_cert[buf][gi];
     }
+    // (3) terms of the surviving correspondences (pass implies kept)
+    float w_store = 0.0f;
     uint32_t n_corr[kNumClasses]; // complete since every k_resolve block of the pair has finished
 #pragma unroll
     for (int k = 0; k < kNumClasses; ++k) n_corr[k] = ps.n_corr[k];
@@ -839,13 +868,7 @@ __device__ __forceinline__ void accumulate_body(DeviceArrays &A, int buf, uint32
 #pragma unroll
         for (int k = 0; k < 27; ++k) t[k] = 0.0;
     }
-    // (3) compaction into the other buffer (order preserved: :1776-1789)
     if (kept) {
-        const uint32_t gd = pc.src_base[c] + dst_local;
-        A.src_pos[buf ^ 1][gd] = p;
-        A.src_nrm[buf ^ 1][gd] = n;
-        A.src_prevj[buf ^ 1][gd] = j;
-        A.src_cert[buf ^ 1][gd] = A.src_cert[buf][gi];
         A.corr_j[gd] = pass ? j : -1;
         A.corr_w[gd] = w_store;
     }
@@ -991,6 +1014,7 @@ __global__ void __launch_bounds__(kIterBlock, 4) k_icp_loop(DeviceArrays A) {
     cg::grid_group grid = cg::this_grid();
     LoopCtl &ctl = *A.ctl;
     __shared__ uint8_t s_need[kIterBlock];
+    __shared__ float4 s_carry[kIterBlock];
     __shared__ uint32_t s_n_need;
     const int n_pairs = ctl.n_pairs, max_iter = ctl.max_iter;
     for (int it = 0; it < max_iter; ++it) {
@@ -1001,7 +1025,7 @@ __global__ void __launch_bounds__(kIterBlock, 4) k_icp_loop(DeviceArrays A) {
         // phase 1: transform + search (+ keep) + claim
         for (uint32_t w = blockIdx.x; w < n_live; w += gridDim.x) {
             const uint32_t chunk = list[w];
-            if (it >= kKeepFromIter) search_keep_chunk(A, buf, chunk, s_need, &s_n_need);
+            if (it >= kKeepFromIter) search_keep_chunk(A, buf, chunk, s_need, s_carry, &s_n_need);
             else if (it == kKeepFromIter - 1) search_quarter<WalkBounds>(A, buf, chunk, threadIdx.x >> 5, true);
             else search_quarter<NoBounds>(A, buf, chunk, threadIdx.x >> 5, false);
             __syncthreads();

@@ -863,7 +863,7 @@ static void launch_search(mulls_ctx *ctx, cudaStream_t st, const DeviceArrays &A
     if (mode < 0 || mode == 1) k_search<1><<<grid, kIterBlock, 0, st>>>(A, buf, it);
     if (mode < 0 || mode == 2) k_search<2><<<grid, kIterBlock, 0, st>>>(A, buf, it);
 }
-constexpr int kShootBlocksPerSm = 8, kResolveBlocksPerSm = 16, kAccumulateBlocksPerSm = 8;
+constexpr int kShootBlocksPerSm = 8, kAccumulateBlocksPerSm = 8;
 constexpr int kPollPause = 64; // _mm_pause() count between two cudaEventQuery calls of the launch loop's flow control
 
 // The iteration loop as a CUDA graph (CUDA 12.4+ conditional nodes): WHILE(handle) { k_search [, k_search_shoot],
