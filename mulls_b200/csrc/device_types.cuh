@@ -17,7 +17,7 @@ constexpr int kMaxLevels = 12;
 constexpr int kCoordBits = 12;            // Morton bits per axis
 constexpr int kDedupMinSrc = 500;         // K_filter_distant_point (cregistration.hpp:1704)
 constexpr unsigned kClaimFree = 0x7f7f7f7fu;
-constexpr int kIterFlags = 256;           // per-iteration stop flags kept for the launch loop of sharded runs
+constexpr int kIterFlags = MULLS_MAX_TRACE_ITERS; // per-iteration stop flags kept for the launch loop of sharded runs
 
 enum PairStatus : int { kRunning = 0, kNeedPosterior = 1, kDone = 2 };
 

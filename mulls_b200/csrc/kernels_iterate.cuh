@@ -309,7 +309,7 @@ __device__ __forceinline__ void search_keep_chunk(DeviceArrays &A, int buf, uint
 // One kernel per mode (own register allocation each): 0 = direct, 1 = direct + certificate, 2 = keep. The iteration
 // graph holds all three; the two that are not this iteration's return at once.
 constexpr int kSearchBlocksPerSm = 10; // 48 registers; the fastest of 8 / 10 / 12 / 16 on H100 (records/h100_search_blocks_sweep.json)
-__device__ __forceinline__ int search_mode_of(int it) { return it >= kKeepFromIter ? 2 : (it == kKeepFromIter - 1 ? 1 : 0); }
+__host__ __device__ __forceinline__ int search_mode_of(int it) { return it >= kKeepFromIter ? 2 : (it == kKeepFromIter - 1 ? 1 : 0); }
 
 template <int kMode>
 __global__ void __launch_bounds__(kIterBlock, kSearchBlocksPerSm) k_search(DeviceArrays A, int buf, int it) {
@@ -1023,10 +1023,11 @@ __global__ void __launch_bounds__(kIterBlock, 4) k_icp_loop(DeviceArrays A) {
         const uint32_t n_live = ctl.n_live[buf];
         if (blockIdx.x == 0 && threadIdx.x == 0) ctl.n_live[buf ^ 1] = 0u; // (k_solve's phase fills it, three barriers later)
         // phase 1: transform + search (+ keep) + claim
+        const int mode = search_mode_of(it);
         for (uint32_t w = blockIdx.x; w < n_live; w += gridDim.x) {
             const uint32_t chunk = list[w];
-            if (it >= kKeepFromIter) search_keep_chunk(A, buf, chunk, s_need, s_carry, &s_n_need);
-            else if (it == kKeepFromIter - 1) search_quarter<WalkBounds>(A, buf, chunk, threadIdx.x >> 5, true);
+            if (mode == 2) search_keep_chunk(A, buf, chunk, s_need, s_carry, &s_n_need);
+            else if (mode == 1) search_quarter<WalkBounds>(A, buf, chunk, threadIdx.x >> 5, true);
             else search_quarter<NoBounds>(A, buf, chunk, threadIdx.x >> 5, false);
             __syncthreads();
         }

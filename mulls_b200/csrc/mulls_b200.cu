@@ -118,6 +118,7 @@ struct mulls_ctx {
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t graph_exec = nullptr;
     int graph_key[2] = {-1, -1}; // the batch shape baked into the kernel nodes
+    uint64_t graph_body_launches = 0, graph_tail_launches = 0; // kernels recorded per loop iteration and after the loop
     LoopCtl *h_ctl = nullptr;            // pinned staging of the control block
     int num_sms = 132;
     bool any_normal_shooting = false;
@@ -203,6 +204,11 @@ static inline double wall_ms() {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
+static void drop_iteration_graph(mulls_ctx *ctx) {
+    if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec), ctx->graph_exec = nullptr;
+    if (ctx->graph) cudaGraphDestroy(ctx->graph), ctx->graph = nullptr;
+}
+
 // The device arrays of one call in one Scratch: take() hands out 256-byte aligned offsets, grow() makes the Scratch
 // hold them all and sets `base`, from which each array is at its offset.
 struct ScratchLayout {
@@ -264,8 +270,7 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->h_running) cudaFreeHost(ctx->h_running);
     if (ctx->nccl_comm && nccl_api().ok) nccl_api().destroy(ctx->nccl_comm);
     if (ctx->h_ctl) cudaFreeHost(ctx->h_ctl);
-    if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
-    if (ctx->graph) cudaGraphDestroy(ctx->graph);
+    drop_iteration_graph(ctx);
     if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
     for (cudaEvent_t e : ctx->ev_done) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->ev_search) cudaEventDestroy(e);
@@ -765,6 +770,13 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
     return MULLS_OK;
 }
 
+// One cross-rank all-reduce of a sharded run: the caller's callback enqueues it on the context's stream.
+static int exchange(mulls_ctx *ctx, mulls_allreduce_fn hook, void *user, void *buf, size_t count, int dtype, int op) {
+    if (hook(user, buf, count, dtype, op, (void *)ctx->stream) == 0) return MULLS_OK;
+    ctx->err = "all-reduce callback failed";
+    return MULLS_E_COMM;
+}
+
 // Ingest phase on the resident inputs: state reset, initial guess, intersection filter, Morton sort,
 // hashed multi-level grid. Shared by the registration path and mulls_pca_features. finite_only (mulls_sor_filter, no
 // source, no motion undistortion): points with a non-finite coordinate stay out of the bbox and of the grid.
@@ -786,10 +798,7 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
     }
     if (hook) { // sharded source: the intersection filter needs the bbox over all shards
         k_shard_pack_setup<<<1, 1, 0, st>>>(A, 0);
-        if (hook(user, A.xch_i32, 6, 1, 1, (void *)st) != 0) {
-            ctx->err = "all-reduce callback failed";
-            return MULLS_E_COMM;
-        }
+        if (const int rc = exchange(ctx, hook, user, A.xch_i32, 6, 1, 1); rc != MULLS_OK) return rc;
         k_shard_pack_setup<<<1, 1, 0, st>>>(A, 1);
         launches += 2;
     }
@@ -821,10 +830,7 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
     ++launches;
     if (hook) { // global class sizes (:1195-1201 counts, K_filter_distant_point test)
         k_shard_pack_setup<<<1, 1, 0, st>>>(A, 2);
-        if (hook(user, A.xch_i32, kNumClasses, 1, 0, (void *)st) != 0) {
-            ctx->err = "all-reduce callback failed";
-            return MULLS_E_COMM;
-        }
+        if (const int rc = exchange(ctx, hook, user, A.xch_i32, kNumClasses, 1, 0); rc != MULLS_OK) return rc;
         k_shard_pack_setup<<<1, 1, 0, st>>>(A, 3);
         launches += 2;
     }
@@ -854,54 +860,109 @@ static unsigned chunk_bucket(const mulls_ctx *ctx) {
 static unsigned resident_grid(const mulls_ctx *ctx, int blocks_per_sm) {
     return std::min((unsigned)(ctx->num_sms * blocks_per_sm), chunk_bucket(ctx));
 }
-// it < 0 (recording the iteration graph): all three modes, each checks the device-side iteration counter; the host
-// launch loop knows the iteration and launches the one that runs
-static void launch_search(mulls_ctx *ctx, cudaStream_t st, const DeviceArrays &A, int buf, int it) {
-    const unsigned grid = resident_grid(ctx, kSearchBlocksPerSm);
-    const int mode = it < 0 ? -1 : (it >= kKeepFromIter ? 2 : (it == kKeepFromIter - 1 ? 1 : 0));
-    if (mode < 0 || mode == 0) k_search<0><<<grid, kIterBlock, 0, st>>>(A, buf, it);
-    if (mode < 0 || mode == 1) k_search<1><<<grid, kIterBlock, 0, st>>>(A, buf, it);
-    if (mode < 0 || mode == 2) k_search<2><<<grid, kIterBlock, 0, st>>>(A, buf, it);
-}
 constexpr int kShootBlocksPerSm = 8, kAccumulateBlocksPerSm = 8;
 constexpr int kPollPause = 64; // _mm_pause() count between two cudaEventQuery calls of the launch loop's flow control
 
-// The iteration loop as a CUDA graph (CUDA 12.4+ conditional nodes): WHILE(handle) { k_search [, k_search_shoot],
-// k_resolve, k_accumulate, k_solve } followed by k_posterior, k_finalize, k_collect. Kernel nodes are recorded once per
-// context with grids sized for its capacity; what a run needs to know (chunk / pair counts, trace switch, loop counter)
-// is read from LoopCtl in device memory. k_solve's last block sets the loop condition: no host polling, one launch.
+// One ICP iteration: k_search [, k_search_shoot], k_resolve, k_accumulate, k_solve, and a sharded run's three exchanges.
+// it < 0 records the graph's loop body: all three k_search modes (each checks the device-side iteration counter) and
+// k_solve over every pair slot, setting the loop condition `handle`. it >= 0 is iteration `it` of the host launch loop:
+// its one search mode, exact grids, the search timed by ev_search[2it], ev_search[2it+1]. Counts its kernels in `launches`.
+static int enqueue_iteration(mulls_ctx *ctx, int it, mulls_allreduce_fn hook, void *user, unsigned long long handle,
+                             uint64_t &launches) {
+    cudaStream_t st = ctx->stream;
+    const DeviceArrays &A = ctx->A;
+    const bool recording = it < 0;
+    const int buf = recording ? -1 : it & 1;
+    if (hook) // other ranks' claims of the previous iteration must not survive in this rank's table
+        CK(cudaMemsetAsync(A.claim, 0x7f, std::max<size_t>(ctx->n_tgt_total, 1) * sizeof(unsigned), st));
+    if (!recording) CK(cudaEventRecord(ctx->ev_search[2 * it], st));
+    const unsigned search_grid = resident_grid(ctx, kSearchBlocksPerSm);
+    const int mode = recording ? -1 : search_mode_of(it);
+    if (mode < 0 || mode == 0) k_search<0><<<search_grid, kIterBlock, 0, st>>>(A, buf, it);
+    if (mode < 0 || mode == 1) k_search<1><<<search_grid, kIterBlock, 0, st>>>(A, buf, it);
+    if (mode < 0 || mode == 2) k_search<2><<<search_grid, kIterBlock, 0, st>>>(A, buf, it);
+    launches += recording ? 3 : 1;
+    if (ctx->any_normal_shooting) {
+        k_search_shoot<<<resident_grid(ctx, kShootBlocksPerSm), kIterBlock, 0, st>>>(A, buf);
+        ++launches;
+    }
+    if (!recording) CK(cudaEventRecord(ctx->ev_search[2 * it + 1], st));
+    if (hook) { // exchange 1: the duplicate-check claims of all shards (min of source indices)
+        if (const int rc = exchange(ctx, hook, user, A.claim, ctx->n_tgt_total, 1, 1); rc != MULLS_OK) return rc;
+    }
+    k_resolve<<<resident_grid(ctx, kResolveBlocksPerSm), kIterBlock, 0, st>>>(A, buf);
+    if (hook) { // exchange 2: correspondence counts (w_ground, -2 test) and surviving source counts
+        k_shard_counts<<<1, kIterBlock, 0, st>>>(A, 0);
+        if (const int rc = exchange(ctx, hook, user, A.xch_i32, 2 * kNumClasses, 1, 0); rc != MULLS_OK) return rc;
+        k_shard_counts<<<1, kIterBlock, 0, st>>>(A, 1);
+        launches += 2;
+    }
+    k_accumulate<<<resident_grid(ctx, kAccumulateBlocksPerSm), kIterBlock, 0, st>>>(A, buf);
+    k_solve<<<recording ? (unsigned)std::max<size_t>(ctx->max_pairs, 1) : (unsigned)ctx->n_pairs, kSolveThreads, 0, st>>>(A, buf, handle);
+    launches += 3;
+    if (hook) { // exchange 3: per-class normal-equation sums; then every rank solves the same system
+        if (const int rc = exchange(ctx, hook, user, A.xch_f64, kNumClasses * kTerms, 0, 0); rc != MULLS_OK) return rc;
+        k_shard_solve<<<1, 32, 0, st>>>(A, buf, it);
+        ++launches;
+    }
+    return MULLS_OK;
+}
+
+// What follows the loop: k_posterior, k_finalize (sharded: k_shard_post, exchange, k_shard_post), k_collect. recording
+// (the iteration graph): grids for the context's capacity. Otherwise exact grids, and ev_iter before k_collect.
+static int enqueue_tail(mulls_ctx *ctx, bool recording, mulls_allreduce_fn hook, void *user, uint64_t &launches) {
+    cudaStream_t st = ctx->stream;
+    const DeviceArrays &A = ctx->A;
+    const unsigned pairs = recording ? (unsigned)std::max<size_t>(ctx->max_pairs, 1) : (unsigned)ctx->n_pairs;
+    const int np = recording ? -1 : (int)ctx->n_pairs;
+    k_posterior<<<recording ? std::min((unsigned)std::max<size_t>(ctx->cap_it_chunks, 1), chunk_bucket(ctx))
+                            : (unsigned)ctx->h_it_chunks.size(), kIterBlock, 0, st>>>(A);
+    if (hook) {
+        k_shard_post<<<1, 32, 0, st>>>(A, 0);
+        if (const int rc = exchange(ctx, hook, user, A.xch_f64, 2, 0, 0); rc != MULLS_OK) return rc;
+        k_shard_post<<<1, 32, 0, st>>>(A, 1);
+    } else {
+        k_finalize<<<(unsigned)ceil_div(pairs, 64), 64, 0, st>>>(A, np);
+    }
+    if (!recording) CK(cudaEventRecord(ctx->ev_iter, st));
+    k_collect<<<(unsigned)ceil_div(pairs, 128), 128, 0, st>>>(A, np, ctx->d_results);
+    launches += hook ? 4 : 3;
+    return MULLS_OK;
+}
+
+// The iteration loop as a CUDA graph (CUDA 12.4+ conditional nodes): WHILE(handle) { enqueue_iteration } followed by
+// enqueue_tail. Kernel nodes are recorded once per context with grids sized for its capacity; what a run needs to know
+// (chunk / pair counts, trace switch, loop counter) is read from LoopCtl in device memory. k_solve's last block sets the
+// loop condition: no host polling, one launch. A failed recording ends its capture and leaves no graph behind.
 static int build_iteration_graph(mulls_ctx *ctx) {
     const int key[2] = {(int)chunk_bucket(ctx), ctx->any_normal_shooting ? 1 : 0};
     if (ctx->graph_exec && std::memcmp(key, ctx->graph_key, sizeof(key)) == 0) return MULLS_OK;
-    if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec), ctx->graph_exec = nullptr;
-    if (ctx->graph) cudaGraphDestroy(ctx->graph), ctx->graph = nullptr;
+    drop_iteration_graph(ctx);
     cudaStream_t st = ctx->stream;
-    DeviceArrays A = ctx->A;
-    const unsigned cap_chunks = (unsigned)std::max<size_t>(ctx->cap_it_chunks, 1), cap_pairs = (unsigned)std::max<size_t>(ctx->max_pairs, 1);
-    CK(cudaGraphCreate(&ctx->graph, 0));
-    cudaGraphConditionalHandle handle;
-    CK(cudaGraphConditionalHandleCreate(&handle, ctx->graph, 1, cudaGraphCondAssignDefault));
-    cudaGraphNodeParams wp = {cudaGraphNodeTypeConditional};
-    wp.conditional.handle = handle;
-    wp.conditional.type = cudaGraphCondTypeWhile;
-    wp.conditional.size = 1;
-    cudaGraphNode_t while_node;
-    CK(cudaGraphAddNode(&while_node, ctx->graph, nullptr, 0, &wp));
-    cudaGraph_t body = wp.conditional.phGraph_out[0];
-    CK(cudaStreamBeginCaptureToGraph(st, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    launch_search(ctx, st, A, -1, -1);
-    if (ctx->any_normal_shooting)
-        k_search_shoot<<<resident_grid(ctx, kShootBlocksPerSm), kIterBlock, 0, st>>>(A, -1);
-    k_resolve<<<resident_grid(ctx, kResolveBlocksPerSm), kIterBlock, 0, st>>>(A, -1);
-    k_accumulate<<<resident_grid(ctx, kAccumulateBlocksPerSm), kIterBlock, 0, st>>>(A, -1);
-    k_solve<<<cap_pairs, kSolveThreads, 0, st>>>(A, -1, (unsigned long long)handle);
-    CK(cudaStreamEndCapture(st, nullptr));
-    CK(cudaStreamBeginCaptureToGraph(st, ctx->graph, &while_node, nullptr, 1, cudaStreamCaptureModeThreadLocal));
-    k_posterior<<<std::min(cap_chunks, chunk_bucket(ctx)), kIterBlock, 0, st>>>(A);
-    k_finalize<<<(unsigned)ceil_div(cap_pairs, 64), 64, 0, st>>>(A, -1);
-    k_collect<<<(unsigned)ceil_div(cap_pairs, 128), 128, 0, st>>>(A, -1, ctx->d_results);
-    CK(cudaStreamEndCapture(st, nullptr));
-    CK(cudaGraphInstantiate(&ctx->graph_exec, ctx->graph, 0));
+    const int rc = [&]() -> int {
+        CK(cudaGraphCreate(&ctx->graph, 0));
+        cudaGraphConditionalHandle handle;
+        CK(cudaGraphConditionalHandleCreate(&handle, ctx->graph, 1, cudaGraphCondAssignDefault));
+        cudaGraphNodeParams wp = {cudaGraphNodeTypeConditional};
+        wp.conditional.handle = handle;
+        wp.conditional.type = cudaGraphCondTypeWhile;
+        wp.conditional.size = 1;
+        cudaGraphNode_t while_node;
+        CK(cudaGraphAddNode(&while_node, ctx->graph, nullptr, 0, &wp));
+        uint64_t body = 0, tail = 0;
+        CK(cudaStreamBeginCaptureToGraph(st, wp.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+        int rc = enqueue_iteration(ctx, -1, nullptr, nullptr, (unsigned long long)handle, body);
+        CK(cudaStreamEndCapture(st, nullptr)); // (before rc is tested: the stream leaves capture mode in any case)
+        if (rc != MULLS_OK) return rc;
+        CK(cudaStreamBeginCaptureToGraph(st, ctx->graph, &while_node, nullptr, 1, cudaStreamCaptureModeThreadLocal));
+        rc = enqueue_tail(ctx, true, nullptr, nullptr, tail);
+        CK(cudaStreamEndCapture(st, nullptr));
+        if (rc != MULLS_OK) return rc;
+        CK(cudaGraphInstantiate(&ctx->graph_exec, ctx->graph, 0));
+        ctx->graph_body_launches = body, ctx->graph_tail_launches = tail;
+        return MULLS_OK;
+    }();
+    if (rc != MULLS_OK) return drop_iteration_graph(ctx), rc;
     std::memcpy(ctx->graph_key, key, sizeof(key));
     return MULLS_OK;
 }
@@ -926,219 +987,151 @@ static int grow_hash_pool(mulls_ctx *ctx) {
     CK(cudaFree(A.hash));
     A.hash = fresh;
     A.hash_pool_entries = need;
-    if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec), ctx->graph_exec = nullptr;
-    if (ctx->graph) cudaGraphDestroy(ctx->graph), ctx->graph = nullptr;
+    drop_iteration_graph(ctx);
     return MULLS_OK;
 }
 
+// run_impl and run_finish return through here: an error exit may leave async copies from / into the caller's buffers
+// (clouds, trace, results) in flight, so nothing is handed back before the stream has drained.
+static int drain_on_error(mulls_ctx *ctx, int rc) {
+    if (rc != MULLS_OK && ctx && ctx->stream) cudaStreamSynchronize(ctx->stream);
+    return rc;
+}
+
+static int run_finish(mulls_ctx *ctx, mulls_icp_result *out);
 // Launch the whole path on the resident inputs. If `hook` is given (sharded mode) it is called between
 // the phases that need a cross-rank exchange.
-static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace *trace, mulls_allreduce_fn hook, void *user,
-                          bool finish_now);
-static int run_finish_inner(mulls_ctx *ctx, mulls_icp_result *out);
 // finish_now = false: everything is enqueued on the context's stream and the call returns; run_finish waits for it
 static int run_impl(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace *trace, mulls_allreduce_fn hook, void *user,
                     bool finish_now = true) {
-    const int rc = run_impl_inner(ctx, out, trace, hook, user, finish_now);
-    // an error exit may leave async copies from / into the caller's buffers (clouds, trace, results) in flight:
-    // nothing is handed back before the stream has drained
-    if (rc != MULLS_OK && ctx && ctx->stream) cudaStreamSynchronize(ctx->stream);
-    return rc;
-}
-static int run_finish(mulls_ctx *ctx, mulls_icp_result *out) {
-    const int rc = run_finish_inner(ctx, out);
-    if (rc != MULLS_OK && ctx && ctx->stream) cudaStreamSynchronize(ctx->stream);
-    return rc;
-}
-static int run_impl_inner(mulls_ctx *ctx, mulls_icp_result *out, mulls_icp_trace *trace, mulls_allreduce_fn hook, void *user,
-                          bool finish_now) {
-    if (!ctx || !ctx->uploaded) return MULLS_E_ARG;
-    ctx->pend.active = false;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
-    DeviceArrays A = ctx->A;
-    const int np = (int)ctx->n_pairs;
-    uint64_t launches = 0;
-    CK(cudaEventRecord(ctx->ev_begin, st));
-    {
-        int rc = launch_ingest(ctx, A, trace != nullptr, launches, hook, user);
-        if (rc != MULLS_OK) return rc;
-    }
-    const unsigned n_itc = (unsigned)ctx->h_it_chunks.size();
-    {
-        LoopCtl &c = *ctx->h_ctl; // (the previous run has been synchronised: the staging copy is free)
-        c = LoopCtl();
-        c.n_it_chunks = (int)n_itc, c.n_pairs = np, c.trace_on = trace ? 1 : 0, c.max_iter = ctx->max_iter_max;
-        CK(cudaMemcpyAsync(A.ctl, ctx->h_ctl, sizeof(LoopCtl), cudaMemcpyHostToDevice, st));
-        if (n_itc) { // the chunks that own source points after the intersection filter: work list of iteration 0
+    return drain_on_error(ctx, [&]() -> int {
+        if (!ctx || !ctx->uploaded) return MULLS_E_ARG;
+        ctx->pend.active = false;
+        CK(cudaSetDevice(ctx->device));
+        cudaStream_t st = ctx->stream;
+        DeviceArrays A = ctx->A;
+        const int np = (int)ctx->n_pairs;
+        uint64_t launches = 0;
+        CK(cudaEventRecord(ctx->ev_begin, st));
+        if (const int rc = launch_ingest(ctx, A, trace != nullptr, launches, hook, user); rc != MULLS_OK) return rc;
+        const unsigned n_itc = (unsigned)ctx->h_it_chunks.size(); // (>= 1: upload_impl gives class 0 of every pair a chunk)
+        {
+            LoopCtl &c = *ctx->h_ctl; // (the previous run has been synchronised: the staging copy is free)
+            c = LoopCtl();
+            c.n_it_chunks = (int)n_itc, c.n_pairs = np, c.trace_on = trace ? 1 : 0, c.max_iter = ctx->max_iter_max;
+            CK(cudaMemcpyAsync(A.ctl, ctx->h_ctl, sizeof(LoopCtl), cudaMemcpyHostToDevice, st));
+            // the chunks that own source points after the intersection filter: work list of iteration 0
             k_live_init<<<(unsigned)ceil_div(n_itc, 256), 256, 0, st>>>(A);
             ++launches;
         }
-    }
-    // small batches: one cooperative kernel runs the whole loop (every chunk and every pair must find a co-resident block)
-    bool looped = false;
-    if (!hook && ctx->use_graph && !ctx->any_normal_shooting && n_itc > 0) {
-        if (ctx->loop_kernel_blocks == 0) {
-            int per_sm = 0, coop = 0;
-            cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx->device);
-            if (coop && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_icp_loop, kIterBlock, 0) == cudaSuccess && per_sm > 0)
-                ctx->loop_kernel_blocks = per_sm * ctx->num_sms;
-            else
-                ctx->loop_kernel_blocks = -1, cudaGetLastError();
+        // small batches: one cooperative kernel runs the whole loop (every chunk and every pair must find a co-resident block)
+        bool looped = false;
+        if (!hook && ctx->use_graph && !ctx->any_normal_shooting) {
+            if (ctx->loop_kernel_blocks == 0) {
+                int per_sm = 0, coop = 0;
+                cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx->device);
+                if (coop && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_icp_loop, kIterBlock, 0) == cudaSuccess && per_sm > 0)
+                    ctx->loop_kernel_blocks = per_sm * ctx->num_sms;
+                else
+                    ctx->loop_kernel_blocks = -1, cudaGetLastError();
+            }
+            looped = ctx->loop_kernel_blocks > 0 && n_itc <= (unsigned)ctx->loop_kernel_blocks && np <= ctx->loop_kernel_blocks;
         }
-        looped = ctx->loop_kernel_blocks > 0 && n_itc <= (unsigned)ctx->loop_kernel_blocks && np <= ctx->loop_kernel_blocks;
-    }
-    const bool graphed = !hook && ctx->use_graph && !looped;
-    if (graphed) {
-        const int rc = build_iteration_graph(ctx);
-        if (rc != MULLS_OK) return rc;
-    }
-    CK(cudaEventRecord(ctx->ev_ingest, st));
-    int n_search_ev = 0;
-    if (looped) {
-        DeviceArrays Aarg = A;
-        void *args[] = {&Aarg};
-        const unsigned grid = std::max(1u, std::min((unsigned)ctx->loop_kernel_blocks, std::max(n_itc, (unsigned)np)));
-        CK(cudaLaunchCooperativeKernel((const void *)k_icp_loop, dim3(grid), dim3(kIterBlock), args, 0, st));
-        k_posterior<<<n_itc, kIterBlock, 0, st>>>(A);
-        k_finalize<<<(unsigned)ceil_div(np, 64), 64, 0, st>>>(A, np);
-        launches += 3;
-    } else if (graphed) {
-        CK(cudaGraphLaunch(ctx->graph_exec, st));
-        CK(cudaMemcpyAsync(ctx->h_ctl, A.ctl, sizeof(LoopCtl), cudaMemcpyDeviceToHost, st)); // iterations executed
-    } else if (n_itc) {
-        for (int it = 0; it < ctx->max_iter_max; ++it) {
-            // flow control: stay at most two iterations ahead of the device and stop launching as soon
-            // as every pair has converged or failed (the device mirrors its counter into mapped memory)
-            if (it >= 2) {
-                // (poll with pauses: several contexts spinning inside the driver slow each other's launches down)
-                while (cudaEventQuery(ctx->ev_done[it - 2]) == cudaErrorNotReady)
-                    for (int k = 0; k < kPollPause; ++k) _mm_pause();
-                // Sharded runs must take this decision identically on every rank (the ranks issue matching collectives):
-                // they read the count the device recorded at the END of iteration it-2 — written once, before
-                // ev_done[it-2] — never the live flag, whose value at this instant depends on each rank's timing.
-                if (hook ? ((volatile int *)ctx->h_running)[1 + std::min(it - 2, kIterFlags - 1)] <= 0
-                         : *(volatile int *)ctx->h_running <= 0)
-                    break;
-            }
-            const int buf = it & 1;
-            if (hook) // other ranks' claims of the previous iteration must not survive in this rank's table
-                CK(cudaMemsetAsync(A.claim, 0x7f, std::max<size_t>(ctx->n_tgt_total, 1) * sizeof(unsigned), st));
-            CK(cudaEventRecord(ctx->ev_search[2 * it], st));
-            launch_search(ctx, st, A, buf, it);
-            if (ctx->any_normal_shooting) {
-                k_search_shoot<<<resident_grid(ctx, kShootBlocksPerSm), kIterBlock, 0, st>>>(A, buf);
-                ++launches;
-            }
-            CK(cudaEventRecord(ctx->ev_search[2 * it + 1], st));
-            if (hook) { // exchange 1: the duplicate-check claims of all shards (min of source indices)
-                if (hook(user, A.claim, ctx->n_tgt_total, 1, 1, (void *)st) != 0) {
-                    ctx->err = "all-reduce callback failed";
-                    return MULLS_E_COMM;
-                }
-            }
-            k_resolve<<<resident_grid(ctx, kResolveBlocksPerSm), kIterBlock, 0, st>>>(A, buf);
-            if (hook) { // exchange 2: correspondence counts (w_ground, -2 test) and surviving source counts
-                k_shard_counts<<<1, kIterBlock, 0, st>>>(A, 0);
-                if (hook(user, A.xch_i32, 2 * kNumClasses, 1, 0, (void *)st) != 0) {
-                    ctx->err = "all-reduce callback failed";
-                    return MULLS_E_COMM;
-                }
-                k_shard_counts<<<1, kIterBlock, 0, st>>>(A, 1);
-                launches += 2;
-            }
-            k_accumulate<<<resident_grid(ctx, kAccumulateBlocksPerSm), kIterBlock, 0, st>>>(A, buf);
-            k_solve<<<(unsigned)np, kSolveThreads, 0, st>>>(A, buf, 0ull);
-            if (hook) { // exchange 3: per-class normal-equation sums; then every rank solves the same system
-                if (hook(user, A.xch_f64, kNumClasses * kTerms, 0, 0, (void *)st) != 0) {
-                    ctx->err = "all-reduce callback failed";
-                    return MULLS_E_COMM;
-                }
-                k_shard_solve<<<1, 32, 0, st>>>(A, buf, std::min(it, kIterFlags - 1));
-                ++launches;
-            }
-            CK(cudaEventRecord(ctx->ev_done[it], st));
-            launches += 4;
-            n_search_ev = it + 1;
-        }
-        k_posterior<<<n_itc, kIterBlock, 0, st>>>(A);
-        if (hook) {
-            k_shard_post<<<1, 32, 0, st>>>(A, 0);
-            if (hook(user, A.xch_f64, 2, 0, 0, (void *)st) != 0) {
-                ctx->err = "all-reduce callback failed";
-                return MULLS_E_COMM;
-            }
-            k_shard_post<<<1, 32, 0, st>>>(A, 1);
-            launches += 3;
+        const bool graphed = !hook && ctx->use_graph && !looped;
+        if (const int rc = graphed ? build_iteration_graph(ctx) : MULLS_OK; rc != MULLS_OK) return rc;
+        CK(cudaEventRecord(ctx->ev_ingest, st));
+        int n_search_ev = 0;
+        if (graphed) {
+            CK(cudaGraphLaunch(ctx->graph_exec, st));
+            CK(cudaMemcpyAsync(ctx->h_ctl, A.ctl, sizeof(LoopCtl), cudaMemcpyDeviceToHost, st)); // iterations executed
+            CK(cudaEventRecord(ctx->ev_iter, st));
         } else {
-            k_finalize<<<(unsigned)ceil_div(np, 64), 64, 0, st>>>(A, np);
-            launches += 2;
+            if (looped) {
+                DeviceArrays Aarg = A;
+                void *args[] = {&Aarg};
+                const unsigned grid = std::max(1u, std::min((unsigned)ctx->loop_kernel_blocks, std::max(n_itc, (unsigned)np)));
+                CK(cudaLaunchCooperativeKernel((const void *)k_icp_loop, dim3(grid), dim3(kIterBlock), args, 0, st));
+                ++launches;
+            } else {
+                for (int it = 0; it < ctx->max_iter_max; ++it) {
+                    // flow control: stay at most two iterations ahead of the device and stop launching as soon
+                    // as every pair has converged or failed (the device mirrors its counter into mapped memory)
+                    if (it >= 2) {
+                        // (poll with pauses: several contexts spinning inside the driver slow each other's launches down)
+                        while (cudaEventQuery(ctx->ev_done[it - 2]) == cudaErrorNotReady)
+                            for (int k = 0; k < kPollPause; ++k) _mm_pause();
+                        // Sharded runs must take this decision identically on every rank (the ranks issue matching collectives):
+                        // they read the count the device recorded at the END of iteration it-2 — written once, before
+                        // ev_done[it-2] — never the live flag, whose value at this instant depends on each rank's timing.
+                        if (hook ? ((volatile int *)ctx->h_running)[1 + (it - 2)] <= 0 : *(volatile int *)ctx->h_running <= 0) break;
+                    }
+                    if (const int rc = enqueue_iteration(ctx, it, hook, user, 0ull, launches); rc != MULLS_OK) return rc;
+                    CK(cudaEventRecord(ctx->ev_done[it], st));
+                    n_search_ev = it + 1;
+                }
+            }
+            if (const int rc = enqueue_tail(ctx, false, hook, user, launches); rc != MULLS_OK) return rc;
         }
-    }
-    CK(cudaEventRecord(ctx->ev_iter, st));
-    if (!graphed) {
-        k_collect<<<(unsigned)ceil_div(np, 128), 128, 0, st>>>(A, np, ctx->d_results);
-        ++launches;
-    }
-    CK(cudaMemcpyAsync(ctx->h_results, ctx->d_results, np * (sizeof(mulls_icp_result) + sizeof(uint64_t)), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    if (trace) CK(cudaMemcpyAsync(trace, ctx->d_trace, np * sizeof(mulls_icp_trace), cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(ctx->ev_end, st));
-    ctx->pend.launches = launches, ctx->pend.n_search_ev = n_search_ev, ctx->pend.graphed = graphed, ctx->pend.hooked = hook != nullptr;
-    ctx->pend.trace = trace, ctx->pend.hook = hook, ctx->pend.user = user;
-    ctx->pend.active = true;
-    if (!finish_now) return MULLS_OK;
-    return run_finish_inner(ctx, out);
+        CK(cudaMemcpyAsync(ctx->h_results, ctx->d_results, np * (sizeof(mulls_icp_result) + sizeof(uint64_t)), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->h_flags, A.hash_used, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        if (trace) CK(cudaMemcpyAsync(trace, ctx->d_trace, np * sizeof(mulls_icp_trace), cudaMemcpyDeviceToHost, st));
+        CK(cudaEventRecord(ctx->ev_end, st));
+        ctx->pend.launches = launches, ctx->pend.n_search_ev = n_search_ev, ctx->pend.graphed = graphed, ctx->pend.hooked = hook != nullptr;
+        ctx->pend.trace = trace, ctx->pend.hook = hook, ctx->pend.user = user;
+        ctx->pend.active = true;
+        if (!finish_now) return MULLS_OK;
+        return run_finish(ctx, out);
+    }());
 }
 
-static int run_finish_inner(mulls_ctx *ctx, mulls_icp_result *out) {
-    if (!ctx || !ctx->pend.active) return MULLS_E_ARG;
-    ctx->pend.active = false;
-    cudaStream_t st = ctx->stream;
-    const int np = (int)ctx->n_pairs;
-    uint64_t launches = ctx->pend.launches;
-    const int n_search_ev = ctx->pend.n_search_ev;
-    const bool graphed = ctx->pend.graphed;
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
-    // (graph: three k_search forms, k_resolve, k_accumulate, k_solve per executed iteration + posterior, finalize, collect)
-    if (graphed) launches += (uint64_t)ctx->h_ctl->it * (6u + (ctx->any_normal_shooting ? 1u : 0u)) + 3u;
-    if (ctx->h_flags[1]) {
-        // the grid did not fit (k_hash_layout stopped every pair): grow the pool and run the call again on the inputs
-        // still in HBM. The grown pool holds the layout's last attempt by construction, so this happens at most once. A
-        // sharded run grows on every rank alike: the target clouds, and so their grids, are the same on all of them.
-        const int rc = grow_hash_pool(ctx);
-        if (rc != MULLS_OK) return rc;
-        return run_impl_inner(ctx, out, ctx->pend.trace, ctx->pend.hook, ctx->pend.user, true);
-    }
-    if (out) std::memcpy(out, ctx->h_results, np * sizeof(mulls_icp_result));
-    // statistics
-    mulls_run_stats &S = ctx->stats;
-    S = mulls_run_stats();
-    S.kernel_launches = launches;
-    cudaEventElapsedTime(&S.ms_ingest, ctx->ev_begin, ctx->ev_ingest);
-    cudaEventElapsedTime(&S.ms_iterate, ctx->ev_ingest, ctx->ev_iter);
-    cudaEventElapsedTime(&S.ms_total, ctx->ev_begin, ctx->ev_end);
-    if (ctx->h2d_timed) cudaEventElapsedTime(&S.ms_h2d, ctx->ev_h2d0, ctx->ev_begin);
-    S.ms_host_pack = ctx->up_ms_pack, S.ms_host_upload = ctx->up_ms_host;
-    ctx->h2d_timed = false;
-    float ms = 0.f;
-    for (int it = 0; it < n_search_ev; ++it) {
-        float t = 0.f;
-        cudaEventElapsedTime(&t, ctx->ev_search[2 * it], ctx->ev_search[2 * it + 1]);
-        S.ms_search_iter[it] = t;
-        ms += t;
-    }
-    S.ms_search = ms;
-    S.search_launches = (uint64_t)n_search_ev;
-    for (int p = 0; p < np; ++p) S.iterations += (uint64_t)ctx->h_results[p].iters;
-    // algorithmic bytes are accumulated on the device per executed iteration (k_collect puts them behind the results)
-    {
-        const uint64_t *ab = reinterpret_cast<const uint64_t *>(ctx->h_results + np);
-        for (int p = 0; p < np; ++p) S.algorithmic_bytes += ab[p];
-    }
-    ctx->grid_valid = !ctx->pend.hooked;
-    return MULLS_OK;
+static int run_finish(mulls_ctx *ctx, mulls_icp_result *out) {
+    return drain_on_error(ctx, [&]() -> int {
+        if (!ctx || !ctx->pend.active) return MULLS_E_ARG;
+        ctx->pend.active = false;
+        cudaStream_t st = ctx->stream;
+        const int np = (int)ctx->n_pairs;
+        uint64_t launches = ctx->pend.launches;
+        const int n_search_ev = ctx->pend.n_search_ev;
+        CK(cudaStreamSynchronize(st));
+        CK(cudaGetLastError());
+        if (ctx->pend.graphed) launches += (uint64_t)ctx->h_ctl->it * ctx->graph_body_launches + ctx->graph_tail_launches;
+        if (ctx->h_flags[1]) {
+            // the grid did not fit (k_hash_layout stopped every pair): grow the pool and run the call again on the inputs
+            // still in HBM. The grown pool holds the layout's last attempt by construction, so this happens at most once. A
+            // sharded run grows on every rank alike: the target clouds, and so their grids, are the same on all of them.
+            const int rc = grow_hash_pool(ctx);
+            if (rc != MULLS_OK) return rc;
+            return run_impl(ctx, out, ctx->pend.trace, ctx->pend.hook, ctx->pend.user);
+        }
+        if (out) std::memcpy(out, ctx->h_results, np * sizeof(mulls_icp_result));
+        // statistics
+        mulls_run_stats &S = ctx->stats;
+        S = mulls_run_stats();
+        S.kernel_launches = launches;
+        cudaEventElapsedTime(&S.ms_ingest, ctx->ev_begin, ctx->ev_ingest);
+        cudaEventElapsedTime(&S.ms_iterate, ctx->ev_ingest, ctx->ev_iter);
+        cudaEventElapsedTime(&S.ms_total, ctx->ev_begin, ctx->ev_end);
+        if (ctx->h2d_timed) cudaEventElapsedTime(&S.ms_h2d, ctx->ev_h2d0, ctx->ev_begin);
+        S.ms_host_pack = ctx->up_ms_pack, S.ms_host_upload = ctx->up_ms_host;
+        ctx->h2d_timed = false;
+        float ms = 0.f;
+        for (int it = 0; it < n_search_ev; ++it) {
+            float t = 0.f;
+            cudaEventElapsedTime(&t, ctx->ev_search[2 * it], ctx->ev_search[2 * it + 1]);
+            S.ms_search_iter[it] = t;
+            ms += t;
+        }
+        S.ms_search = ms;
+        S.search_launches = (uint64_t)n_search_ev;
+        for (int p = 0; p < np; ++p) S.iterations += (uint64_t)ctx->h_results[p].iters;
+        // algorithmic bytes are accumulated on the device per executed iteration (k_collect puts them behind the results)
+        {
+            const uint64_t *ab = reinterpret_cast<const uint64_t *>(ctx->h_results + np);
+            for (int p = 0; p < np; ++p) S.algorithmic_bytes += ab[p];
+        }
+        ctx->grid_valid = !ctx->pend.hooked;
+        return MULLS_OK;
+    }());
 }
 
 int mulls_batch_upload(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *tgt, const mulls_cloud_view *src,
