@@ -5,7 +5,7 @@
 //   k_resolve     I2b     duplicate check (:1755-1792), distance rejector (:1794-1796), normal check (:1798-1830),
 //                         per-class correspondence counts
 //   k_accumulate  I3-I5   order-preserving source compaction (:1776-1789), 21+6 normal-equation terms per
-//                         correspondence (:1976-2275), fixed-order block reduction -> one partial per chunk
+//                         correspondence (:1976-2275), fixed-order reduction -> one partial per chunk
 //   k_solve       I5-I9   per pair: partials summed in chunk order, 6x6 solve, Euler/Jacobian, convergence and
 //                         status logic (:1301-1400) — the iteration driver lives on the device
 // After the loop: k_posterior + k_finalize (:2518-2677, :1386). Source-sharded registrations (k_shard_*) insert the
@@ -460,7 +460,7 @@ __global__ void __launch_bounds__(kIterBlock, kResolveBlocksPerSm) k_resolve(Dev
 //   [0..20]  lower triangle of ATPA, column by column: (0,0)(1,0)..(5,0)(1,1)(2,1)..(5,5)
 //   [21..26] ATPb
 // ------------------------------------------------------------------------------------------------
-// `t`: anything indexable that takes the 27 terms (k_accumulate: a column of the block's shared-memory term matrix)
+// `t`: anything indexable that takes the 27 terms (a register array, or a column of a shared-memory term matrix)
 template <class Sink>
 __device__ __forceinline__ void terms_pt2pl(const float4 p, const float pi, const float4 q, const float4 qn,
                                             float weight, int iter_num, bool dist_w, bool resid_w, bool inten_w,
@@ -632,7 +632,7 @@ __device__ __forceinline__ void pair_left_running(DeviceArrays &A) {
     __threadfence_system();
 }
 
-// Solve + state update of one pair; executed by thread 0 of the last block of k_accumulate
+// Solve + state update of one pair; executed by thread 0 of the pair's k_solve block
 // (cregistration.hpp:1301-1400 after the summations). S = per-class sums [6][kTerms] in shared memory.
 __device__ __noinline__ void solve_and_advance(DeviceArrays &A, uint32_t pair, const double *S, double *sm /*>= 150 doubles*/,
                                   int buf_written) {
@@ -761,7 +761,141 @@ __device__ __noinline__ void solve_and_advance(DeviceArrays &A, uint32_t pair, c
 }
 
 // ---- k_accumulate ------------------------------------------------------------------------------
-__device__ __forceinline__ void accumulate_body(DeviceArrays &A, int buf, uint32_t chunk) {
+// One source of a chunk: (2) a kept source is compacted into the other buffer (order preserved: :1776-1789), moved; a
+// source that is not kept is never read again. (3) `emit(t)` takes the 27 terms of a surviving correspondence (pass
+// implies kept), zeros otherwise; it is called in each branch that computes terms, so that they need not all be live
+// after the branches. `gd` is the kept source's destination.
+template <class Emit>
+__device__ __forceinline__ void accumulate_source(DeviceArrays &A, const PairConst &pc, const PairState &ps, int c,
+                                                  int buf, int it, uint32_t gi, uint32_t gd, uint32_t fl, bool few,
+                                                  const uint32_t *n_corr, Emit emit) {
+    const bool kept = (fl & 1) != 0, pass = (fl & 2) != 0;
+    float4 p = make_float4(0, 0, 0, 0);
+    int j = -1;
+    float d2 = 0.0f;
+    if (kept) {
+        p = advanced_pos(ps, A.src_pos[buf][gi]);
+        j = A.nn_idx[gi];
+        d2 = A.nn_d2[gi];
+        // reset the claim table for the next iteration: where k_resolve checked duplicates, a claimed target was claimed
+        // by its winner, the one matched source that is kept; elsewhere every matched source is kept and resets its own.
+        // (Sharded runs clear the whole table before each search: a winner may belong to another rank.)
+        if (j >= 0) A.claim[pc.tgt_base[c] + j] = kClaimFree;
+        A.src_pos[buf ^ 1][gd] = p;
+        A.src_nrm[buf ^ 1][gd] = advanced_nrm(ps, A.src_nrm[buf][gi]);
+        A.src_prevj[buf ^ 1][gd] = j;
+        // certificates exist from the iteration before the first keep test on (k_search<1>)
+        if (it >= kKeepFromIter - 1) A.src_cert[buf ^ 1][gd] = A.src_cert[buf][gi];
+    }
+    float w_store = 0.0f;
+    double t[27];
+    if (pass && !few) {
+        const float4 q = A.tgt_pos[pc.tgt_base[c] + j];
+        const float4 qn = A.tgt_nrm[pc.tgt_base[c] + j];
+        const bool resid_w = pc.w_residual && it > 2; // :1905-1907
+        const bool dist_w = pc.w_dist != 0, inten_w = pc.w_intensity != 0;
+        if (c == MULLS_GROUND || c == MULLS_FACADE || c == MULLS_ROOF) {
+            const float wc = (c == MULLS_FACADE) ? 1.0f : balanced_ground_weight(pc, n_corr);
+            terms_pt2pl(p, p.w, q, qn, wc, it, dist_w, resid_w, inten_w, pc.win_pt2pl, t, w_store);
+            emit(t);
+        } else if (c == MULLS_PILLAR || c == MULLS_BEAM) {
+            terms_pt2li(p, p.w, q, qn, 1.0f, it, dist_w, resid_w, inten_w, pc.win_pt2li, t, w_store);
+            emit(t);
+        } else {
+            terms_pt2pt(p, p.w, q, 1.0f, it, dist_w, resid_w, inten_w, pc.win_pt2pt, t);
+            w_store = d2; // pt2pt never stores a weight: the posterior reads the squared NN distance (Q2)
+            emit(t);
+        }
+    } else {
+        constexpr double kZeros[27] = {};
+        emit(kZeros);
+    }
+    if (kept) {
+        A.corr_j[gd] = pass ? j : -1;
+        A.corr_w[gd] = w_store;
+    }
+}
+
+// Both reductions of a chunk's terms add in the same fixed order, so the partial is bit-reproducible and independent of
+// who takes the chunk when: term k of thread (or lane slot) l is row[l] = the chunk's source l, and the partial is
+// ((row[l] + row[l + 32]) + row[l + 64]) + row[l + 96] on lane l, then a butterfly over xor 16, 8, 4, 2, 1.
+//
+// k_accumulate: one WARP per chunk, fetched from the live list as k_search's direct mode fetches its quarters. Lane l
+// takes sources l, l + 32, l + 64, l + 96 in that order and sums their terms in registers: no shared memory, no block
+// barrier. Throughput over many chunks is what counts here.
+constexpr int kAccumulateBlocksPerSm = 4; // 128 registers (54 of them the sums) and no spill
+__device__ __forceinline__ void accumulate_chunk_warp(DeviceArrays &A, int buf, uint32_t chunk) {
+    const ChunkDesc cd = A.it_chunks[chunk];
+    const PairConst &pc = A.pc[cd.pair];
+    PairState &ps = A.ps[cd.pair];
+    if (ps.status != kRunning) return;
+    const int c = (int)cd.seg;
+    const int ns = ps.n_src[c];
+    // chunks entirely past the live part of the class have nothing to contribute (k_solve skips them)
+    if ((int)cd.first >= ns) return;
+    const int lane = threadIdx.x & 31;
+    constexpr int kSlots = kIterBlock / 32;
+    const uint32_t first = pc.src_base[c] + cd.first;
+    uint32_t fl = 0; // the flags of the lane's four sources, a byte each
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s)
+        if ((int)cd.first + 32 * s + lane < ns) fl |= (uint32_t)A.flags[first + 32 * s + lane] << (8 * s);
+    // (1) destination of the kept sources: after those of the chunks before this one in the same (pair, class)
+    uint32_t dst = 0;
+#pragma unroll 4
+    for (uint32_t b = pc.class_chunk_begin[c] + lane; b < chunk; b += 32) dst += A.blk_kept[b];
+    for (int o = 16; o > 0; o >>= 1) dst += __shfl_xor_sync(0xffffffffu, dst, o);
+    uint32_t n_corr[kNumClasses]; // complete since every k_resolve block of the pair has finished
+#pragma unroll
+    for (int k = 0; k < kNumClasses; ++k) n_corr[k] = ps.n_corr[k];
+    float ratio_unused;
+    const bool few = too_few(pc, ps, n_corr, ratio_unused);
+    const int it = ps.iter;
+    // the lane's sums start at -0.0, the identity of IEEE addition (-0.0 + x == x for every x, -0.0 included): the
+    // first source's terms are taken as they are
+    double acc[27];
+#pragma unroll
+    for (int k = 0; k < 27; ++k) acc[k] = -0.0;
+#pragma unroll 1
+    for (int s = 0; s < kSlots; ++s, fl >>= 8) {
+        const unsigned kb = __ballot_sync(0xffffffffu, (fl & 1) != 0);
+        const uint32_t gd = pc.src_base[c] + dst + __popc(kb & ((1u << lane) - 1u));
+        dst += __popc(kb);
+        accumulate_source(A, pc, ps, c, buf, it, first + 32 * s + lane, gd, fl, few, n_corr, [&acc](const double *t) {
+#pragma unroll
+            for (int k = 0; k < 27; ++k) acc[k] += t[k];
+        });
+    }
+    // (4) the butterfly (every lane ends with the same total); lane k stores term k
+    double mine = 0.0;
+#pragma unroll
+    for (int k = 0; k < 27; ++k) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == k) mine = v;
+    }
+    if (lane < 27) A.partials[(size_t)chunk * kTerms + lane] = mine;
+}
+__global__ void __launch_bounds__(kIterBlock, kAccumulateBlocksPerSm) k_accumulate(DeviceArrays A, int buf) {
+    buf = loop_buf(A, buf);
+    LoopCtl &ctl = *A.ctl;
+    if (blockIdx.x == 0 && threadIdx.x == 0) ctl.work[0] = 0u; // the next iteration's k_search starts its list at 0
+    const uint32_t n = ctl.n_live[buf];
+    const uint32_t *list = A.live_chunks + (size_t)buf * A.live_stride;
+    for (;;) { // fetched per warp: no barrier, a warp that finishes early moves on
+        uint32_t w = 0;
+        if ((threadIdx.x & 31) == 0) w = atomicAdd(&ctl.work[2], 1u);
+        w = __shfl_sync(0xffffffffu, w, 0);
+        if (w >= n) break;
+        accumulate_chunk_warp(A, buf, list[w]);
+    }
+}
+
+// k_icp_loop's phase 3: one BLOCK per chunk, a thread per source, the terms in a 27 x 128 shared-memory matrix that
+// warp w sums rows w, w + 4, ... of. The cooperative kernel runs batches of a few chunks, where a chunk's latency
+// counts: its 128 sources are handled at once, not four after another.
+__device__ __forceinline__ void accumulate_chunk_block(DeviceArrays &A, int buf, uint32_t chunk) {
     const ChunkDesc cd = A.it_chunks[chunk];
     const PairConst &pc = A.pc[cd.pair];
     PairState &ps = A.ps[cd.pair];
@@ -772,21 +906,14 @@ __device__ __forceinline__ void accumulate_body(DeviceArrays &A, int buf, uint32
     const bool valid = (int)local < ns;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     constexpr int kWarps = kIterBlock / 32;
-    // the block's term matrix: 27 rows of 128 doubles, one column per thread (27 KB: 8 blocks per SM)
     __shared__ double s_terms[27 * kIterBlock];
     __shared__ uint32_t s_off[kWarps + 1];
     __shared__ uint32_t s_base;
 
     // blocks entirely past the live part of the class have nothing to contribute (k_solve skips them)
     if ((int)cd.first >= ns) return;
-    uint32_t dst_local = 0;
     uint8_t fl = 0;
     uint32_t gi = 0;
-    bool kept = false, pass = false;
-    struct Column { // row k of this thread's column
-        double *base;
-        __device__ __forceinline__ double &operator[](int k) const { return base[k * kIterBlock]; }
-    } t = {s_terms + threadIdx.x};
     // (1) destination of the kept sources: blocks before this one in the same (pair, class)
     {
         uint32_t acc = 0;
@@ -806,8 +933,7 @@ __device__ __forceinline__ void accumulate_body(DeviceArrays &A, int buf, uint32
         gi = pc.src_base[c] + local;
         fl = A.flags[gi];
     }
-    kept = (fl & 1) != 0, pass = (fl & 2) != 0;
-    const unsigned kb = __ballot_sync(0xffffffffu, kept);
+    const unsigned kb = __ballot_sync(0xffffffffu, (fl & 1) != 0);
     if (lane == 0) s_off[warp] = __popc(kb);
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -820,61 +946,17 @@ __device__ __forceinline__ void accumulate_body(DeviceArrays &A, int buf, uint32
         s_off[kWarps] = run;
     }
     __syncthreads();
-    dst_local = s_base + s_off[warp] + __popc(kb & ((1u << lane) - 1u));
-
-    // (2) compaction into the other buffer (order preserved: :1776-1789), of the moved source: a source that is not kept
-    // is never read again
-    float4 p = make_float4(0, 0, 0, 0);
-    int j = -1;
-    float d2 = 0.0f;
-    const uint32_t gd = pc.src_base[c] + dst_local;
-    if (kept) {
-        p = advanced_pos(ps, A.src_pos[buf][gi]);
-        j = A.nn_idx[gi];
-        d2 = A.nn_d2[gi];
-        // reset the claim table for the next iteration: where k_resolve checked duplicates, a claimed target was claimed
-        // by its winner, the one matched source that is kept; elsewhere every matched source is kept and resets its own.
-        // (Sharded runs clear the whole table before each search: a winner may belong to another rank.)
-        if (j >= 0) A.claim[pc.tgt_base[c] + j] = kClaimFree;
-        A.src_pos[buf ^ 1][gd] = p;
-        A.src_nrm[buf ^ 1][gd] = advanced_nrm(ps, A.src_nrm[buf][gi]);
-        A.src_prevj[buf ^ 1][gd] = j;
-        // certificates exist from the iteration before the first keep test on (k_search<1>)
-        if (ps.iter >= kKeepFromIter - 1) A.src_cert[buf ^ 1][gd] = A.src_cert[buf][gi];
-    }
-    // (3) terms of the surviving correspondences (pass implies kept)
-    float w_store = 0.0f;
+    const uint32_t gd = pc.src_base[c] + s_base + s_off[warp] + __popc(kb & ((1u << lane) - 1u));
     uint32_t n_corr[kNumClasses]; // complete since every k_resolve block of the pair has finished
 #pragma unroll
     for (int k = 0; k < kNumClasses; ++k) n_corr[k] = ps.n_corr[k];
     float ratio_unused;
     const bool few = too_few(pc, ps, n_corr, ratio_unused);
-    if (pass && !few) {
-        const float4 q = A.tgt_pos[pc.tgt_base[c] + j];
-        const float4 qn = A.tgt_nrm[pc.tgt_base[c] + j];
-        const int it = ps.iter;
-        const bool resid_w = pc.w_residual && it > 2; // :1905-1907
-        const bool dist_w = pc.w_dist != 0, inten_w = pc.w_intensity != 0;
-        if (c == MULLS_GROUND || c == MULLS_FACADE || c == MULLS_ROOF) {
-            const float wc = (c == MULLS_FACADE) ? 1.0f : balanced_ground_weight(pc, n_corr);
-            terms_pt2pl(p, p.w, q, qn, wc, it, dist_w, resid_w, inten_w, pc.win_pt2pl, t, w_store);
-        } else if (c == MULLS_PILLAR || c == MULLS_BEAM) {
-            terms_pt2li(p, p.w, q, qn, 1.0f, it, dist_w, resid_w, inten_w, pc.win_pt2li, t, w_store);
-        } else {
-            terms_pt2pt(p, p.w, q, 1.0f, it, dist_w, resid_w, inten_w, pc.win_pt2pt, t);
-            w_store = d2; // pt2pt never stores a weight: the posterior reads the squared NN distance (Q2)
-        }
-    } else {
+    accumulate_source(A, pc, ps, c, buf, ps.iter, gi, gd, fl, few, n_corr, [](const double *t) {
 #pragma unroll
-        for (int k = 0; k < 27; ++k) t[k] = 0.0;
-    }
-    if (kept) {
-        A.corr_j[gd] = pass ? j : -1;
-        A.corr_w[gd] = w_store;
-    }
-    // (4) block reduction in a fixed order: warp w sums rows w, w + 4, ... of the term matrix — four columns per lane,
-    // then a butterfly over the lanes (every lane ends with the same total): bit-reproducible, independent of the
-    // order in which blocks fetch chunks
+        for (int k = 0; k < 27; ++k) s_terms[k * kIterBlock + threadIdx.x] = t[k]; // this thread's column
+    });
+    // (4) warp w sums rows w, w + 4, ... of the term matrix
     __syncthreads();
 #pragma unroll 1
     for (int k = warp; k < 27; k += kWarps) {
@@ -884,11 +966,6 @@ __device__ __forceinline__ void accumulate_body(DeviceArrays &A, int buf, uint32
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
         if (lane == 0) A.partials[(size_t)chunk * kTerms + k] = v;
     }
-}
-__global__ void __launch_bounds__(kIterBlock, 8) k_accumulate(DeviceArrays A, int buf) {
-    buf = loop_buf(A, buf);
-    if (blockIdx.x == 0 && threadIdx.x == 0) A.ctl->work[0] = 0u; // the next iteration's k_search starts its list at 0
-    for_each_live_chunk(A, buf, 2, [&](uint32_t chunk) { accumulate_body(A, buf, chunk); });
 }
 
 // the chunks of this pair that still own live sources go onto the next iteration's list (whole block; the pair's state
@@ -1040,7 +1117,7 @@ __global__ void __launch_bounds__(kIterBlock, 4) k_icp_loop(DeviceArrays A) {
         grid.sync();
         // phase 3: compaction + normal-equation partials
         for (uint32_t w = blockIdx.x; w < n_live; w += gridDim.x) {
-            accumulate_body(A, buf, list[w]);
+            accumulate_chunk_block(A, buf, list[w]);
             __syncthreads();
         }
         grid.sync();

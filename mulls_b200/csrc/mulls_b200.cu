@@ -857,10 +857,10 @@ static unsigned chunk_bucket(const mulls_ctx *ctx) {
     while (b < (unsigned)ctx->h_it_chunks.size()) b <<= 1;
     return b;
 }
-static unsigned resident_grid(const mulls_ctx *ctx, int blocks_per_sm) {
-    return std::min((unsigned)(ctx->num_sms * blocks_per_sm), chunk_bucket(ctx));
+static unsigned resident_grid(const mulls_ctx *ctx, int blocks_per_sm, unsigned chunks_per_block = 1) {
+    return std::min((unsigned)(ctx->num_sms * blocks_per_sm), (chunk_bucket(ctx) + chunks_per_block - 1) / chunks_per_block);
 }
-constexpr int kShootBlocksPerSm = 8, kAccumulateBlocksPerSm = 8;
+constexpr int kShootBlocksPerSm = 8;
 constexpr int kPollPause = 64; // _mm_pause() count between two cudaEventQuery calls of the launch loop's flow control
 
 // One ICP iteration: k_search [, k_search_shoot], k_resolve, k_accumulate, k_solve, and a sharded run's three exchanges.
@@ -897,7 +897,7 @@ static int enqueue_iteration(mulls_ctx *ctx, int it, mulls_allreduce_fn hook, vo
         k_shard_counts<<<1, kIterBlock, 0, st>>>(A, 1);
         launches += 2;
     }
-    k_accumulate<<<resident_grid(ctx, kAccumulateBlocksPerSm), kIterBlock, 0, st>>>(A, buf);
+    k_accumulate<<<resident_grid(ctx, kAccumulateBlocksPerSm, kIterBlock / 32), kIterBlock, 0, st>>>(A, buf); // a chunk per warp
     k_solve<<<recording ? (unsigned)std::max<size_t>(ctx->max_pairs, 1) : (unsigned)ctx->n_pairs, kSolveThreads, 0, st>>>(A, buf, handle);
     launches += 3;
     if (hook) { // exchange 3: per-class normal-equation sums; then every rank solves the same system
