@@ -278,6 +278,36 @@ int coarse_reg_ransac(const typename pcl::PointCloud<PointT>::Ptr &target_pts, c
     return status;
 }
 
+// lo::CRegistration<PointT>::omp_ndt (cregistration.hpp:945-1021) with use_direct_search (DIRECT7), same arguments and
+// defaults (test/mulls_slam.cpp:634-636, :671-673): target = block1->pc_down, source = block2->pc_down, their
+// local_bounds, on the device (mulls_omp_ndt, readings in abi.h). Returns 1, or -3 when the fitness exceeds
+// fitness_score_thre, and writes Trans1_2, as the reference does. A library error is logged and returns -3 with Trans1_2
+// left as it was.
+template <typename PointT>
+int omp_ndt(constraint_t &registration_cons, float ndt_resolution = 1.0, Eigen::Matrix4d initial_guess = Eigen::Matrix4d::Identity(),
+            bool apply_intersection_filter = true, float fitness_score_thre = 10.0) {
+    const typename pcl::PointCloud<PointT>::Ptr &t = registration_cons.block1->pc_down, &s = registration_cons.block2->pc_down;
+    double guess[16], tb[6], sb[6];
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) guess[4 * r + c] = initial_guess(r, c);
+    const bounds_t &b1 = registration_cons.block1->local_bound, &b2 = registration_cons.block2->local_bound;
+    const double tb_[6] = {b1.min_x, b1.min_y, b1.min_z, b1.max_x, b1.max_y, b1.max_z};
+    const double sb_[6] = {b2.min_x, b2.min_y, b2.min_z, b2.max_x, b2.max_y, b2.max_z};
+    std::memcpy(tb, tb_, sizeof(tb));
+    std::memcpy(sb, sb_, sizeof(sb));
+    mulls_ndt_result res;
+    mulls_ctx *ctx = thread_context(s->points.size(), t->points.size());
+    if (!ctx || mulls_omp_ndt(ctx, view_of<PointT>(t), view_of<PointT>(s), ndt_resolution, 1, guess, apply_intersection_filter ? 1 : 0,
+                              fitness_score_thre, tb, sb, &res, nullptr, 0) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return -3;
+    }
+    LOG(INFO) << "fitness score: " << res.fitness; // base_align, :779
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) registration_cons.Trans1_2(r, c) = res.trans[4 * r + c];
+    return res.code;
+}
+
 } // namespace b200
 } // namespace lo
 #endif

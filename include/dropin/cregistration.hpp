@@ -14,7 +14,7 @@
 //     (:1584-1592), find_feature_correspondence_ncc (:409-411) and coarse_reg_ransac (:605-607) run on the GPU through
 //     the C-ABI (include/mulls_b200/abi.h). All other public members the callers use
 //     — determine_source_target_cloud, assign_source_target_cloud, coarse_reg_teaser,
-//     omp_ndt, omp_gicp, ... (SURVEY.md section 8b) — are inherited from the reference; every overload of
+//     omp_gicp, ... (SURVEY.md section 8b) — are inherited from the reference; every overload of
 //     coarse_reg_ransac the reference class declares stays visible next to the device one.
 // Differences in contract are listed in INTEGRATION.md (block1->tree_* are not populated: use mulls_nn_query or
 // the drop-in lo::MapManager of dropin/map_manager.h, which does not need them).
@@ -82,6 +82,17 @@ class CRegistration : public CRegistration_reference<PointT> {
     int coarse_reg_ransac(const typename pcl::PointCloud<PointT>::Ptr &target_pts, const typename pcl::PointCloud<PointT>::Ptr &source_pts,
                           Eigen::Matrix4d &tran_mat, float noise_bound = 0.2, int min_inlier_num = 8, int max_iter_num = 20000) {
         return b200::coarse_reg_ransac<PointT>(target_pts, source_pts, tran_mat, noise_bound, min_inlier_num, max_iter_num);
+    }
+    // cregistration.hpp:945-947. The device runs the DIRECT7 neighbourhood; KDTREE (use_direct_search = false) is the
+    // reference member. A template on the guess type, so that the class compiles against a reference build that does
+    // not declare omp_ndt as long as nobody calls the KDTREE form.
+    template <typename Matrix4 = Eigen::Matrix4d>
+    int omp_ndt(constraint_t &registration_cons, float ndt_resolution = 1.0, bool use_direct_search = true,
+                Matrix4 initial_guess = Matrix4::Identity(), bool apply_intersection_filter = true, float fitness_score_thre = 10.0) {
+        if (!use_direct_search)
+            return CRegistration_reference<PointT>::omp_ndt(registration_cons, ndt_resolution, use_direct_search, initial_guess,
+                                                            apply_intersection_filter, fitness_score_thre);
+        return b200::omp_ndt<PointT>(registration_cons, ndt_resolution, initial_guess, apply_intersection_filter, fitness_score_thre);
     }
 };
 

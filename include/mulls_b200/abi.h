@@ -39,6 +39,7 @@
  *   mulls_ncc_correspondences <- lo::CRegistration<PointT>::find_feature_correspondence_ncc, cregistration.hpp:409-601
  *   mulls_coarse_reg_ransac  <- lo::CRegistration<PointT>::coarse_reg_ransac, cregistration.hpp:604-661
  *   mulls_non_max_suppress   <- lo::CFilter<PointT>::non_max_suppress(cloud_in_out, non_max_radius), cfilter.hpp:1183-1240
+ *   mulls_omp_ndt            <- lo::CRegistration<PointT>::omp_ndt with use_direct_search (DIRECT7), cregistration.hpp:945-1021
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
  *
@@ -595,6 +596,53 @@ int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_c
  * MULLS_E_ARG. */
 int mulls_non_max_suppress(mulls_ctx *ctx, mulls_cloud_view cloud, float non_max_radius, int32_t *kept_idx /* [cloud.n] */,
                            size_t *n_kept, int *performed);
+
+/* NDT registration: lo::CRegistration<PointT>::omp_ndt(reg_con, ndt_resolution, use_direct_search, initial_guess,
+ * apply_intersection_filter, fitness_score_thre) (cregistration.hpp:945-1021), i.e. koide_reg::NormalDistributionsTransform
+ * (include/baseline_reg/ndt_omp_impl.hpp) over koide_reg::VoxelGridCovariance with the DIRECT7 neighbourhood.
+ * target = block1->pc_down, source = block2->pc_down, target_bound / source_bound = block1 / block2 ->local_bound
+ * (min_x min_y min_z max_x max_y max_z). The readings of the reference are listed in mulls_b200/csrc/ndt_core.cuh
+ * (N1-N6, C1-C2); in short:
+ *   - prologue: a non-identity initial guess (isIdentity(1e-6)) moves the source in double with a float store and the
+ *     intersection box is target_bound with the moved source's bbox, else the two bounds; padded by 2.0; with
+ *     apply_intersection_filter both clouds keep the points strictly inside it;
+ *   - target leaves of edge ndt_resolution: sums in input order in double, covariance finalised, eigenvalues checked and
+ *     inflated to 0.01 of the largest, inverse cast to float; a leaf needs 6 points to be a neighbour; more than
+ *     INT32_MAX cells: no leaves;
+ *   - the Newton walk with the constants omp_ndt leaves at their defaults (step_size 0.1, transformation_epsilon 0.1,
+ *     max_iterations 35, outlier_ratio 0.55): every step is clamp(|newton step|, 0.05, 0.1) along the normalised
+ *     direction, so even a converged run may end up to 0.05 (mixed m / rad) past the Newton point;
+ *   - fitness = getFitnessScore(): the mean squared distance of the moved (filtered) source to its nearest target,
+ *     DBL_MAX when no point counts (empty source or target); code -3 when fitness > fitness_score_thre, else 1;
+ *   - Trans1_2 = (double)final_transformation * initial_guess when the guess moved the source, else the former;
+ *   - an empty target (for instance after the intersection filter) has no leaves: no point finds a neighbour, the
+ *     gradient is zero and the walk ends at once with the identity (the reference is undefined there);
+ *   - points with a non-finite coordinate take part in nothing.
+ * The walk runs on the host: one evaluation (a few kernels and one 344-byte download) per iteration. The call replaces
+ * the resident batch (the fitness search uses the ingest's grid). iterations = nr_iterations_ (at most 37), converged
+ * = converged_. trace (may be NULL with trace_cap 0) receives up to trace_cap iterations: the pose vector after the step,
+ * the step length, the score at it and whether the direction was reversed. use_direct_search = 0 (KDTREE): MULLS_E_UNSUPPORTED (the drop-in calls the
+ * reference member). A NULL output or matrix, NULL rows with n > 0, or ndt_resolution <= 0: MULLS_E_ARG. A target above
+ * max_tgt_pts or a source above max_src_pts: MULLS_E_CAPACITY. */
+typedef struct mulls_ndt_result {
+    double trans[16];  /* Trans1_2, row-major */
+    int code;          /* 1, or -3 when fitness > fitness_score_thre */
+    int iterations;
+    int converged;
+    int n_target;      /* points after the intersection filter (finite) */
+    int n_source;      /* points after the intersection filter */
+    double fitness;
+} mulls_ndt_result;
+typedef struct mulls_ndt_iter {
+    double p[6];  /* x y z roll pitch yaw after the step */
+    double step;  /* step length: 0, or in [0.05, 0.1] */
+    double score; /* the score at p */
+    int reversed; /* 1: the Newton direction pointed downhill and was turned around */
+} mulls_ndt_iter;
+int mulls_omp_ndt(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view source, float ndt_resolution, int use_direct_search,
+                  const double initial_guess[16] /* row-major */, int apply_intersection_filter, float fitness_score_thre,
+                  const double target_bound[6], const double source_bound[6], mulls_ndt_result *out, mulls_ndt_iter *trace,
+                  int trace_cap);
 
 /* The wire format the library ships host clouds in when the "host_pack" tunable is on (csrc/host_pack.h): the 28 of the
  * 48 bytes of a pcl::PointXYZINormal row (utility.hpp:40) that the path reads, repacked on the host cores into pinned

@@ -104,6 +104,25 @@ class PcaOut(C.Structure):
     ]
 
 
+class NdtResult(C.Structure):
+    """mulls_ndt_result: Trans1_2, the code omp_ndt returns, the walk's iteration count and convergence, the fitness score
+    and the point counts after the intersection filter."""
+    _fields_ = [
+        ("trans", C.c_double * 16),
+        ("code", C.c_int),
+        ("iterations", C.c_int),
+        ("converged", C.c_int),
+        ("n_target", C.c_int),
+        ("n_source", C.c_int),
+        ("fitness", C.c_double),
+    ]
+
+
+class NdtIter(C.Structure):
+    """mulls_ndt_iter: one Newton iteration of the NDT walk (pose vector after the step, step length, score, reversal)."""
+    _fields_ = [("p", C.c_double * 6), ("step", C.c_double), ("score", C.c_double), ("reversed", C.c_int)]
+
+
 class SorStats(C.Structure):
     """mulls_sor_stats: what pcl::StatisticalOutlierRemoval computed (mean, stddev, threshold) and the point counts."""
     _fields_ = [
@@ -290,6 +309,7 @@ EXPORTED_SYMBOLS = (
     "mulls_ncc_correspondences",
     "mulls_coarse_reg_ransac",
     "mulls_non_max_suppress",
+    "mulls_omp_ndt",
     "mulls_scan_probe",
     "mulls_scan_read",
     "mulls_pose_write",
@@ -376,6 +396,9 @@ def load_library() -> C.CDLL:
     lib.mulls_non_max_suppress.restype = C.c_int
     lib.mulls_non_max_suppress.argtypes = [vp, CloudView, C.c_float, C.POINTER(C.c_int32), C.POINTER(C.c_size_t),
                                            C.POINTER(C.c_int)]
+    lib.mulls_omp_ndt.restype = C.c_int
+    lib.mulls_omp_ndt.argtypes = [vp, CloudView, CloudView, C.c_float, C.c_int, C.POINTER(C.c_double), C.c_int, C.c_float,
+                                  C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(NdtResult), C.POINTER(NdtIter), C.c_int]
     lib.mulls_pack_rows.restype = C.c_int
     lib.mulls_pack_rows.argtypes = [C.POINTER(C.c_float), C.c_size_t, C.c_int, C.POINTER(C.c_float)]
     lib.mulls_scan_probe.restype = C.c_int

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_run_length_encode.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
@@ -30,6 +31,7 @@
 #include "kernels_rawscan.cuh"
 #include "kernels_ncc.cuh"
 #include "kernels_ransac.cuh"
+#include "kernels_ndt.cuh"
 
 using namespace mulls;
 
@@ -160,6 +162,7 @@ struct mulls_ctx {
     Scratch ncc_buf;             // NCC keypoint matching: rows, descriptors, row / column minima or select state, sort
     Scratch rc_buf;              // RANSAC coarse registration: correspondences, hypotheses, counts, refinement state
     Scratch nms_buf;             // keypoint NMS: rows, sorted rows, keys, sort scratch, cell hash, kept indices
+    Scratch ndt_buf;             // NDT: clouds, leaf keys and sort scratch, leaves, tile sums, fitness distances
     void *rc_host = nullptr;     // pinned: two chunks of sample triples and their counts
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
@@ -1940,6 +1943,142 @@ int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_c
     return front_call(ctx, [&](uint64_t &launches) {
         return ransac_impl(ctx, target_pts, source_pts, noise_bound, min_inlier_num, max_iter_num, tran_mat, status, n_inliers,
                            n_hypotheses, launches);
+    });
+}
+
+// ================================================================================================
+// NDT registration (CRegistration::omp_ndt, cregistration.hpp:945-1021, DIRECT7): ndt_core.cuh, kernels_ndt.cuh
+// ================================================================================================
+static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, float resolution, int use_direct_search,
+                    const double *guess, int apply_filter, float fitness_thre, const double *tbound, const double *sbound,
+                    mulls_ndt_result *out, mulls_ndt_iter *trace, int trace_cap, uint64_t &launches) {
+    if (!out || !guess || !tbound || !sbound || (tv.n && !tv.aos48) || (sv.n && !sv.aos48) || !(resolution > 0.f) ||
+        (trace_cap > 0 && !trace))
+        return MULLS_E_ARG;
+    const char *fn = "mulls_omp_ndt";
+    if (!use_direct_search) {
+        ctx->err = std::string(fn) + ": only the DIRECT7 neighbour search runs on the device";
+        return MULLS_E_UNSUPPORTED;
+    }
+    int rc;
+    if ((rc = check_capacity(ctx, tv.n, fn)) != MULLS_OK) return rc;
+    if (sv.n > ctx->max_src) {
+        ctx->err = std::string(fn) + ": " + std::to_string(sv.n) + " source points exceed max_src_pts of the context";
+        return MULLS_E_CAPACITY;
+    }
+    std::vector<float4> tgt, src;
+    bool moved = false;
+    ndt_prologue(tv.aos48, tv.n, sv.aos48, sv.n, guess, apply_filter, tbound, sbound, tgt, src, moved);
+    const NdtGrid g = ndt_grid_from(tgt, resolution);
+    const int nt = (int)tgt.size(), ns = (int)src.size(), tiles = (int)ceil_div((size_t)ns, kNdtTile);
+    cudaStream_t st = ctx->stream;
+    size_t cub_sort = 0, cub_rle = 0, cub_scan = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_sort, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint32_t *)nullptr,
+                                       (uint32_t *)nullptr, std::max(nt, 1)));
+    CK(cub::DeviceRunLengthEncode::Encode(nullptr, cub_rle, (uint64_t *)nullptr, (uint64_t *)nullptr, (int *)nullptr,
+                                          (int *)nullptr, std::max(nt, 1)));
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_scan, (int *)nullptr, (int *)nullptr, std::max(nt, 1)));
+    const size_t cub_bytes = std::max(cub_sort, std::max(cub_rle, cub_scan));
+    ScratchLayout L;
+    const size_t o_t = L.take(nt * sizeof(float4)), o_s = L.take(ns * sizeof(float4)), o_ka = L.take(nt * 8ull),
+                 o_kb = L.take(nt * 8ull), o_va = L.take(nt * 4ull), o_vb = L.take(nt * 4ull), o_uk = L.take(nt * 8ull),
+                 o_cnt = L.take(nt * 4ull), o_off = L.take(nt * 4ull), o_nr = L.take(sizeof(int)),
+                 o_lv = L.take(nt * sizeof(NdtLeaf)), o_ts = L.take((size_t)tiles * kNdtTerms * 8),
+                 o_out = L.take(kNdtTerms * 8), o_d2 = L.take(ns * sizeof(float)), o_cub = L.take(cub_bytes);
+    char *base;
+    if ((rc = L.grow(ctx, ctx->ndt_buf, base)) != MULLS_OK) return rc;
+    float4 *d_t = (float4 *)(base + o_t), *d_s = (float4 *)(base + o_s);
+    uint64_t *d_ka = (uint64_t *)(base + o_ka), *d_kb = (uint64_t *)(base + o_kb), *d_uk = (uint64_t *)(base + o_uk);
+    uint32_t *d_va = (uint32_t *)(base + o_va), *d_vb = (uint32_t *)(base + o_vb);
+    int *d_cnt = (int *)(base + o_cnt), *d_off = (int *)(base + o_off), *d_nr = (int *)(base + o_nr);
+    NdtLeaf *d_lv = (NdtLeaf *)(base + o_lv);
+    double *d_ts = (double *)(base + o_ts), *d_out = (double *)(base + o_out);
+    float *d_d2 = (float *)(base + o_d2);
+    void *d_cub = base + o_cub;
+    if (nt) CK(cudaMemcpyAsync(d_t, tgt.data(), nt * sizeof(float4), cudaMemcpyHostToDevice, st));
+    if (ns) CK(cudaMemcpyAsync(d_s, src.data(), ns * sizeof(float4), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(d_nr, 0, sizeof(int), st));
+    if (g.ok) { // the leaves (N1)
+        size_t b = cub_bytes;
+        k_ndt_keys<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, nt, g, d_ka, d_va);
+        CK(cub::DeviceRadixSort::SortPairs(d_cub, b, d_ka, d_kb, d_va, d_vb, nt, 0, 64, st));
+        CK(cudaMemsetAsync(d_cnt, 0, nt * 4ull, st));
+        b = cub_bytes;
+        CK(cub::DeviceRunLengthEncode::Encode(d_cub, b, d_kb, d_uk, d_cnt, d_nr, nt, st));
+        b = cub_bytes;
+        CK(cub::DeviceScan::ExclusiveSum(d_cub, b, d_cnt, d_off, nt, st));
+        k_ndt_leaves<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, d_vb, d_off, d_cnt, d_nr, d_lv);
+        launches += 2;
+    }
+    NdtEvalConst E;
+    {
+        double d1, d2;
+        ndt_gauss(resolution, d1, d2);
+        E.gauss_d1 = d1, E.gauss_d2 = (float)d2;
+    }
+    NdtEvalArgs EA{d_s, ns, g, d_uk, d_lv, d_nr, d_ts};
+    int err = MULLS_OK;
+    auto eval = [&](const double p[6], const float T[12], double r[kNdtTerms]) {
+        for (int c = 0; c < kNdtTerms; ++c) r[c] = 0.0;
+        if (err != MULLS_OK || ns == 0) return;
+        std::memcpy(E.T, T, sizeof(E.T));
+        ndt_angle_tables(p, E);
+        k_ndt_eval<<<(unsigned)tiles, kNdtTile, 0, st>>>(EA, E);
+        k_ndt_tiles<<<1, 64, 0, st>>>(d_ts, tiles, d_out);
+        launches += 2;
+        cudaError_t e = cudaMemcpyAsync(r, d_out, kNdtTerms * sizeof(double), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) {
+            ctx->err = std::string(fn) + ": " + cudaGetErrorString(e);
+            err = MULLS_E_CUDA;
+        }
+    };
+    std::vector<NdtIter> tr(trace_cap > 0 ? trace_cap : 0);
+    float T[12];
+    int converged = 0;
+    const int iters = ndt_walk(eval, T, converged, tr.data(), (int)tr.size());
+    if (err != MULLS_OK) return err;
+    // getFitnessScore: the exact unbounded nearest target of every moved source point, summed in index order
+    double fitness = DBL_MAX;
+    if (nt > 0 && ns > 0) {
+        std::vector<float> rows((size_t)nt * 12, 0.f);
+        for (int i = 0; i < nt; ++i) rows[12 * (size_t)i] = tgt[i].x, rows[12 * (size_t)i + 1] = tgt[i].y, rows[12 * (size_t)i + 2] = tgt[i].z;
+        DeviceArrays A;
+        int n_in = 0;
+        mulls_cloud_view cv{rows.data(), (size_t)nt};
+        if ((rc = ingest_cloud(ctx, cv, false, 0.f, true, true, A, n_in, launches)) != MULLS_OK) return rc;
+        std::memcpy(E.T, T, sizeof(E.T));
+        k_ndt_fitness<<<(unsigned)ceil_div(ns, 128), 128, 0, st>>>(A, d_s, ns, E, d_d2);
+        launches += 1;
+        std::vector<float> d2(ns);
+        CK(cudaMemcpyAsync(d2.data(), d_d2, ns * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        double sum = 0.0;
+        int cnt = 0;
+        for (int i = 0; i < ns; ++i)
+            if (d2[i] >= 0.f) sum += (double)d2[i], ++cnt;
+        if (cnt) fitness = sum / cnt;
+    }
+    ndt_epilogue(T, guess, moved, out->trans);
+    out->code = fitness > (double)fitness_thre ? -3 : 1;
+    out->iterations = iters;
+    out->converged = converged;
+    out->fitness = fitness;
+    out->n_target = nt;
+    out->n_source = ns;
+    for (int i = 0; i < std::min(iters, trace_cap); ++i) {
+        for (int c = 0; c < 6; ++c) trace[i].p[c] = tr[i].p[c];
+        trace[i].step = tr[i].step, trace[i].score = tr[i].score, trace[i].reversed = tr[i].reversed;
+    }
+    return MULLS_OK;
+}
+int mulls_omp_ndt(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view source, float ndt_resolution, int use_direct_search,
+                  const double initial_guess[16], int apply_intersection_filter, float fitness_score_thre,
+                  const double target_bound[6], const double source_bound[6], mulls_ndt_result *out, mulls_ndt_iter *trace,
+                  int trace_cap) {
+    return front_call(ctx, [&](uint64_t &launches) {
+        return ndt_impl(ctx, target, source, ndt_resolution, use_direct_search, initial_guess, apply_intersection_filter,
+                        fitness_score_thre, target_bound, source_bound, out, trace, trace_cap, launches);
     });
 }
 

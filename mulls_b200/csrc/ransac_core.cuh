@@ -168,17 +168,19 @@ inline void rc_sums_serial(int M, Member in, Value v, double out[K]) {
 }
 
 // ---- R3: Eigen 3.3's JacobiSVD of a 3x3 double (ComputeFullU | ComputeFullV) ----------------------------------------------
-GF_HD void rc_rot_rows(double A[3][3], int p, int q, double c, double s) { // A.applyOnTheLeft(p, q, J(c, s))
+template <int N>
+GF_HD void rc_rot_rows(double (*A)[N], int p, int q, double c, double s) { // A.applyOnTheLeft(p, q, J(c, s))
     if (c == 1.0 && s == 0.0) return;
-    for (int i = 0; i < 3; ++i) {
+    for (int i = 0; i < N; ++i) {
         const double x = A[p][i], y = A[q][i];
         A[p][i] = c * x + s * y;
         A[q][i] = -s * x + c * y;
     }
 }
-GF_HD void rc_rot_cols(double A[3][3], int p, int q, double c, double s) { // apply_rotation_in_the_plane(col p, col q, J(c, s))
+template <int N>
+GF_HD void rc_rot_cols(double (*A)[N], int p, int q, double c, double s) { // apply_rotation_in_the_plane(col p, col q, J(c, s))
     if (c == 1.0 && s == 0.0) return;
-    for (int i = 0; i < 3; ++i) {
+    for (int i = 0; i < N; ++i) {
         const double x = A[i][p], y = A[i][q];
         A[i][p] = c * x + s * y;
         A[i][q] = -s * x + c * y;
@@ -188,26 +190,29 @@ GF_HD double rc_det3(const double m[3][3]) {
     return m[0][0] * (m[1][1] * m[2][2] - m[1][2] * m[2][1]) - m[0][1] * (m[1][0] * m[2][2] - m[1][2] * m[2][0]) +
            m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]);
 }
-GF_HD void rc_svd3(const double A[3][3], double U[3][3], double V[3][3]) {
+// Eigen 3.3's two-sided JacobiSVD of a square N x N double (no QR preconditioner for a square matrix). sv: the singular
+// values, descending; the return value is m_nonzeroSingularValues (the sort stops at the first zero maximum).
+template <int N>
+GF_HD int rc_svd(const double (*A)[N], double (*U)[N], double (*V)[N], double sv[N]) {
     double scale = 0.0;
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j)
+    for (int i = 0; i < N; ++i)
+        for (int j = 0; j < N; ++j)
             if (fabs(A[i][j]) > scale) scale = fabs(A[i][j]);
     if (scale == 0.0) scale = 1.0;
-    double W[3][3];
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) {
+    double W[N][N];
+    for (int i = 0; i < N; ++i)
+        for (int j = 0; j < N; ++j) {
             W[i][j] = A[i][j] / scale;
             U[i][j] = V[i][j] = (i == j) ? 1.0 : 0.0;
         }
     const double considerAsZero = DBL_MIN, precision = 2.0 * DBL_EPSILON;
     double maxDiag = fabs(W[0][0]);
-    if (maxDiag < fabs(W[1][1])) maxDiag = fabs(W[1][1]);
-    if (maxDiag < fabs(W[2][2])) maxDiag = fabs(W[2][2]);
+    for (int i = 1; i < N; ++i)
+        if (maxDiag < fabs(W[i][i])) maxDiag = fabs(W[i][i]);
     bool finished = false;
     for (int sweep = 0; !finished && sweep < kRcSvdSweeps; ++sweep) {
         finished = true;
-        for (int p = 1; p < 3; ++p)
+        for (int p = 1; p < N; ++p)
             for (int q = 0; q < p; ++q) {
                 const double threshold = (considerAsZero < precision * maxDiag) ? precision * maxDiag : considerAsZero;
                 if (!(fabs(W[p][q]) > threshold || fabs(W[q][p]) > threshold)) continue;
@@ -240,32 +245,35 @@ GF_HD void rc_svd3(const double A[3][3], double U[3][3], double V[3][3]) {
                 }
                 // j_left = rot1 * j_right.transpose(), j_right.transpose() = (cr, -sr)
                 const double cl = c1 * cr - s1 * -sr, sl = c1 * -sr + s1 * cr;
-                rc_rot_rows(W, p, q, cl, sl);   // m_workMatrix.applyOnTheLeft(p, q, j_left)
-                rc_rot_cols(U, p, q, cl, sl);   // m_matrixU.applyOnTheRight(p, q, j_left.transpose())
-                rc_rot_cols(W, p, q, cr, -sr);  // m_workMatrix.applyOnTheRight(p, q, j_right)
-                rc_rot_cols(V, p, q, cr, -sr);  // m_matrixV.applyOnTheRight(p, q, j_right)
+                rc_rot_rows<N>(W, p, q, cl, sl);   // m_workMatrix.applyOnTheLeft(p, q, j_left)
+                rc_rot_cols<N>(U, p, q, cl, sl);   // m_matrixU.applyOnTheRight(p, q, j_left.transpose())
+                rc_rot_cols<N>(W, p, q, cr, -sr);  // m_workMatrix.applyOnTheRight(p, q, j_right)
+                rc_rot_cols<N>(V, p, q, cr, -sr);  // m_matrixV.applyOnTheRight(p, q, j_right)
                 const double dp = fabs(W[p][p]), dq = fabs(W[q][q]);
                 const double dm = (dp < dq) ? dq : dp;
                 if (maxDiag < dm) maxDiag = dm;
             }
     }
-    double sv[3];
-    for (int i = 0; i < 3; ++i) {
+    for (int i = 0; i < N; ++i) {
         const double a = W[i][i];
         sv[i] = fabs(a);
         if (a < 0.0)
-            for (int r = 0; r < 3; ++r) U[r][i] = -U[r][i];
+            for (int r = 0; r < N; ++r) U[r][i] = -U[r][i];
     }
-    for (int i = 0; i < 3; ++i) sv[i] *= scale;
-    for (int i = 0; i < 3; ++i) { // descending, the first maximum of the tail
+    for (int i = 0; i < N; ++i) sv[i] *= scale;
+    int nonzero = N;
+    for (int i = 0; i < N; ++i) { // descending, the first maximum of the tail
         int pos = i;
-        for (int j = i + 1; j < 3; ++j)
+        for (int j = i + 1; j < N; ++j)
             if (sv[j] > sv[pos]) pos = j;
-        if (sv[pos] == 0.0) break;
+        if (sv[pos] == 0.0) {
+            nonzero = i;
+            break;
+        }
         if (pos != i) {
             const double ts = sv[i];
             sv[i] = sv[pos], sv[pos] = ts;
-            for (int r = 0; r < 3; ++r) {
+            for (int r = 0; r < N; ++r) {
                 double x = U[r][i];
                 U[r][i] = U[r][pos], U[r][pos] = x;
                 x = V[r][i];
@@ -273,6 +281,11 @@ GF_HD void rc_svd3(const double A[3][3], double U[3][3], double V[3][3]) {
             }
         }
     }
+    return nonzero;
+}
+GF_HD void rc_svd3(const double A[3][3], double U[3][3], double V[3][3]) {
+    double sv[3];
+    rc_svd<3>(A, U, V, sv);
 }
 
 // the Umeyama fit from the fixed-order sums: ms[6] = sums of (sx sy sz tx ty tz), cs[9] = sums of

@@ -365,6 +365,41 @@ class Context:
                                                      C.byref(nh)))
         return st.value, buf.reshape(4, 4), ni.value, nh.value
 
+    def omp_ndt(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, ndt_resolution: float = 1.0,
+                use_direct_search: bool = True, initial_guess=None, apply_intersection_filter: bool = True,
+                fitness_score_thre: float = 10.0, trace_cap: int = 0):
+        """CRegistration::omp_ndt (cregistration.hpp:945-1021, DIRECT7) on the GPU: target / source are block1 / block2
+        ->pc_down ((n, 3), (n, 7) or (n, 12) rows), the bounds their local_bound (min_x min_y min_z max_x max_y max_z). Returns a dict: code (1, or -3 when
+        the fitness exceeds fitness_score_thre), trans (Trans1_2, (4, 4) float64), iterations, converged, fitness,
+        n_target / n_source after the intersection filter, and with trace_cap > 0 `trace`: per iteration the pose vector
+        p (6), the step length, the score and whether the direction was reversed. use_direct_search=False (KDTREE) raises. Replaces the resident batch."""
+        def aos48(c):  # (n, 3) xyz rows are accepted too: NDT reads positions only
+            c = np.asarray(c, np.float32)
+            if c.ndim == 2 and c.shape[1] == 3:
+                c = np.concatenate([c, np.zeros((len(c), 9), np.float32)], axis=1)
+            return abi.as_aos48(c)
+
+        t, s = aos48(target), aos48(source)
+        g = np.ascontiguousarray(np.eye(4) if initial_guess is None else initial_guess, np.float64).reshape(16).copy()
+        tb = np.ascontiguousarray(target_bound, np.float64).reshape(6).copy()
+        sb = np.ascontiguousarray(source_bound, np.float64).reshape(6).copy()
+        res = abi.NdtResult()
+        tr = (abi.NdtIter * max(int(trace_cap), 1))()
+        dp = C.POINTER(C.c_double)
+        self._check(self.lib.mulls_omp_ndt(self.handle, abi.cloud_view(t), abi.cloud_view(s), float(ndt_resolution),
+                                           int(bool(use_direct_search)), g.ctypes.data_as(dp), int(bool(apply_intersection_filter)),
+                                           float(fitness_score_thre), tb.ctypes.data_as(dp), sb.ctypes.data_as(dp), C.byref(res),
+                                           tr, int(trace_cap)))
+        out = dict(code=res.code, trans=np.array(res.trans[:], np.float64).reshape(4, 4), iterations=res.iterations,
+                   converged=bool(res.converged), fitness=res.fitness, n_target=res.n_target, n_source=res.n_source)
+        if trace_cap > 0:
+            k = min(res.iterations, int(trace_cap))
+            out["trace"] = dict(p=np.array([tr[i].p[:] for i in range(k)], np.float64).reshape(k, 6),
+                                step=np.array([tr[i].step for i in range(k)], np.float64),
+                                score=np.array([tr[i].score for i in range(k)], np.float64),
+                                reversed=np.array([tr[i].reversed for i in range(k)], np.int32))
+        return out
+
     def non_max_suppress(self, cloud: np.ndarray, non_max_radius: float):
         """CFilter::non_max_suppress(cloud_in_out, non_max_radius) (cfilter.hpp:1183-1240) on the GPU. Returns
         (kept_idx, performed): kept_idx is an int32 array of the input rows the reference leaves in the cloud, in its
@@ -537,6 +572,15 @@ class CRegistration:
         given (4, 4) matrix (identity when None), replaced by the estimate when status >= 0 and left as it was on -1."""
         status, T, _, _ = self._ctx.coarse_reg_ransac(target_pts, source_pts, noise_bound, min_inlier_num, max_iter_num, tran_mat)
         return status, T
+
+    def omp_ndt(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, ndt_resolution: float = 1.0,
+                use_direct_search: bool = True, initial_guess=None, apply_intersection_filter: bool = True,
+                fitness_score_thre: float = 10.0):
+        """lo::CRegistration::omp_ndt (cregistration.hpp:945-1021): returns (code, Trans1_2) for block1 = target and
+        block2 = source with their local_bounds. Only the DIRECT7 search (use_direct_search=True) runs here."""
+        r = self._ctx.omp_ndt(target, source, target_bound, source_bound, ndt_resolution, use_direct_search, initial_guess,
+                              apply_intersection_filter, fitness_score_thre)
+        return r["code"], r["trans"]
 
     def mm_lls_icp_4dof_global(self, registration_con: Constraint, heading_step_d: float, max_iter_num: int = 20,
                                dis_thre_unit: float = 1.5, converge_translation: float = 0.005,
