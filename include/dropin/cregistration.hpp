@@ -11,10 +11,10 @@
 //     CRegistration_reference — every member the reference defines stays available, unchanged;
 //   * lo::CRegistration<PointT> is then defined HERE as a class derived from it whose mm_lls_icp
 //     (cregistration.hpp:1114-1123: same name, argument order, types and defaults) and mm_lls_icp_4dof_global
-//     (:1584-1592), find_feature_correspondence_ncc (:409-411) and coarse_reg_ransac (:605-607) run on the GPU through
-//     the C-ABI (include/mulls_b200/abi.h). All other public members the callers use
+//     (:1584-1592), find_feature_correspondence_ncc (:409-411), coarse_reg_ransac (:605-607), omp_ndt (:945-947) and
+//     omp_gicp (:1024-1027) run on the GPU through the C-ABI (include/mulls_b200/abi.h). All other public members the callers use
 //     — determine_source_target_cloud, assign_source_target_cloud, coarse_reg_teaser,
-//     omp_gicp, ... (SURVEY.md section 8b) — are inherited from the reference; every overload of
+//     ... (SURVEY.md section 8b) — are inherited from the reference; every overload of
 //     coarse_reg_ransac the reference class declares stays visible next to the device one.
 // Differences in contract are listed in INTEGRATION.md (block1->tree_* are not populated: use mulls_nn_query or
 // the drop-in lo::MapManager of dropin/map_manager.h, which does not need them).
@@ -93,6 +93,24 @@ class CRegistration : public CRegistration_reference<PointT> {
             return CRegistration_reference<PointT>::omp_ndt(registration_cons, ndt_resolution, use_direct_search, initial_guess,
                                                             apply_intersection_filter, fitness_score_thre);
         return b200::omp_ndt<PointT>(registration_cons, ndt_resolution, initial_guess, apply_intersection_filter, fitness_score_thre);
+    }
+    // cregistration.hpp:1024-1027. The device runs the voxelized GICP (FastVGICP), where max_iter_num and dis_thre_unit
+    // have no effect; using_voxel_gicp = false (PCL-style GICP) and the calls the library refuses (fewer than 20
+    // points in a cloud) are the reference member. A template on the guess type, as omp_ndt.
+    template <typename Matrix4 = Eigen::Matrix4d>
+    int omp_gicp(constraint_t &registration_cons, int max_iter_num = 20, float dis_thre_unit = 1.5, bool using_voxel_gicp = true,
+                 float voxel_size = 1.0, Matrix4 initial_guess = Matrix4::Identity(), bool apply_intersection_filter = false,
+                 float fitness_score_thre = 10.0) {
+        bool unsupported = !using_voxel_gicp;
+        int code = -3;
+        if (using_voxel_gicp)
+            code = b200::omp_gicp<PointT>(registration_cons, voxel_size, initial_guess, apply_intersection_filter, fitness_score_thre,
+                                          &unsupported);
+        if (unsupported)
+            return CRegistration_reference<PointT>::omp_gicp(registration_cons, max_iter_num, dis_thre_unit, using_voxel_gicp,
+                                                             voxel_size, initial_guess, apply_intersection_filter,
+                                                             fitness_score_thre);
+        return code;
     }
 };
 

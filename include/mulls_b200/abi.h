@@ -40,6 +40,7 @@
  *   mulls_coarse_reg_ransac  <- lo::CRegistration<PointT>::coarse_reg_ransac, cregistration.hpp:604-661
  *   mulls_non_max_suppress   <- lo::CFilter<PointT>::non_max_suppress(cloud_in_out, non_max_radius), cfilter.hpp:1183-1240
  *   mulls_omp_ndt            <- lo::CRegistration<PointT>::omp_ndt with use_direct_search (DIRECT7), cregistration.hpp:945-1021
+ *   mulls_omp_gicp           <- lo::CRegistration<PointT>::omp_gicp with using_voxel_gicp (FastVGICP), cregistration.hpp:1024-1098
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
  *
@@ -643,6 +644,50 @@ int mulls_omp_ndt(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view sour
                   const double initial_guess[16] /* row-major */, int apply_intersection_filter, float fitness_score_thre,
                   const double target_bound[6], const double source_bound[6], mulls_ndt_result *out, mulls_ndt_iter *trace,
                   int trace_cap);
+
+/* Voxelized GICP registration: lo::CRegistration<PointT>::omp_gicp(reg_con, max_iter_num, dis_thre_unit, using_voxel_gicp,
+ * voxel_size, initial_guess, apply_intersection_filter, fitness_score_thre) (cregistration.hpp:1024-1098) with
+ * using_voxel_gicp, i.e. koide_reg::FastVGICP (include/baseline_reg/fast_vgicp_impl.hpp) in its Sophus build.
+ * target = block1->pc_down, source = block2->pc_down, target_bound / source_bound = block1 / block2 ->local_bound. The
+ * readings of the reference are listed in mulls_b200/csrc/gicp_core.cuh (G1-G7, C1-C3); in short:
+ *   - prologue: omp_ndt's (see mulls_omp_ndt), with apply_intersection_filter defaulting to false in omp_gicp; points
+ *     with a non-finite coordinate are dropped from both clouds;
+ *   - each cloud's covariances from its 20 nearest neighbours (the point itself included), PLANE-regularised; target
+ *     voxels of edge voxel_size (coord floor(x / res - 0.5)) with the ADDITIVE means and covariances;
+ *   - the Gauss-Newton walk with FastVGICP's defaults (64 iterations, rotation / translation epsilons 2e-3 / 5e-4,
+ *     DIRECT1): max_iter_num and dis_thre_unit have no effect in the reference and are not parameters here;
+ *   - the walk draws from the process's rand() where the reference does: 3 draws for its start point, 6 more for every
+ *     step the LLT solve leaves non-finite (for instance when no source point hits a voxel);
+ *   - fitness = getFitnessScore() as mulls_omp_ndt; code -3 when fitness > fitness_score_thre, else 1;
+ *     Trans1_2 = (double)final_transformation * initial_guess when the guess moved the source, else the former.
+ * The walk runs on the host: one evaluation (two kernels and one 224-byte download) per iteration. The call replaces
+ * the resident batch (both clouds go through the ingest). iterations = the Gauss-Newton steps taken (at most 64; the
+ * reference's nr_iterations_ + 1), converged = converged_, x0 = the start point (so3, translation). trace (may be NULL
+ * with trace_cap 0) receives up to trace_cap iterations: the point after the step, the step, the correspondence count
+ * and whether the step was the random fallback. Refused with MULLS_E_UNSUPPORTED: using_voxel_gicp = 0 (the drop-in
+ * calls the reference member), fewer than 20 points in either cloud after the prologue (the reference reads
+ * uninitialised memory there), a target whose voxel coordinates do not fit 21 bits. A NULL output or matrix, NULL rows
+ * with n > 0, or voxel_size <= 0: MULLS_E_ARG. Either cloud above max_tgt_pts: MULLS_E_CAPACITY. */
+typedef struct mulls_gicp_result {
+    double trans[16];  /* Trans1_2, row-major */
+    int code;          /* 1, or -3 when fitness > fitness_score_thre */
+    int iterations;
+    int converged;
+    int n_target;      /* points after the prologue (finite) */
+    int n_source;
+    double fitness;
+    float x0[6];       /* the walk's start point: so3 then translation */
+} mulls_gicp_result;
+typedef struct mulls_gicp_iter {
+    float x[6];        /* so3 then translation after the step */
+    float delta[6];    /* the Gauss-Newton step */
+    int n_corr;        /* correspondences (source points in a voxel) of the evaluation */
+    int random_step;   /* 1: the solve was not finite and the step is Random() * 1e-2 */
+} mulls_gicp_iter;
+int mulls_omp_gicp(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view source, int using_voxel_gicp, float voxel_size,
+                   const double initial_guess[16] /* row-major */, int apply_intersection_filter, float fitness_score_thre,
+                   const double target_bound[6], const double source_bound[6], mulls_gicp_result *out, mulls_gicp_iter *trace,
+                   int trace_cap);
 
 /* The wire format the library ships host clouds in when the "host_pack" tunable is on (csrc/host_pack.h): the 28 of the
  * 48 bytes of a pcl::PointXYZINormal row (utility.hpp:40) that the path reads, repacked on the host cores into pinned

@@ -123,6 +123,27 @@ class NdtIter(C.Structure):
     _fields_ = [("p", C.c_double * 6), ("step", C.c_double), ("score", C.c_double), ("reversed", C.c_int)]
 
 
+class GicpResult(C.Structure):
+    """mulls_gicp_result: Trans1_2, the code omp_gicp returns, the walk's step count and convergence, the point counts
+    after the prologue, the fitness score and the walk's start point x0 (so3, translation)."""
+    _fields_ = [
+        ("trans", C.c_double * 16),
+        ("code", C.c_int),
+        ("iterations", C.c_int),
+        ("converged", C.c_int),
+        ("n_target", C.c_int),
+        ("n_source", C.c_int),
+        ("fitness", C.c_double),
+        ("x0", C.c_float * 6),
+    ]
+
+
+class GicpIter(C.Structure):
+    """mulls_gicp_iter: one Gauss-Newton step of the VGICP walk (point after the step, the step, correspondences,
+    whether the step was the random fallback)."""
+    _fields_ = [("x", C.c_float * 6), ("delta", C.c_float * 6), ("n_corr", C.c_int), ("random_step", C.c_int)]
+
+
 class SorStats(C.Structure):
     """mulls_sor_stats: what pcl::StatisticalOutlierRemoval computed (mean, stddev, threshold) and the point counts."""
     _fields_ = [
@@ -310,6 +331,7 @@ EXPORTED_SYMBOLS = (
     "mulls_coarse_reg_ransac",
     "mulls_non_max_suppress",
     "mulls_omp_ndt",
+    "mulls_omp_gicp",
     "mulls_scan_probe",
     "mulls_scan_read",
     "mulls_pose_write",
@@ -399,6 +421,10 @@ def load_library() -> C.CDLL:
     lib.mulls_omp_ndt.restype = C.c_int
     lib.mulls_omp_ndt.argtypes = [vp, CloudView, CloudView, C.c_float, C.c_int, C.POINTER(C.c_double), C.c_int, C.c_float,
                                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(NdtResult), C.POINTER(NdtIter), C.c_int]
+    lib.mulls_omp_gicp.restype = C.c_int
+    lib.mulls_omp_gicp.argtypes = [vp, CloudView, CloudView, C.c_int, C.c_float, C.POINTER(C.c_double), C.c_int, C.c_float,
+                                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(GicpResult), C.POINTER(GicpIter),
+                                   C.c_int]
     lib.mulls_pack_rows.restype = C.c_int
     lib.mulls_pack_rows.argtypes = [C.POINTER(C.c_float), C.c_size_t, C.c_int, C.POINTER(C.c_float)]
     lib.mulls_scan_probe.restype = C.c_int

@@ -66,6 +66,33 @@ __device__ __forceinline__ int ndt_find_leaf(const uint64_t *keys, int n, uint64
     return (lo < n && keys[lo] == key) ? lo : -1;
 }
 
+// C1 of ndt_core.cuh over one block of kNdtTile threads, each holding its point's kTerms sums in acc: the pairwise tree
+// inside each warp (shuffles), then over the warps; thread c < kTerms stores the tile's sum of term c at
+// tile_sums[blockIdx.x * kTerms + c]. Shared by every evaluation that sums in that order (NDT, GICP).
+template <int kTerms>
+__device__ __forceinline__ void tile_tree_store(const double (&acc)[kTerms], double *tile_sums) {
+    __shared__ double s_w[kNdtTile / 32][kTerms];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+    for (int c = 0; c < kTerms; ++c) {
+        double v = acc[c];
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) v += __shfl_down_sync(0xffffffffu, v, s);
+        if (lane == 0) s_w[w][c] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < kTerms) {
+        double q[kNdtTile / 32];
+#pragma unroll
+        for (int g = 0; g < kNdtTile / 32; ++g) q[g] = s_w[g][threadIdx.x];
+#pragma unroll
+        for (int s = kNdtTile / 64; s > 0; s >>= 1)
+#pragma unroll
+            for (int t = 0; t < s; ++t) q[t] += q[t + s];
+        tile_sums[(size_t)blockIdx.x * kTerms + threadIdx.x] = q[0];
+    }
+}
+
 __global__ void __launch_bounds__(kNdtTile) k_ndt_eval(NdtEvalArgs A, NdtEvalConst E) {
     const int i = blockIdx.x * kNdtTile + threadIdx.x;
     double acc[kNdtTerms];
@@ -90,27 +117,7 @@ __global__ void __launch_bounds__(kNdtTile) k_ndt_eval(NdtEvalArgs A, NdtEvalCon
                 }
         }
     }
-    // C1: the pairwise tree inside the warp, then over the warps
-    __shared__ double s_w[kNdtTile / 32][kNdtTerms];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#pragma unroll
-    for (int c = 0; c < kNdtTerms; ++c) {
-        double v = acc[c];
-#pragma unroll
-        for (int s = 16; s > 0; s >>= 1) v += __shfl_down_sync(0xffffffffu, v, s);
-        if (lane == 0) s_w[w][c] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kNdtTerms) {
-        double q[kNdtTile / 32];
-#pragma unroll
-        for (int g = 0; g < kNdtTile / 32; ++g) q[g] = s_w[g][threadIdx.x];
-#pragma unroll
-        for (int s = kNdtTile / 64; s > 0; s >>= 1)
-#pragma unroll
-            for (int t = 0; t < s; ++t) q[t] += q[t + s];
-        A.tile_sums[(size_t)blockIdx.x * kNdtTerms + threadIdx.x] = q[0];
-    }
+    tile_tree_store<kNdtTerms>(acc, A.tile_sums);
 }
 
 __global__ void __launch_bounds__(64) k_ndt_tiles(const double *__restrict__ tile_sums, int tiles, double *__restrict__ out) {

@@ -32,6 +32,7 @@
 #include "kernels_ncc.cuh"
 #include "kernels_ransac.cuh"
 #include "kernels_ndt.cuh"
+#include "kernels_gicp.cuh"
 
 using namespace mulls;
 
@@ -163,6 +164,7 @@ struct mulls_ctx {
     Scratch rc_buf;              // RANSAC coarse registration: correspondences, hypotheses, counts, refinement state
     Scratch nms_buf;             // keypoint NMS: rows, sorted rows, keys, sort scratch, cell hash, kept indices
     Scratch ndt_buf;             // NDT: clouds, leaf keys and sort scratch, leaves, tile sums, fitness distances
+    Scratch gicp_buf;            // GICP: clouds, covariances, voxel keys and sort scratch, voxels, tile sums, distances
     void *rc_host = nullptr;     // pinned: two chunks of sample triples and their counts
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
@@ -265,7 +267,8 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (void *p : ctx->allocs) cudaFree(p);
     if (ctx->cub_temp) cudaFree(ctx->cub_temp);
-    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf, &ctx->ncc_buf, &ctx->rc_buf, &ctx->nms_buf})
+    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf, &ctx->ncc_buf, &ctx->rc_buf, &ctx->nms_buf,
+                        &ctx->ndt_buf, &ctx->gicp_buf})
         if (s->p) cudaFree(s->p);
     if (ctx->rc_host) cudaFreeHost(ctx->rc_host);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
@@ -1947,6 +1950,68 @@ int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_c
 }
 
 // ================================================================================================
+// The baseline registrations (CRegistration::omp_ndt, omp_gicp): what both share on the host
+// ================================================================================================
+// the temporary bytes of sort_runs over n keys
+static int sort_runs_bytes(mulls_ctx *ctx, int n, size_t &bytes) {
+    size_t cub_sort = 0, cub_rle = 0, cub_scan = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_sort, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint32_t *)nullptr,
+                                       (uint32_t *)nullptr, std::max(n, 1)));
+    CK(cub::DeviceRunLengthEncode::Encode(nullptr, cub_rle, (uint64_t *)nullptr, (uint64_t *)nullptr, (int *)nullptr,
+                                          (int *)nullptr, std::max(n, 1)));
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_scan, (int *)nullptr, (int *)nullptr, std::max(n, 1)));
+    bytes = std::max(cub_sort, std::max(cub_rle, cub_scan));
+    return MULLS_OK;
+}
+// keys ka with values va (the point indices) sorted stably into kb / vb, then the runs of equal keys: uk the run keys
+// (ascending), cnt the run lengths, off their exclusive prefix sum, *nr the run count
+static int sort_runs(mulls_ctx *ctx, void *d_cub, size_t cub_bytes, int n, uint64_t *ka, uint64_t *kb, uint32_t *va,
+                     uint32_t *vb, uint64_t *uk, int *cnt, int *off, int *nr, cudaStream_t st) {
+    size_t b = cub_bytes;
+    CK(cub::DeviceRadixSort::SortPairs(d_cub, b, ka, kb, va, vb, n, 0, 64, st));
+    CK(cudaMemsetAsync(cnt, 0, n * 4ull, st));
+    b = cub_bytes;
+    CK(cub::DeviceRunLengthEncode::Encode(d_cub, b, kb, uk, cnt, nr, n, st));
+    b = cub_bytes;
+    CK(cub::DeviceScan::ExclusiveSum(d_cub, b, cnt, off, n, st));
+    return MULLS_OK;
+}
+// the full-pyramid grid of finite points (the rows the ingest takes): what getFitnessScore and the k-nearest
+// covariances search
+static int ingest_points(mulls_ctx *ctx, const std::vector<float4> &pts, DeviceArrays &A, uint64_t &launches) {
+    std::vector<float> rows(pts.size() * 12, 0.f);
+    for (size_t i = 0; i < pts.size(); ++i) rows[12 * i] = pts[i].x, rows[12 * i + 1] = pts[i].y, rows[12 * i + 2] = pts[i].z;
+    int n_in = 0;
+    mulls_cloud_view cv{rows.data(), pts.size()};
+    return ingest_cloud(ctx, cv, false, 0.f, true, true, A, n_in, launches);
+}
+// the epilogue: getFitnessScore (the exact unbounded nearest target of every moved source point, summed in index
+// order; DBL_MAX when nothing counts) over the target's grid A (NULL: no target), Trans1_2 and the code
+static int baseline_finish(mulls_ctx *ctx, const DeviceArrays *A, const float4 *d_s, int ns, float *d_d2, const float T[12],
+                           const double *guess, bool moved, float fitness_thre, double trans[16], int &code, double &fitness,
+                           uint64_t &launches) {
+    cudaStream_t st = ctx->stream;
+    fitness = DBL_MAX;
+    if (A && ns > 0) {
+        NdtEvalConst E;
+        std::memcpy(E.T, T, sizeof(E.T));
+        k_ndt_fitness<<<(unsigned)ceil_div(ns, 128), 128, 0, st>>>(*A, d_s, ns, E, d_d2);
+        launches += 1;
+        std::vector<float> d2(ns);
+        CK(cudaMemcpyAsync(d2.data(), d_d2, ns * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        double sum = 0.0;
+        int cnt = 0;
+        for (int i = 0; i < ns; ++i)
+            if (d2[i] >= 0.f) sum += (double)d2[i], ++cnt;
+        if (cnt) fitness = sum / cnt;
+    }
+    ndt_epilogue(T, guess, moved, trans);
+    code = fitness > (double)fitness_thre ? -3 : 1;
+    return MULLS_OK;
+}
+
+// ================================================================================================
 // NDT registration (CRegistration::omp_ndt, cregistration.hpp:945-1021, DIRECT7): ndt_core.cuh, kernels_ndt.cuh
 // ================================================================================================
 static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, float resolution, int use_direct_search,
@@ -1972,13 +2037,8 @@ static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, fl
     const NdtGrid g = ndt_grid_from(tgt, resolution);
     const int nt = (int)tgt.size(), ns = (int)src.size(), tiles = (int)ceil_div((size_t)ns, kNdtTile);
     cudaStream_t st = ctx->stream;
-    size_t cub_sort = 0, cub_rle = 0, cub_scan = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_sort, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint32_t *)nullptr,
-                                       (uint32_t *)nullptr, std::max(nt, 1)));
-    CK(cub::DeviceRunLengthEncode::Encode(nullptr, cub_rle, (uint64_t *)nullptr, (uint64_t *)nullptr, (int *)nullptr,
-                                          (int *)nullptr, std::max(nt, 1)));
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_scan, (int *)nullptr, (int *)nullptr, std::max(nt, 1)));
-    const size_t cub_bytes = std::max(cub_sort, std::max(cub_rle, cub_scan));
+    size_t cub_bytes = 0;
+    if ((rc = sort_runs_bytes(ctx, nt, cub_bytes)) != MULLS_OK) return rc;
     ScratchLayout L;
     const size_t o_t = L.take(nt * sizeof(float4)), o_s = L.take(ns * sizeof(float4)), o_ka = L.take(nt * 8ull),
                  o_kb = L.take(nt * 8ull), o_va = L.take(nt * 4ull), o_vb = L.take(nt * 4ull), o_uk = L.take(nt * 8ull),
@@ -1999,14 +2059,8 @@ static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, fl
     if (ns) CK(cudaMemcpyAsync(d_s, src.data(), ns * sizeof(float4), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(d_nr, 0, sizeof(int), st));
     if (g.ok) { // the leaves (N1)
-        size_t b = cub_bytes;
         k_ndt_keys<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, nt, g, d_ka, d_va);
-        CK(cub::DeviceRadixSort::SortPairs(d_cub, b, d_ka, d_kb, d_va, d_vb, nt, 0, 64, st));
-        CK(cudaMemsetAsync(d_cnt, 0, nt * 4ull, st));
-        b = cub_bytes;
-        CK(cub::DeviceRunLengthEncode::Encode(d_cub, b, d_kb, d_uk, d_cnt, d_nr, nt, st));
-        b = cub_bytes;
-        CK(cub::DeviceScan::ExclusiveSum(d_cub, b, d_cnt, d_off, nt, st));
+        if ((rc = sort_runs(ctx, d_cub, cub_bytes, nt, d_ka, d_kb, d_va, d_vb, d_uk, d_cnt, d_off, d_nr, st)) != MULLS_OK) return rc;
         k_ndt_leaves<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, d_vb, d_off, d_cnt, d_nr, d_lv);
         launches += 2;
     }
@@ -2038,32 +2092,14 @@ static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, fl
     int converged = 0;
     const int iters = ndt_walk(eval, T, converged, tr.data(), (int)tr.size());
     if (err != MULLS_OK) return err;
-    // getFitnessScore: the exact unbounded nearest target of every moved source point, summed in index order
-    double fitness = DBL_MAX;
-    if (nt > 0 && ns > 0) {
-        std::vector<float> rows((size_t)nt * 12, 0.f);
-        for (int i = 0; i < nt; ++i) rows[12 * (size_t)i] = tgt[i].x, rows[12 * (size_t)i + 1] = tgt[i].y, rows[12 * (size_t)i + 2] = tgt[i].z;
-        DeviceArrays A;
-        int n_in = 0;
-        mulls_cloud_view cv{rows.data(), (size_t)nt};
-        if ((rc = ingest_cloud(ctx, cv, false, 0.f, true, true, A, n_in, launches)) != MULLS_OK) return rc;
-        std::memcpy(E.T, T, sizeof(E.T));
-        k_ndt_fitness<<<(unsigned)ceil_div(ns, 128), 128, 0, st>>>(A, d_s, ns, E, d_d2);
-        launches += 1;
-        std::vector<float> d2(ns);
-        CK(cudaMemcpyAsync(d2.data(), d_d2, ns * sizeof(float), cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        double sum = 0.0;
-        int cnt = 0;
-        for (int i = 0; i < ns; ++i)
-            if (d2[i] >= 0.f) sum += (double)d2[i], ++cnt;
-        if (cnt) fitness = sum / cnt;
-    }
-    ndt_epilogue(T, guess, moved, out->trans);
-    out->code = fitness > (double)fitness_thre ? -3 : 1;
+    DeviceArrays A;
+    const bool fit = nt > 0 && ns > 0;
+    if (fit && (rc = ingest_points(ctx, tgt, A, launches)) != MULLS_OK) return rc;
+    if ((rc = baseline_finish(ctx, fit ? &A : nullptr, d_s, ns, d_d2, T, guess, moved, fitness_thre, out->trans, out->code,
+                              out->fitness, launches)) != MULLS_OK)
+        return rc;
     out->iterations = iters;
     out->converged = converged;
-    out->fitness = fitness;
     out->n_target = nt;
     out->n_source = ns;
     for (int i = 0; i < std::min(iters, trace_cap); ++i) {
@@ -2079,6 +2115,126 @@ int mulls_omp_ndt(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view sour
     return front_call(ctx, [&](uint64_t &launches) {
         return ndt_impl(ctx, target, source, ndt_resolution, use_direct_search, initial_guess, apply_intersection_filter,
                         fitness_score_thre, target_bound, source_bound, out, trace, trace_cap, launches);
+    });
+}
+
+// ================================================================================================
+// Voxelized GICP registration (CRegistration::omp_gicp, cregistration.hpp:1024-1098, FastVGICP): gicp_core.cuh,
+// kernels_gicp.cuh
+// ================================================================================================
+static int gicp_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, int using_voxel_gicp, float voxel_size,
+                     const double *guess, int apply_filter, float fitness_thre, const double *tbound, const double *sbound,
+                     mulls_gicp_result *out, mulls_gicp_iter *trace, int trace_cap, uint64_t &launches) {
+    if (!out || !guess || !tbound || !sbound || (tv.n && !tv.aos48) || (sv.n && !sv.aos48) || !(voxel_size > 0.f) ||
+        (trace_cap > 0 && !trace))
+        return MULLS_E_ARG;
+    const char *fn = "mulls_omp_gicp";
+    if (!using_voxel_gicp) {
+        ctx->err = std::string(fn) + ": only the voxelized GICP (FastVGICP) runs on the device";
+        return MULLS_E_UNSUPPORTED;
+    }
+    int rc;
+    // both clouds go through the ingest (their k-nearest covariances)
+    if ((rc = check_capacity(ctx, tv.n, fn)) != MULLS_OK || (rc = check_capacity(ctx, sv.n, fn)) != MULLS_OK) return rc;
+    std::vector<float4> tgt, src;
+    bool moved = false;
+    ndt_prologue(tv.aos48, tv.n, sv.aos48, sv.n, guess, apply_filter, tbound, sbound, tgt, src, moved);
+    gicp_keep_finite(src); // (the prologue keeps the target's finite points only)
+    const int nt = (int)tgt.size(), ns = (int)src.size(), tiles = (int)ceil_div((size_t)ns, kNdtTile);
+    if (nt < kGicpK || ns < kGicpK) {
+        ctx->err = std::string(fn) + ": " + std::to_string(nt) + " target and " + std::to_string(ns) +
+                   " source points after the prologue; the covariances need " + std::to_string(kGicpK) + " in each";
+        return MULLS_E_UNSUPPORTED;
+    }
+    { // C2: the voxel coordinate is monotonic in each axis, so the target's bounds bound every key
+        float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+        for (const float4 &p : tgt) {
+            const float v[3] = {p.x, p.y, p.z};
+            for (int d = 0; d < 3; ++d) mn[d] = std::min(mn[d], v[d]), mx[d] = std::max(mx[d], v[d]);
+        }
+        uint64_t k;
+        if (!gicp_key_of(mn[0], mn[1], mn[2], voxel_size, k) || !gicp_key_of(mx[0], mx[1], mx[2], voxel_size, k)) {
+            ctx->err = std::string(fn) + ": the target's voxel coordinates exceed " + std::to_string(kGicpCoordBits) + " bits";
+            return MULLS_E_UNSUPPORTED;
+        }
+    }
+    cudaStream_t st = ctx->stream;
+    size_t cub_bytes = 0;
+    if ((rc = sort_runs_bytes(ctx, nt, cub_bytes)) != MULLS_OK) return rc;
+    ScratchLayout L;
+    const size_t o_t = L.take(nt * sizeof(float4)), o_s = L.take(ns * sizeof(float4)), o_ct = L.take(nt * 36ull),
+                 o_cs = L.take(ns * 36ull), o_ka = L.take(nt * 8ull), o_kb = L.take(nt * 8ull), o_va = L.take(nt * 4ull),
+                 o_vb = L.take(nt * 4ull), o_uk = L.take(nt * 8ull), o_cnt = L.take(nt * 4ull), o_off = L.take(nt * 4ull),
+                 o_nr = L.take(sizeof(int)), o_vx = L.take(nt * sizeof(GicpVoxel)),
+                 o_ts = L.take((size_t)tiles * kGicpTerms * 8), o_out = L.take(kGicpTerms * 8),
+                 o_d2 = L.take(ns * sizeof(float)), o_cub = L.take(cub_bytes);
+    char *base;
+    if ((rc = L.grow(ctx, ctx->gicp_buf, base)) != MULLS_OK) return rc;
+    float4 *d_t = (float4 *)(base + o_t), *d_s = (float4 *)(base + o_s);
+    float *d_ct = (float *)(base + o_ct), *d_cs = (float *)(base + o_cs), *d_d2 = (float *)(base + o_d2);
+    uint64_t *d_ka = (uint64_t *)(base + o_ka), *d_kb = (uint64_t *)(base + o_kb), *d_uk = (uint64_t *)(base + o_uk);
+    uint32_t *d_va = (uint32_t *)(base + o_va), *d_vb = (uint32_t *)(base + o_vb);
+    int *d_cnt = (int *)(base + o_cnt), *d_off = (int *)(base + o_off), *d_nr = (int *)(base + o_nr);
+    GicpVoxel *d_vx = (GicpVoxel *)(base + o_vx);
+    double *d_ts = (double *)(base + o_ts), *d_out = (double *)(base + o_out);
+    void *d_cub = base + o_cub;
+    CK(cudaMemcpyAsync(d_t, tgt.data(), nt * sizeof(float4), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_s, src.data(), ns * sizeof(float4), cudaMemcpyHostToDevice, st));
+    // G1: the source's covariances, then the target's (its grid stays for the fitness)
+    DeviceArrays A;
+    if ((rc = ingest_points(ctx, src, A, launches)) != MULLS_OK) return rc;
+    k_gicp_cov<<<(unsigned)ceil_div(ns, kGicpCovBlock), kGicpCovBlock, 0, st>>>(A, d_cs);
+    k_gicp_plane<<<(unsigned)ceil_div(ns, kGicpCovBlock), kGicpCovBlock, 0, st>>>(d_cs, ns);
+    if ((rc = ingest_points(ctx, tgt, A, launches)) != MULLS_OK) return rc;
+    k_gicp_cov<<<(unsigned)ceil_div(nt, kGicpCovBlock), kGicpCovBlock, 0, st>>>(A, d_ct);
+    k_gicp_plane<<<(unsigned)ceil_div(nt, kGicpCovBlock), kGicpCovBlock, 0, st>>>(d_ct, nt);
+    // G2: the voxels
+    k_gicp_keys<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, nt, voxel_size, d_ka, d_va);
+    if ((rc = sort_runs(ctx, d_cub, cub_bytes, nt, d_ka, d_kb, d_va, d_vb, d_uk, d_cnt, d_off, d_nr, st)) != MULLS_OK) return rc;
+    k_gicp_voxels<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, d_ct, d_vb, d_off, d_cnt, d_nr, d_vx);
+    launches += 6;
+    GicpEvalArgs EA{d_s, d_cs, ns, voxel_size, d_uk, d_vx, d_nr, d_ts};
+    NdtEvalConst E;
+    int err = MULLS_OK;
+    auto eval = [&](const float T[12], double r[kGicpTerms]) {
+        for (int c = 0; c < kGicpTerms; ++c) r[c] = 0.0;
+        if (err != MULLS_OK) return;
+        std::memcpy(E.T, T, sizeof(E.T));
+        k_gicp_eval<<<(unsigned)tiles, kNdtTile, 0, st>>>(EA, E);
+        k_gicp_tiles<<<1, 32, 0, st>>>(d_ts, tiles, d_out);
+        launches += 2;
+        cudaError_t e = cudaMemcpyAsync(r, d_out, kGicpTerms * sizeof(double), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) {
+            ctx->err = std::string(fn) + ": " + cudaGetErrorString(e);
+            err = MULLS_E_CUDA;
+        }
+    };
+    std::vector<GicpIter> tr(trace_cap > 0 ? trace_cap : 0);
+    float T[12];
+    int converged = 0;
+    const int iters = gicp_walk(eval, T, out->x0, converged, tr.data(), (int)tr.size());
+    if (err != MULLS_OK) return err;
+    if ((rc = baseline_finish(ctx, &A, d_s, ns, d_d2, T, guess, moved, fitness_thre, out->trans, out->code, out->fitness,
+                              launches)) != MULLS_OK)
+        return rc;
+    out->iterations = iters;
+    out->converged = converged;
+    out->n_target = nt;
+    out->n_source = ns;
+    for (int i = 0; i < std::min(iters, trace_cap); ++i) {
+        for (int c = 0; c < 6; ++c) trace[i].x[c] = tr[i].x[c], trace[i].delta[c] = tr[i].delta[c];
+        trace[i].n_corr = tr[i].n_corr, trace[i].random_step = tr[i].random;
+    }
+    return MULLS_OK;
+}
+int mulls_omp_gicp(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view source, int using_voxel_gicp, float voxel_size,
+                   const double initial_guess[16], int apply_intersection_filter, float fitness_score_thre,
+                   const double target_bound[6], const double source_bound[6], mulls_gicp_result *out, mulls_gicp_iter *trace,
+                   int trace_cap) {
+    return front_call(ctx, [&](uint64_t &launches) {
+        return gicp_impl(ctx, target, source, using_voxel_gicp, voxel_size, initial_guess, apply_intersection_filter,
+                         fitness_score_thre, target_bound, source_bound, out, trace, trace_cap, launches);
     });
 }
 

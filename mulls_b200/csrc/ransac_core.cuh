@@ -168,20 +168,30 @@ inline void rc_sums_serial(int M, Member in, Value v, double out[K]) {
 }
 
 // ---- R3: Eigen 3.3's JacobiSVD of a 3x3 double (ComputeFullU | ComputeFullV) ----------------------------------------------
-template <int N>
-GF_HD void rc_rot_rows(double (*A)[N], int p, int q, double c, double s) { // A.applyOnTheLeft(p, q, J(c, s))
-    if (c == 1.0 && s == 0.0) return;
+// the limits of JacobiSVD's scalar (R3)
+template <class T> struct rc_lim;
+template <> struct rc_lim<double> {
+    GF_HD static double min() { return DBL_MIN; }
+    GF_HD static double eps() { return DBL_EPSILON; }
+};
+template <> struct rc_lim<float> {
+    GF_HD static float min() { return FLT_MIN; }
+    GF_HD static float eps() { return FLT_EPSILON; }
+};
+template <int N, class T = double>
+GF_HD void rc_rot_rows(T (*A)[N], int p, int q, T c, T s) { // A.applyOnTheLeft(p, q, J(c, s))
+    if (c == T(1) && s == T(0)) return;
     for (int i = 0; i < N; ++i) {
-        const double x = A[p][i], y = A[q][i];
+        const T x = A[p][i], y = A[q][i];
         A[p][i] = c * x + s * y;
         A[q][i] = -s * x + c * y;
     }
 }
-template <int N>
-GF_HD void rc_rot_cols(double (*A)[N], int p, int q, double c, double s) { // apply_rotation_in_the_plane(col p, col q, J(c, s))
-    if (c == 1.0 && s == 0.0) return;
+template <int N, class T = double>
+GF_HD void rc_rot_cols(T (*A)[N], int p, int q, T c, T s) { // apply_rotation_in_the_plane(col p, col q, J(c, s))
+    if (c == T(1) && s == T(0)) return;
     for (int i = 0; i < N; ++i) {
-        const double x = A[i][p], y = A[i][q];
+        const T x = A[i][p], y = A[i][q];
         A[i][p] = c * x + s * y;
         A[i][q] = -s * x + c * y;
     }
@@ -190,23 +200,25 @@ GF_HD double rc_det3(const double m[3][3]) {
     return m[0][0] * (m[1][1] * m[2][2] - m[1][2] * m[2][1]) - m[0][1] * (m[1][0] * m[2][2] - m[1][2] * m[2][0]) +
            m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]);
 }
-// Eigen 3.3's two-sided JacobiSVD of a square N x N double (no QR preconditioner for a square matrix). sv: the singular
-// values, descending; the return value is m_nonzeroSingularValues (the sort stops at the first zero maximum).
-template <int N>
-GF_HD int rc_svd(const double (*A)[N], double (*U)[N], double (*V)[N], double sv[N]) {
-    double scale = 0.0;
+// Eigen 3.3's two-sided JacobiSVD of a square N x N matrix of T = double or float (no QR preconditioner for a square
+// matrix): JacobiSVD<Matrix<T, N, N>> is one template over the scalar, with its limits (considerAsZero = min(),
+// precision = 2 epsilon()) and every operation in T. sv: the singular values, descending; the return value is
+// m_nonzeroSingularValues (the sort stops at the first zero maximum).
+template <int N, class T = double>
+GF_HD int rc_svd(const T (*A)[N], T (*U)[N], T (*V)[N], T sv[N]) {
+    T scale = T(0);
     for (int i = 0; i < N; ++i)
         for (int j = 0; j < N; ++j)
             if (fabs(A[i][j]) > scale) scale = fabs(A[i][j]);
-    if (scale == 0.0) scale = 1.0;
-    double W[N][N];
+    if (scale == T(0)) scale = T(1);
+    T W[N][N];
     for (int i = 0; i < N; ++i)
         for (int j = 0; j < N; ++j) {
             W[i][j] = A[i][j] / scale;
-            U[i][j] = V[i][j] = (i == j) ? 1.0 : 0.0;
+            U[i][j] = V[i][j] = (i == j) ? T(1) : T(0);
         }
-    const double considerAsZero = DBL_MIN, precision = 2.0 * DBL_EPSILON;
-    double maxDiag = fabs(W[0][0]);
+    const T considerAsZero = rc_lim<T>::min(), precision = T(2) * rc_lim<T>::eps();
+    T maxDiag = fabs(W[0][0]);
     for (int i = 1; i < N; ++i)
         if (maxDiag < fabs(W[i][i])) maxDiag = fabs(W[i][i]);
     bool finished = false;
@@ -214,50 +226,50 @@ GF_HD int rc_svd(const double (*A)[N], double (*U)[N], double (*V)[N], double sv
         finished = true;
         for (int p = 1; p < N; ++p)
             for (int q = 0; q < p; ++q) {
-                const double threshold = (considerAsZero < precision * maxDiag) ? precision * maxDiag : considerAsZero;
+                const T threshold = (considerAsZero < precision * maxDiag) ? precision * maxDiag : considerAsZero;
                 if (!(fabs(W[p][q]) > threshold || fabs(W[q][p]) > threshold)) continue;
                 finished = false;
                 // real_2x2_jacobi_svd
-                double m00 = W[p][p], m01 = W[p][q], m10 = W[q][p], m11 = W[q][q];
-                double c1 = 1.0, s1 = 0.0;
-                const double t = m00 + m11, d = m10 - m01;
-                if (!(fabs(d) < DBL_MIN)) {
-                    const double u = t / d, tmp = sqrt(1.0 + u * u);
-                    s1 = 1.0 / tmp;
+                T m00 = W[p][p], m01 = W[p][q], m10 = W[q][p], m11 = W[q][q];
+                T c1 = T(1), s1 = T(0);
+                const T t = m00 + m11, d = m10 - m01;
+                if (!(fabs(d) < rc_lim<T>::min())) {
+                    const T u = t / d, tmp = sqrt(T(1) + u * u);
+                    s1 = T(1) / tmp;
                     c1 = u / tmp;
                 }
-                if (!(c1 == 1.0 && s1 == 0.0)) {
-                    const double a0 = c1 * m00 + s1 * m10, a1 = c1 * m01 + s1 * m11;
-                    const double b0 = -s1 * m00 + c1 * m10, b1 = -s1 * m01 + c1 * m11;
+                if (!(c1 == T(1) && s1 == T(0))) {
+                    const T a0 = c1 * m00 + s1 * m10, a1 = c1 * m01 + s1 * m11;
+                    const T b0 = -s1 * m00 + c1 * m10, b1 = -s1 * m01 + c1 * m11;
                     m00 = a0, m01 = a1, m10 = b0, m11 = b1;
                 }
                 (void)m10;
                 // j_right.makeJacobi(m00, m01, m11)
-                double cr = 1.0, sr = 0.0;
-                const double deno = 2.0 * fabs(m01);
-                if (!(deno < DBL_MIN)) {
-                    const double tau = (m00 - m11) / deno, w = sqrt(tau * tau + 1.0);
-                    const double tt = (tau > 0.0) ? 1.0 / (tau + w) : 1.0 / (tau - w);
-                    const double sign_t = tt > 0.0 ? 1.0 : -1.0;
-                    const double n = 1.0 / sqrt(tt * tt + 1.0);
+                T cr = T(1), sr = T(0);
+                const T deno = T(2) * fabs(m01);
+                if (!(deno < rc_lim<T>::min())) {
+                    const T tau = (m00 - m11) / deno, w = sqrt(tau * tau + T(1));
+                    const T tt = (tau > T(0)) ? T(1) / (tau + w) : T(1) / (tau - w);
+                    const T sign_t = tt > T(0) ? T(1) : -T(1);
+                    const T n = T(1) / sqrt(tt * tt + T(1));
                     sr = ((-sign_t * (m01 / fabs(m01))) * fabs(tt)) * n;
                     cr = n;
                 }
                 // j_left = rot1 * j_right.transpose(), j_right.transpose() = (cr, -sr)
-                const double cl = c1 * cr - s1 * -sr, sl = c1 * -sr + s1 * cr;
-                rc_rot_rows<N>(W, p, q, cl, sl);   // m_workMatrix.applyOnTheLeft(p, q, j_left)
-                rc_rot_cols<N>(U, p, q, cl, sl);   // m_matrixU.applyOnTheRight(p, q, j_left.transpose())
-                rc_rot_cols<N>(W, p, q, cr, -sr);  // m_workMatrix.applyOnTheRight(p, q, j_right)
-                rc_rot_cols<N>(V, p, q, cr, -sr);  // m_matrixV.applyOnTheRight(p, q, j_right)
-                const double dp = fabs(W[p][p]), dq = fabs(W[q][q]);
-                const double dm = (dp < dq) ? dq : dp;
+                const T cl = c1 * cr - s1 * -sr, sl = c1 * -sr + s1 * cr;
+                rc_rot_rows<N, T>(W, p, q, cl, sl);   // m_workMatrix.applyOnTheLeft(p, q, j_left)
+                rc_rot_cols<N, T>(U, p, q, cl, sl);   // m_matrixU.applyOnTheRight(p, q, j_left.transpose())
+                rc_rot_cols<N, T>(W, p, q, cr, -sr);  // m_workMatrix.applyOnTheRight(p, q, j_right)
+                rc_rot_cols<N, T>(V, p, q, cr, -sr);  // m_matrixV.applyOnTheRight(p, q, j_right)
+                const T dp = fabs(W[p][p]), dq = fabs(W[q][q]);
+                const T dm = (dp < dq) ? dq : dp;
                 if (maxDiag < dm) maxDiag = dm;
             }
     }
     for (int i = 0; i < N; ++i) {
-        const double a = W[i][i];
+        const T a = W[i][i];
         sv[i] = fabs(a);
-        if (a < 0.0)
+        if (a < T(0))
             for (int r = 0; r < N; ++r) U[r][i] = -U[r][i];
     }
     for (int i = 0; i < N; ++i) sv[i] *= scale;
@@ -266,15 +278,15 @@ GF_HD int rc_svd(const double (*A)[N], double (*U)[N], double (*V)[N], double sv
         int pos = i;
         for (int j = i + 1; j < N; ++j)
             if (sv[j] > sv[pos]) pos = j;
-        if (sv[pos] == 0.0) {
+        if (sv[pos] == T(0)) {
             nonzero = i;
             break;
         }
         if (pos != i) {
-            const double ts = sv[i];
+            const T ts = sv[i];
             sv[i] = sv[pos], sv[pos] = ts;
             for (int r = 0; r < N; ++r) {
-                double x = U[r][i];
+                T x = U[r][i];
                 U[r][i] = U[r][pos], U[r][pos] = x;
                 x = V[r][i];
                 V[r][i] = V[r][pos], V[r][pos] = x;

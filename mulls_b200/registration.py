@@ -400,6 +400,46 @@ class Context:
                                 reversed=np.array([tr[i].reversed for i in range(k)], np.int32))
         return out
 
+    def omp_gicp(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, max_iter_num: int = 20,
+                 dis_thre_unit: float = 1.5, using_voxel_gicp: bool = True, voxel_size: float = 1.0, initial_guess=None,
+                 apply_intersection_filter: bool = False, fitness_score_thre: float = 10.0, trace_cap: int = 0):
+        """CRegistration::omp_gicp (cregistration.hpp:1024-1098, FastVGICP) on the GPU: target / source are block1 /
+        block2 ->pc_down ((n, 3), (n, 7) or (n, 12) rows), the bounds their local_bound. max_iter_num and dis_thre_unit
+        are accepted and ignored, as the reference ignores them. The walk draws from the process's rand() where the
+        reference does. Returns a dict: code (1, or -3 when the fitness exceeds fitness_score_thre), trans (Trans1_2,
+        (4, 4) float64), iterations, converged, fitness, n_target / n_source after the prologue, x0 (the start point),
+        and with trace_cap > 0 `trace`: per step the point x (6), the step delta (6), the correspondence count and
+        whether the step was the random fallback. using_voxel_gicp=False raises. Replaces the resident batch."""
+        del max_iter_num, dis_thre_unit  # not read by FastVGICP
+
+        def aos48(c):  # (n, 3) xyz rows are accepted too: GICP reads positions only
+            c = np.asarray(c, np.float32)
+            if c.ndim == 2 and c.shape[1] == 3:
+                c = np.concatenate([c, np.zeros((len(c), 9), np.float32)], axis=1)
+            return abi.as_aos48(c)
+
+        t, s = aos48(target), aos48(source)
+        g = np.ascontiguousarray(np.eye(4) if initial_guess is None else initial_guess, np.float64).reshape(16).copy()
+        tb = np.ascontiguousarray(target_bound, np.float64).reshape(6).copy()
+        sb = np.ascontiguousarray(source_bound, np.float64).reshape(6).copy()
+        res = abi.GicpResult()
+        tr = (abi.GicpIter * max(int(trace_cap), 1))()
+        dp = C.POINTER(C.c_double)
+        self._check(self.lib.mulls_omp_gicp(self.handle, abi.cloud_view(t), abi.cloud_view(s), int(bool(using_voxel_gicp)),
+                                            float(voxel_size), g.ctypes.data_as(dp), int(bool(apply_intersection_filter)),
+                                            float(fitness_score_thre), tb.ctypes.data_as(dp), sb.ctypes.data_as(dp),
+                                            C.byref(res), tr, int(trace_cap)))
+        out = dict(code=res.code, trans=np.array(res.trans[:], np.float64).reshape(4, 4), iterations=res.iterations,
+                   converged=bool(res.converged), fitness=res.fitness, n_target=res.n_target, n_source=res.n_source,
+                   x0=np.array(res.x0[:], np.float32))
+        if trace_cap > 0:
+            k = min(res.iterations, int(trace_cap))
+            out["trace"] = dict(x=np.array([tr[i].x[:] for i in range(k)], np.float32).reshape(k, 6),
+                                delta=np.array([tr[i].delta[:] for i in range(k)], np.float32).reshape(k, 6),
+                                n_corr=np.array([tr[i].n_corr for i in range(k)], np.int32),
+                                random_step=np.array([tr[i].random_step for i in range(k)], np.int32))
+        return out
+
     def non_max_suppress(self, cloud: np.ndarray, non_max_radius: float):
         """CFilter::non_max_suppress(cloud_in_out, non_max_radius) (cfilter.hpp:1183-1240) on the GPU. Returns
         (kept_idx, performed): kept_idx is an int32 array of the input rows the reference leaves in the cloud, in its
@@ -580,6 +620,15 @@ class CRegistration:
         block2 = source with their local_bounds. Only the DIRECT7 search (use_direct_search=True) runs here."""
         r = self._ctx.omp_ndt(target, source, target_bound, source_bound, ndt_resolution, use_direct_search, initial_guess,
                               apply_intersection_filter, fitness_score_thre)
+        return r["code"], r["trans"]
+
+    def omp_gicp(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, max_iter_num: int = 20,
+                 dis_thre_unit: float = 1.5, using_voxel_gicp: bool = True, voxel_size: float = 1.0, initial_guess=None,
+                 apply_intersection_filter: bool = False, fitness_score_thre: float = 10.0):
+        """lo::CRegistration::omp_gicp (cregistration.hpp:1024-1098): returns (code, Trans1_2) for block1 = target and
+        block2 = source with their local_bounds. Only the voxelized GICP (using_voxel_gicp=True) runs here."""
+        r = self._ctx.omp_gicp(target, source, target_bound, source_bound, max_iter_num, dis_thre_unit, using_voxel_gicp,
+                               voxel_size, initial_guess, apply_intersection_filter, fitness_score_thre)
         return r["code"], r["trans"]
 
     def mm_lls_icp_4dof_global(self, registration_con: Constraint, heading_step_d: float, max_iter_num: int = 20,
