@@ -309,6 +309,50 @@ int omp_ndt(constraint_t &registration_cons, float ndt_resolution = 1.0, Eigen::
     return res.code;
 }
 
+// omp_ndt over every constraint of registration_cons in one call (mulls_omp_ndt_batch), with the arguments of the
+// reference's omp_ndt in its order and with its defaults, shared by all constraints. Each Trans1_2 is written and each
+// code returned as omp_ndt above would for that constraint alone. A library error (use_direct_search = false included:
+// the reference has no batch member to hand KDTREE to) is logged and returns -3 for every constraint, with every
+// Trans1_2 left as it was.
+template <typename PointT>
+std::vector<int> omp_ndt_batch(std::vector<constraint_t> &registration_cons, float ndt_resolution = 1.0,
+                               bool use_direct_search = true, Eigen::Matrix4d initial_guess = Eigen::Matrix4d::Identity(),
+                               bool apply_intersection_filter = true, float fitness_score_thre = 10.0) {
+    const size_t n = registration_cons.size();
+    std::vector<int> codes(n, -3);
+    if (n == 0) return codes;
+    std::vector<mulls_cloud_view> tv(n), sv(n);
+    std::vector<double> guess(16 * n), tb(6 * n), sb(6 * n);
+    size_t max_t = 0, max_s = 0;
+    for (size_t i = 0; i < n; ++i) {
+        const constraint_t &con = registration_cons[i];
+        tv[i] = view_of<PointT>(con.block1->pc_down), sv[i] = view_of<PointT>(con.block2->pc_down);
+        max_t = std::max(max_t, tv[i].n), max_s = std::max(max_s, sv[i].n);
+        for (int r = 0; r < 4; ++r)
+            for (int c = 0; c < 4; ++c) guess[16 * i + 4 * r + c] = initial_guess(r, c);
+        const bounds_t &b1 = con.block1->local_bound, &b2 = con.block2->local_bound;
+        const double tb_[6] = {b1.min_x, b1.min_y, b1.min_z, b1.max_x, b1.max_y, b1.max_z};
+        const double sb_[6] = {b2.min_x, b2.min_y, b2.min_z, b2.max_x, b2.max_y, b2.max_z};
+        std::memcpy(&tb[6 * i], tb_, sizeof(tb_));
+        std::memcpy(&sb[6 * i], sb_, sizeof(sb_));
+    }
+    std::vector<mulls_ndt_result> res(n);
+    mulls_ctx *ctx = thread_batch_context(n, max_s, max_t);
+    if (!ctx || mulls_omp_ndt_batch(ctx, n, tv.data(), sv.data(), ndt_resolution, use_direct_search ? 1 : 0, guess.data(),
+                                    apply_intersection_filter ? 1 : 0, fitness_score_thre, tb.data(), sb.data(), res.data(),
+                                    nullptr, 0) != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return codes;
+    }
+    for (size_t i = 0; i < n; ++i) {
+        LOG(INFO) << "fitness score: " << res[i].fitness; // base_align, :779
+        for (int r = 0; r < 4; ++r)
+            for (int c = 0; c < 4; ++c) registration_cons[i].Trans1_2(r, c) = res[i].trans[4 * r + c];
+        codes[i] = res[i].code;
+    }
+    return codes;
+}
+
 // lo::CRegistration<PointT>::omp_gicp (cregistration.hpp:1024-1098) with using_voxel_gicp (FastVGICP), same arguments
 // and defaults but the two FastVGICP never reads (max_iter_num, dis_thre_unit; test/mulls_slam.cpp:637-639, :674-676):
 // target = block1->pc_down, source = block2->pc_down, their local_bounds, on the device (mulls_omp_gicp, readings in

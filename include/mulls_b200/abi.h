@@ -40,6 +40,7 @@
  *   mulls_coarse_reg_ransac  <- lo::CRegistration<PointT>::coarse_reg_ransac, cregistration.hpp:604-661
  *   mulls_non_max_suppress   <- lo::CFilter<PointT>::non_max_suppress(cloud_in_out, non_max_radius), cfilter.hpp:1183-1240
  *   mulls_omp_ndt            <- lo::CRegistration<PointT>::omp_ndt with use_direct_search (DIRECT7), cregistration.hpp:945-1021
+ *   mulls_omp_ndt_batch      <- P independent omp_ndt calls with shared parameters, in one call
  *   mulls_omp_gicp           <- lo::CRegistration<PointT>::omp_gicp with using_voxel_gicp (FastVGICP), cregistration.hpp:1024-1098
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
@@ -644,6 +645,23 @@ int mulls_omp_ndt(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view sour
                   const double initial_guess[16] /* row-major */, int apply_intersection_filter, float fitness_score_thre,
                   const double target_bound[6], const double source_bound[6], mulls_ndt_result *out, mulls_ndt_iter *trace,
                   int trace_cap);
+
+/* A batch of NDT registrations: n_pairs independent mulls_omp_ndt calls in one. ndt_resolution, use_direct_search,
+ * apply_intersection_filter and fitness_score_thre are shared by the batch (as the driver's flags are); pair i has its
+ * target and source views, initial_guesses[16 i .. 16 i + 15] (row-major), target_bounds[6 i ..] and source_bounds[6 i ..].
+ * out[i] and trace[i * trace_cap ..] (up to trace_cap iterations; may be NULL with trace_cap 0) receive what
+ * mulls_omp_ndt returns for pair i alone with the same parameters, bit for bit: code, iterations, converged, n_target,
+ * n_source, every bit of trans and fitness, every trace row. The pairs' walks run in lockstep on the host: each
+ * iteration evaluates every pair whose walk has not ended in one launch and downloads their terms at once.
+ * Refusals, with the pair named in mulls_last_error where one pair is the cause; a refused batch writes no result:
+ * use_direct_search = 0: MULLS_E_UNSUPPORTED. n_pairs above the context's max_pairs, or a pair whose target exceeds
+ * max_tgt_pts or whose source exceeds max_src_pts: MULLS_E_CAPACITY. n_pairs = 0, a NULL array, NULL rows with n > 0
+ * or ndt_resolution <= 0: MULLS_E_ARG. The call replaces the resident batch, as mulls_omp_ndt does. */
+int mulls_omp_ndt_batch(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *targets, const mulls_cloud_view *sources,
+                        float ndt_resolution, int use_direct_search, const double *initial_guesses /* [16 n_pairs] */,
+                        int apply_intersection_filter, float fitness_score_thre, const double *target_bounds /* [6 n_pairs] */,
+                        const double *source_bounds /* [6 n_pairs] */, mulls_ndt_result *out /* [n_pairs] */,
+                        mulls_ndt_iter *trace /* [n_pairs * trace_cap] */, int trace_cap);
 
 /* Voxelized GICP registration: lo::CRegistration<PointT>::omp_gicp(reg_con, max_iter_num, dis_thre_unit, using_voxel_gicp,
  * voxel_size, initial_guess, apply_intersection_filter, fitness_score_thre) (cregistration.hpp:1024-1098) with

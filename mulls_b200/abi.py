@@ -331,6 +331,7 @@ EXPORTED_SYMBOLS = (
     "mulls_coarse_reg_ransac",
     "mulls_non_max_suppress",
     "mulls_omp_ndt",
+    "mulls_omp_ndt_batch",
     "mulls_omp_gicp",
     "mulls_scan_probe",
     "mulls_scan_read",
@@ -421,6 +422,10 @@ def load_library() -> C.CDLL:
     lib.mulls_omp_ndt.restype = C.c_int
     lib.mulls_omp_ndt.argtypes = [vp, CloudView, CloudView, C.c_float, C.c_int, C.POINTER(C.c_double), C.c_int, C.c_float,
                                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(NdtResult), C.POINTER(NdtIter), C.c_int]
+    lib.mulls_omp_ndt_batch.restype = C.c_int
+    lib.mulls_omp_ndt_batch.argtypes = [vp, C.c_size_t, C.POINTER(CloudView), C.POINTER(CloudView), C.c_float, C.c_int,
+                                        C.POINTER(C.c_double), C.c_int, C.c_float, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                        C.POINTER(NdtResult), C.POINTER(NdtIter), C.c_int]
     lib.mulls_omp_gicp.restype = C.c_int
     lib.mulls_omp_gicp.argtypes = [vp, CloudView, CloudView, C.c_int, C.c_float, C.POINTER(C.c_double), C.c_int, C.c_float,
                                    C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(GicpResult), C.POINTER(GicpIter),

@@ -85,6 +85,8 @@ struct PackJob {
     size_t first, count;
     int fmt;
     std::atomic<int> *pending; // decremented when the job is done
+    void (*task)(void *) = nullptr; // set: the job runs task(arg) instead of packing rows
+    void *arg = nullptr;
 };
 
 class PackPool {
@@ -142,8 +144,11 @@ class PackPool {
 
   private:
     static void run(const PackJob &j) {
-        pack_rows(j.rows, j.first, j.count, j.fmt, j.pos, j.nrm);
-        _mm_sfence(); // the streaming stores must be visible before the DMA is queued
+        if (j.task) j.task(j.arg);
+        else {
+            pack_rows(j.rows, j.first, j.count, j.fmt, j.pos, j.nrm);
+            _mm_sfence(); // the streaming stores must be visible before the DMA is queued
+        }
         j.pending->fetch_sub(1, std::memory_order_release);
     }
     void worker() {

@@ -56,14 +56,36 @@ struct NdtEvalArgs {
     double *tile_sums; // [tiles][kNdtTerms]
 };
 
-__device__ __forceinline__ int ndt_find_leaf(const uint64_t *keys, int n, uint64_t key) {
-    int lo = 0, hi = n;
+// the leaf of `key` among keys[lo, hi) (ascending), -1 when there is none
+__device__ __forceinline__ int ndt_find_leaf(const uint64_t *keys, int lo, int hi, uint64_t key) {
+    const int n = hi;
     while (lo < hi) {
         const int mid = (lo + hi) >> 1;
         if (keys[mid] < key) lo = mid + 1;
         else hi = mid;
     }
     return (lo < n && keys[lo] == key) ? lo : -1;
+}
+__device__ __forceinline__ int ndt_find_leaf(const uint64_t *keys, int n, uint64_t key) { return ndt_find_leaf(keys, 0, n, key); }
+
+// N4 for source point p: transform, the 7 probes among the leaves keys[lo, hi) (each key carries `key_hi` above the
+// leaf index: the pair in a batch, 0 for one pair), ndt_update per neighbour into acc
+__device__ __forceinline__ void ndt_point_terms(float4 p, const NdtGrid &g, const uint64_t *keys, uint64_t key_hi, int lo, int hi,
+                                                const NdtLeaf *leaves, const NdtEvalConst &E, double (&acc)[kNdtTerms]) {
+    if (!ndt_finite3(p.x, p.y, p.z)) return;
+    const float x[3] = {p.x, p.y, p.z};
+    float t[3];
+    ndt_transform(E.T, p.x, p.y, p.z, t);
+    if (!ndt_finite3(t[0], t[1], t[2])) return;
+    for (int k = 0; k < 7; ++k) {
+        int64_t key;
+        if (!ndt_probe_key(g, t[0], t[1], t[2], k, key)) continue;
+        const int l = ndt_find_leaf(keys, lo, hi, key_hi | (uint64_t)key);
+        if (l < 0 || !leaves[l].ok) continue;
+        const NdtLeaf &L = leaves[l];
+        const double xt[3] = {(double)t[0] - L.mean[0], (double)t[1] - L.mean[1], (double)t[2] - L.mean[2]};
+        ndt_update(E, x, xt, L.icov, acc);
+    }
 }
 
 // C1 of ndt_core.cuh over one block of kNdtTile threads, each holding its point's kTerms sums in acc: the pairwise tree
@@ -98,25 +120,7 @@ __global__ void __launch_bounds__(kNdtTile) k_ndt_eval(NdtEvalArgs A, NdtEvalCon
     double acc[kNdtTerms];
 #pragma unroll
     for (int c = 0; c < kNdtTerms; ++c) acc[c] = 0.0;
-    if (i < A.n_src && A.g.ok) {
-        const float4 p = A.src[i];
-        if (ndt_finite3(p.x, p.y, p.z)) {
-            const float x[3] = {p.x, p.y, p.z};
-            float t[3];
-            ndt_transform(E.T, p.x, p.y, p.z, t);
-            const int nl = *A.n_leaves;
-            if (ndt_finite3(t[0], t[1], t[2]))
-                for (int k = 0; k < 7; ++k) {
-                    int64_t key;
-                    if (!ndt_probe_key(A.g, t[0], t[1], t[2], k, key)) continue;
-                    const int l = ndt_find_leaf(A.leaf_keys, nl, (uint64_t)key);
-                    if (l < 0 || !A.leaves[l].ok) continue;
-                    const NdtLeaf &L = A.leaves[l];
-                    const double xt[3] = {(double)t[0] - L.mean[0], (double)t[1] - L.mean[1], (double)t[2] - L.mean[2]};
-                    ndt_update(E, x, xt, L.icov, acc);
-                }
-        }
-    }
+    if (i < A.n_src && A.g.ok) ndt_point_terms(A.src[i], A.g, A.leaf_keys, 0, 0, *A.n_leaves, A.leaves, E, acc);
     tile_tree_store<kNdtTerms>(acc, A.tile_sums);
 }
 
@@ -139,6 +143,139 @@ __global__ void __launch_bounds__(128) k_ndt_fitness(DeviceArrays A, const float
     float r = -1.f;
     if (ndt_finite3(p.x, p.y, p.z) && ndt_finite3(t[0], t[1], t[2]) && A.ps[0].n_tgt[0] > 0 && !A.hash_used[1]) {
         const GridView g = grid_of(A, A.pc[0], A.ps[0], 0);
+        KnnList<1> kl;
+        knn_search(g, t[0], t[1], t[2], 1, 1, kl);
+        if (kl.n > 0) r = kl.d2[0];
+    }
+    d2[i] = r;
+}
+
+// ---- a batch of pairs (mulls_omp_ndt_batch) -------------------------------------------------------------------------
+// The leaves of all targets come from one sort: a pair's leaf index (below 2^31, N1) goes in the low 32 bits of the key
+// and the pair above it, so the stable sort keeps each leaf's points in input order and each pair's leaves are the one
+// pair's leaves, consecutive. The evaluation runs over the tiles of every live pair at once; a tile never spans two
+// pairs, so each pair's tile sums and their order are the one pair's (C1).
+struct NdtPairDev {
+    NdtGrid g;
+    int src_off, n_src;       // the pair's sources in the batch's source array
+    int tgt_off, n_tgt;       // its target points in the leaf build (n_tgt = 0 when the grid is not ok)
+    int leaf_begin, leaf_end; // its leaves among the sorted runs (k_ndt_leaf_ranges)
+};
+
+// a live pair of one evaluation launch: its constants and its tiles [tile_begin, tile_end) of the launch
+struct NdtLiveSlot {
+    NdtEvalConst E;
+    int pair, tile_begin, tile_end;
+};
+
+// the last of pairs[0, n) whose offset (member `off`) is <= i: the pair of element i (empty pairs share the offset of
+// the next one and are skipped)
+template <int NdtPairDev::*off>
+__device__ __forceinline__ int ndt_pair_of(const NdtPairDev *pairs, int n, int i) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (pairs[mid].*off <= i) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(kNdtKeyBlock) k_ndt_keys_batch(const float4 *__restrict__ tgt, int n, const NdtPairDev *__restrict__ pairs,
+                                                                 int n_pairs, uint64_t *__restrict__ keys, uint32_t *__restrict__ vals) {
+    const int i = blockIdx.x * kNdtKeyBlock + threadIdx.x;
+    if (i >= n) return;
+    const int p = ndt_pair_of<&NdtPairDev::tgt_off>(pairs, n_pairs, i);
+    const float4 q = tgt[i];
+    // a finite point inside its pair's min / max: the leaf index is in [0, 2^31) (N1)
+    keys[i] = ((uint64_t)p << 32) | (uint64_t)ndt_build_key(pairs[p].g, q.x, q.y, q.z);
+    vals[i] = (uint32_t)i;
+}
+
+// one thread per pair: its leaves among the n_runs sorted run keys
+__global__ void __launch_bounds__(64) k_ndt_leaf_ranges(const uint64_t *__restrict__ run_keys, const int *__restrict__ n_runs,
+                                                        NdtPairDev *__restrict__ pairs, int n_pairs) {
+    const int p = blockIdx.x * 64 + threadIdx.x;
+    if (p >= n_pairs) return;
+    const int n = *n_runs;
+    int b[2];
+    for (int e = 0; e < 2; ++e) {
+        const uint64_t key = (uint64_t)(p + e) << 32;
+        int lo = 0, hi = n;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (run_keys[mid] < key) lo = mid + 1;
+            else hi = mid;
+        }
+        b[e] = lo;
+    }
+    pairs[p].leaf_begin = b[0], pairs[p].leaf_end = b[1];
+}
+
+struct NdtBatchEvalArgs {
+    const float4 *src;
+    const NdtPairDev *pairs;
+    const uint64_t *leaf_keys;
+    const NdtLeaf *leaves;
+    const NdtLiveSlot *slots;
+    int n_slots;
+    double *tile_sums; // [launch tiles][kNdtTerms]
+};
+
+__global__ void __launch_bounds__(kNdtTile) k_ndt_eval_batch(NdtBatchEvalArgs A) {
+    __shared__ NdtEvalConst s_E;
+    __shared__ int s_slot;
+    if (threadIdx.x == 0) {
+        int lo = 0, hi = A.n_slots - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (A.slots[mid].tile_begin <= (int)blockIdx.x) lo = mid;
+            else hi = mid - 1;
+        }
+        s_slot = lo;
+    }
+    __syncthreads();
+    const NdtLiveSlot *S = A.slots + s_slot;
+    static_assert(sizeof(NdtEvalConst) % 4 == 0, "copied as words");
+    for (int w = threadIdx.x; w < (int)(sizeof(NdtEvalConst) / 4); w += kNdtTile)
+        reinterpret_cast<int *>(&s_E)[w] = reinterpret_cast<const int *>(&S->E)[w];
+    __syncthreads();
+    const int pair = S->pair;
+    const NdtPairDev &P = A.pairs[pair];
+    const int i = ((int)blockIdx.x - S->tile_begin) * kNdtTile + threadIdx.x;
+    double acc[kNdtTerms];
+#pragma unroll
+    for (int c = 0; c < kNdtTerms; ++c) acc[c] = 0.0;
+    if (i < P.n_src && P.g.ok)
+        ndt_point_terms(A.src[P.src_off + i], P.g, A.leaf_keys, (uint64_t)pair << 32, P.leaf_begin, P.leaf_end, A.leaves, s_E, acc);
+    tile_tree_store<kNdtTerms>(acc, A.tile_sums);
+}
+
+// block s, thread c: live slot s's tiles summed in tile order (k_ndt_tiles per pair) into out[s][c]
+__global__ void __launch_bounds__(64) k_ndt_tiles_batch(const double *__restrict__ tile_sums, const NdtLiveSlot *__restrict__ slots,
+                                                        double *__restrict__ out) {
+    const int c = threadIdx.x;
+    if (c >= kNdtTerms) return;
+    const int b = slots[blockIdx.x].tile_begin, e = slots[blockIdx.x].tile_end;
+    double s = 0.0;
+    for (int t = b; t < e; ++t) s += tile_sums[(size_t)t * kNdtTerms + c];
+    out[(size_t)blockIdx.x * kNdtTerms + c] = s;
+}
+
+// k_ndt_fitness over the sources of all pairs, each moved by its pair's final transform T[pair] and searched in its
+// pair's grid (pair p of the ingest's batch)
+__global__ void __launch_bounds__(128) k_ndt_fitness_batch(DeviceArrays A, const float4 *__restrict__ src, int n,
+                                                           const NdtPairDev *__restrict__ pairs, int n_pairs,
+                                                           const float *__restrict__ T, float *__restrict__ d2) {
+    const int i = blockIdx.x * 128 + threadIdx.x;
+    if (i >= n) return;
+    const int p = ndt_pair_of<&NdtPairDev::src_off>(pairs, n_pairs, i);
+    const float4 q = src[i];
+    float t[3];
+    ndt_transform(T + 12 * p, q.x, q.y, q.z, t);
+    float r = -1.f;
+    if (ndt_finite3(q.x, q.y, q.z) && ndt_finite3(t[0], t[1], t[2]) && A.ps[p].n_tgt[0] > 0 && !A.hash_used[1]) {
+        const GridView g = grid_of(A, A.pc[p], A.ps[p], 0);
         KnnList<1> kl;
         knn_search(g, t[0], t[1], t[2], 1, 1, kl);
         if (kl.n > 0) r = kl.d2[0];

@@ -1356,8 +1356,9 @@ static int check_capacity(mulls_ctx *ctx, size_t n, const char *fn) {
 // finite_only keeps points with a non-finite coordinate out of the bbox and the grid. The grid must fit the hash pool
 // before a kernel reads it: else the pool grows and the grid is built again from the cloud already in HBM (it fits by
 // construction). `A` receives the device arrays, n_tgt the count of target points in the grid.
-static int ingest_cloud(mulls_ctx *ctx, mulls_cloud_view cloud, bool on_device, float radius, bool full_pyramid,
-                        bool finite_only, DeviceArrays &A, int &n_tgt, uint64_t &launches) {
+// ingest_clouds: the same for n host clouds at once, cloud i as the target of pair i (n_tgt is pair 0's count).
+static int ingest_clouds(mulls_ctx *ctx, size_t n, const mulls_cloud_view *clouds, bool on_device, float radius,
+                         bool full_pyramid, bool finite_only, DeviceArrays &A, int &n_tgt, uint64_t &launches) {
     mulls_icp_params P;
     mulls_icp_default_params(&P);
     std::strcpy(P.used_feature_type, "100000");
@@ -1365,10 +1366,14 @@ static int ingest_cloud(mulls_ctx *ctx, mulls_cloud_view cloud, bool on_device, 
     if (radius > 0.f) P.dis_thre_unit = radius;
     if (full_pyramid) P.normal_shooting_on = 1;
     P.max_iter_num = 0;
-    mulls_cloud_view tgt[MULLS_NUM_CLASSES] = {cloud, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
-    mulls_cloud_view src[MULLS_NUM_CLASSES] = {{nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}, {nullptr, 0}};
-    const double ident[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    int rc = upload_impl(ctx, 1, tgt, src, &P, ident, nullptr, nullptr, /*resident=*/false, on_device);
+    std::vector<mulls_icp_params> params(n, P);
+    std::vector<mulls_cloud_view> tgt(n * MULLS_NUM_CLASSES, mulls_cloud_view{nullptr, 0}), src(tgt);
+    std::vector<double> ident(16 * n, 0.0);
+    for (size_t i = 0; i < n; ++i) {
+        tgt[i * MULLS_NUM_CLASSES] = clouds[i];
+        for (int d = 0; d < 4; ++d) ident[16 * i + 5 * d] = 1.0;
+    }
+    int rc = upload_impl(ctx, n, tgt.data(), src.data(), params.data(), ident.data(), nullptr, nullptr, /*resident=*/false, on_device);
     ctx->uploaded = false;
     if (rc != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
@@ -1385,6 +1390,10 @@ static int ingest_cloud(mulls_ctx *ctx, mulls_cloud_view cloud, bool on_device, 
         if ((rc = launch_ingest(ctx, A, false, launches, nullptr, nullptr, finite_only)) != MULLS_OK) return rc;
     }
     return MULLS_OK;
+}
+static int ingest_cloud(mulls_ctx *ctx, mulls_cloud_view cloud, bool on_device, float radius, bool full_pyramid,
+                        bool finite_only, DeviceArrays &A, int &n_tgt, uint64_t &launches) {
+    return ingest_clouds(ctx, 1, &cloud, on_device, radius, full_pyramid, finite_only, A, n_tgt, launches);
 }
 
 // PCA features of one cloud (host rows, or rows already in HBM) into ctx->pca_buf; `args` receives the device arrays.
@@ -1985,29 +1994,35 @@ static int ingest_points(mulls_ctx *ctx, const std::vector<float4> &pts, DeviceA
     mulls_cloud_view cv{rows.data(), pts.size()};
     return ingest_cloud(ctx, cv, false, 0.f, true, true, A, n_in, launches);
 }
+// the host's share of the epilogue: the mean of the n distances d2 that count (DBL_MAX when none does), Trans1_2 and the code
+static void baseline_score(const float *d2, int n, const float T[12], const double *guess, bool moved, float fitness_thre,
+                           double trans[16], int &code, double &fitness) {
+    fitness = DBL_MAX;
+    double sum = 0.0;
+    int cnt = 0;
+    for (int i = 0; i < n; ++i)
+        if (d2[i] >= 0.f) sum += (double)d2[i], ++cnt;
+    if (cnt) fitness = sum / cnt;
+    ndt_epilogue(T, guess, moved, trans);
+    code = fitness > (double)fitness_thre ? -3 : 1;
+}
 // the epilogue: getFitnessScore (the exact unbounded nearest target of every moved source point, summed in index
 // order; DBL_MAX when nothing counts) over the target's grid A (NULL: no target), Trans1_2 and the code
 static int baseline_finish(mulls_ctx *ctx, const DeviceArrays *A, const float4 *d_s, int ns, float *d_d2, const float T[12],
                            const double *guess, bool moved, float fitness_thre, double trans[16], int &code, double &fitness,
                            uint64_t &launches) {
     cudaStream_t st = ctx->stream;
-    fitness = DBL_MAX;
+    std::vector<float> d2;
     if (A && ns > 0) {
         NdtEvalConst E;
         std::memcpy(E.T, T, sizeof(E.T));
         k_ndt_fitness<<<(unsigned)ceil_div(ns, 128), 128, 0, st>>>(*A, d_s, ns, E, d_d2);
         launches += 1;
-        std::vector<float> d2(ns);
+        d2.resize(ns);
         CK(cudaMemcpyAsync(d2.data(), d_d2, ns * sizeof(float), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
-        double sum = 0.0;
-        int cnt = 0;
-        for (int i = 0; i < ns; ++i)
-            if (d2[i] >= 0.f) sum += (double)d2[i], ++cnt;
-        if (cnt) fitness = sum / cnt;
     }
-    ndt_epilogue(T, guess, moved, trans);
-    code = fitness > (double)fitness_thre ? -3 : 1;
+    baseline_score(d2.data(), (int)d2.size(), T, guess, moved, fitness_thre, trans, code, fitness);
     return MULLS_OK;
 }
 
@@ -2115,6 +2130,216 @@ int mulls_omp_ndt(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view sour
     return front_call(ctx, [&](uint64_t &launches) {
         return ndt_impl(ctx, target, source, ndt_resolution, use_direct_search, initial_guess, apply_intersection_filter,
                         fitness_score_thre, target_bound, source_bound, out, trace, trace_cap, launches);
+    });
+}
+
+// A batch of NDT registrations with shared parameters (mulls_omp_ndt_batch): pair i computes what ndt_impl computes for
+// it alone. The prologues run on the host's worker pool; the leaves of all targets come from one sort
+// (k_ndt_keys_batch); every iteration evaluates all live pairs in one launch and downloads their 43 terms at once;
+// one ingest of all filtered targets and one fitness launch end the batch.
+struct NdtBatchPair {
+    mulls_cloud_view tv, sv;
+    const double *guess, *tbound, *sbound;
+    int apply_filter;
+    float resolution;
+    std::vector<float4> tgt, src;
+    bool moved = false;
+    NdtGrid g;
+    static void prologue(void *arg) {
+        NdtBatchPair &b = *(NdtBatchPair *)arg;
+        ndt_prologue(b.tv.aos48, b.tv.n, b.sv.aos48, b.sv.n, b.guess, b.apply_filter, b.tbound, b.sbound, b.tgt, b.src, b.moved);
+        b.g = ndt_grid_from(b.tgt, b.resolution);
+    }
+};
+static int ndt_batch_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *tv, const mulls_cloud_view *sv,
+                          float resolution, int use_direct_search, const double *guesses, int apply_filter, float fitness_thre,
+                          const double *tbounds, const double *sbounds, mulls_ndt_result *out, mulls_ndt_iter *trace,
+                          int trace_cap, uint64_t &launches) {
+    if (!out || !tv || !sv || !guesses || !tbounds || !sbounds || n_pairs == 0 || !(resolution > 0.f) || (trace_cap > 0 && !trace))
+        return MULLS_E_ARG;
+    const std::string fn = "mulls_omp_ndt_batch";
+    for (size_t p = 0; p < n_pairs; ++p)
+        if ((tv[p].n && !tv[p].aos48) || (sv[p].n && !sv[p].aos48)) {
+            ctx->err = fn + ": pair " + std::to_string(p) + ": NULL rows with n > 0";
+            return MULLS_E_ARG;
+        }
+    if (!use_direct_search) {
+        ctx->err = fn + ": only the DIRECT7 neighbour search runs on the device";
+        return MULLS_E_UNSUPPORTED;
+    }
+    if (n_pairs > ctx->max_pairs) {
+        ctx->err = fn + ": " + std::to_string(n_pairs) + " pairs exceed max_pairs of the context";
+        return MULLS_E_CAPACITY;
+    }
+    for (size_t p = 0; p < n_pairs; ++p)
+        if (tv[p].n > ctx->max_tgt || sv[p].n > ctx->max_src) {
+            ctx->err = fn + ": pair " + std::to_string(p) + ": " + std::to_string(tv[p].n) + " target / " +
+                       std::to_string(sv[p].n) + " source points exceed max_tgt_pts / max_src_pts of the context";
+            return MULLS_E_CAPACITY;
+        }
+    const int P = (int)n_pairs;
+    std::vector<NdtBatchPair> B(P);
+    { // the prologues on the worker pool
+        PackPool &pool = PackPool::get();
+        pool.ensure_workers(0);
+        std::atomic<int> pending(P);
+        std::vector<PackJob> jobs(P);
+        for (int p = 0; p < P; ++p) {
+            NdtBatchPair &b = B[p];
+            b.tv = tv[p], b.sv = sv[p], b.guess = guesses + 16 * p, b.tbound = tbounds + 6 * p, b.sbound = sbounds + 6 * p;
+            b.apply_filter = apply_filter, b.resolution = resolution;
+            jobs[p].pending = &pending;
+            jobs[p].task = &NdtBatchPair::prologue;
+            jobs[p].arg = &b;
+        }
+        pool.submit(jobs);
+        pool.help_until_done(pending);
+    }
+    // the pair table: sources of every pair, targets of the pairs with leaves, tiles of the evaluation
+    std::vector<NdtPairDev> pd(P);
+    std::vector<int> tile_off(P + 1, 0);
+    int nt_leaf = 0, ns_all = 0;
+    for (int p = 0; p < P; ++p) {
+        NdtPairDev &d = pd[p];
+        d.g = B[p].g;
+        d.src_off = ns_all, d.n_src = (int)B[p].src.size();
+        d.tgt_off = nt_leaf, d.n_tgt = d.g.ok ? (int)B[p].tgt.size() : 0;
+        d.leaf_begin = d.leaf_end = 0;
+        ns_all += d.n_src, nt_leaf += d.n_tgt;
+        tile_off[p + 1] = tile_off[p] + (int)ceil_div((size_t)d.n_src, kNdtTile);
+    }
+    const int tiles_all = tile_off[P];
+    cudaStream_t st = ctx->stream;
+    size_t cub_bytes = 0;
+    int rc;
+    if ((rc = sort_runs_bytes(ctx, nt_leaf, cub_bytes)) != MULLS_OK) return rc;
+    ScratchLayout L;
+    const size_t o_pd = L.take(P * sizeof(NdtPairDev)), o_sl = L.take(P * sizeof(NdtLiveSlot)), o_T = L.take(P * 12 * sizeof(float)),
+                 o_t = L.take(nt_leaf * sizeof(float4)), o_s = L.take(ns_all * sizeof(float4)), o_ka = L.take(nt_leaf * 8ull),
+                 o_kb = L.take(nt_leaf * 8ull), o_va = L.take(nt_leaf * 4ull), o_vb = L.take(nt_leaf * 4ull),
+                 o_uk = L.take(nt_leaf * 8ull), o_cnt = L.take(nt_leaf * 4ull), o_off = L.take(nt_leaf * 4ull),
+                 o_nr = L.take(sizeof(int)), o_lv = L.take(nt_leaf * sizeof(NdtLeaf)),
+                 o_ts = L.take((size_t)tiles_all * kNdtTerms * 8), o_out = L.take((size_t)P * kNdtTerms * 8),
+                 o_d2 = L.take(ns_all * sizeof(float)), o_cub = L.take(cub_bytes);
+    char *base;
+    if ((rc = L.grow(ctx, ctx->ndt_buf, base)) != MULLS_OK) return rc;
+    NdtPairDev *d_pd = (NdtPairDev *)(base + o_pd);
+    NdtLiveSlot *d_sl = (NdtLiveSlot *)(base + o_sl);
+    float *d_T = (float *)(base + o_T), *d_d2 = (float *)(base + o_d2);
+    float4 *d_t = (float4 *)(base + o_t), *d_s = (float4 *)(base + o_s);
+    uint64_t *d_ka = (uint64_t *)(base + o_ka), *d_kb = (uint64_t *)(base + o_kb), *d_uk = (uint64_t *)(base + o_uk);
+    uint32_t *d_va = (uint32_t *)(base + o_va), *d_vb = (uint32_t *)(base + o_vb);
+    int *d_cnt = (int *)(base + o_cnt), *d_off = (int *)(base + o_off), *d_nr = (int *)(base + o_nr);
+    NdtLeaf *d_lv = (NdtLeaf *)(base + o_lv);
+    double *d_ts = (double *)(base + o_ts), *d_out = (double *)(base + o_out);
+    void *d_cub = base + o_cub;
+    for (int p = 0; p < P; ++p) {
+        if (pd[p].n_tgt)
+            CK(cudaMemcpyAsync(d_t + pd[p].tgt_off, B[p].tgt.data(), pd[p].n_tgt * sizeof(float4), cudaMemcpyHostToDevice, st));
+        if (pd[p].n_src)
+            CK(cudaMemcpyAsync(d_s + pd[p].src_off, B[p].src.data(), pd[p].n_src * sizeof(float4), cudaMemcpyHostToDevice, st));
+    }
+    CK(cudaMemcpyAsync(d_pd, pd.data(), P * sizeof(NdtPairDev), cudaMemcpyHostToDevice, st));
+    if (nt_leaf) { // the leaves of every pair whose grid is ok (N1)
+        k_ndt_keys_batch<<<(unsigned)ceil_div(nt_leaf, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, nt_leaf, d_pd, P, d_ka, d_va);
+        if ((rc = sort_runs(ctx, d_cub, cub_bytes, nt_leaf, d_ka, d_kb, d_va, d_vb, d_uk, d_cnt, d_off, d_nr, st)) != MULLS_OK)
+            return rc;
+        k_ndt_leaves<<<(unsigned)ceil_div(nt_leaf, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, d_vb, d_off, d_cnt, d_nr, d_lv);
+        k_ndt_leaf_ranges<<<(unsigned)ceil_div(P, 64), 64, 0, st>>>(d_uk, d_nr, d_pd, P);
+        launches += 3;
+    }
+    // the walks in lockstep: each round evaluates every live pair with sources in one launch
+    double gd1, gd2;
+    ndt_gauss(resolution, gd1, gd2);
+    std::vector<NdtWalk> W(P);
+    std::vector<NdtIter> tr((size_t)P * (trace_cap > 0 ? trace_cap : 0));
+    const int cap = trace_cap > 0 ? trace_cap : 0;
+    std::vector<int> live(P), next;
+    for (int p = 0; p < P; ++p) ndt_walk_start(W[p]), live[p] = p;
+    std::vector<NdtLiveSlot> slots;
+    std::vector<double> r;
+    while (!live.empty()) {
+        slots.clear();
+        for (int p : live) {
+            for (int c = 0; c < kNdtTerms; ++c) W[p].r[c] = 0.0;
+            if (pd[p].n_src == 0) continue;
+            NdtLiveSlot s;
+            std::memcpy(s.E.T, W[p].T, sizeof(s.E.T));
+            ndt_angle_tables(W[p].q, s.E);
+            s.E.gauss_d1 = gd1, s.E.gauss_d2 = (float)gd2;
+            s.pair = p;
+            s.tile_begin = slots.empty() ? 0 : slots.back().tile_end;
+            s.tile_end = s.tile_begin + (tile_off[p + 1] - tile_off[p]);
+            slots.push_back(s);
+        }
+        if (!slots.empty()) {
+            const int ns = (int)slots.size();
+            CK(cudaMemcpyAsync(d_sl, slots.data(), ns * sizeof(NdtLiveSlot), cudaMemcpyHostToDevice, st));
+            NdtBatchEvalArgs EA{d_s, d_pd, d_uk, d_lv, d_sl, ns, d_ts};
+            k_ndt_eval_batch<<<(unsigned)slots.back().tile_end, kNdtTile, 0, st>>>(EA);
+            k_ndt_tiles_batch<<<(unsigned)ns, 64, 0, st>>>(d_ts, d_sl, d_out);
+            launches += 2;
+            r.resize((size_t)ns * kNdtTerms);
+            CK(cudaMemcpyAsync(r.data(), d_out, r.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            for (int k = 0; k < ns; ++k) std::memcpy(W[slots[k].pair].r, &r[(size_t)k * kNdtTerms], kNdtTerms * sizeof(double));
+        }
+        next.clear();
+        for (int p : live)
+            if (ndt_walk_advance(W[p], tr.data() + (size_t)p * cap, cap)) next.push_back(p);
+        live.swap(next);
+    }
+    // the fitness: one ingest of the filtered targets that need it, one search over all sources
+    std::vector<float> d2(ns_all, -1.f);
+    std::vector<std::vector<float>> rows(P);
+    std::vector<mulls_cloud_view> views(P, mulls_cloud_view{nullptr, 0});
+    bool any_fit = false;
+    for (int p = 0; p < P; ++p) {
+        if (B[p].tgt.empty() || B[p].src.empty()) continue;
+        const std::vector<float4> &t = B[p].tgt;
+        rows[p].assign(t.size() * 12, 0.f);
+        for (size_t i = 0; i < t.size(); ++i) rows[p][12 * i] = t[i].x, rows[p][12 * i + 1] = t[i].y, rows[p][12 * i + 2] = t[i].z;
+        views[p] = mulls_cloud_view{rows[p].data(), t.size()};
+        any_fit = true;
+    }
+    if (any_fit) {
+        DeviceArrays A;
+        int n_in = 0;
+        if ((rc = ingest_clouds(ctx, P, views.data(), false, 0.f, true, true, A, n_in, launches)) != MULLS_OK) return rc;
+        std::vector<float> T(12 * P);
+        for (int p = 0; p < P; ++p) std::memcpy(&T[12 * p], W[p].T, 12 * sizeof(float));
+        CK(cudaMemcpyAsync(d_T, T.data(), T.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+        k_ndt_fitness_batch<<<(unsigned)ceil_div(ns_all, 128), 128, 0, st>>>(A, d_s, ns_all, d_pd, P, d_T, d_d2);
+        launches += 1;
+        CK(cudaMemcpyAsync(d2.data(), d_d2, ns_all * sizeof(float), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    for (int p = 0; p < P; ++p) {
+        mulls_ndt_result &o = out[p];
+        const bool fit = views[p].n > 0;
+        baseline_score(d2.data() + pd[p].src_off, fit ? pd[p].n_src : 0, W[p].T, B[p].guess, B[p].moved, fitness_thre, o.trans,
+                       o.code, o.fitness);
+        o.iterations = W[p].nr;
+        o.converged = W[p].converged;
+        o.n_target = (int)B[p].tgt.size();
+        o.n_source = pd[p].n_src;
+        for (int i = 0; i < std::min(W[p].nr, cap); ++i) {
+            const NdtIter &t = tr[(size_t)p * cap + i];
+            mulls_ndt_iter &d = trace[(size_t)p * cap + i];
+            for (int c = 0; c < 6; ++c) d.p[c] = t.p[c];
+            d.step = t.step, d.score = t.score, d.reversed = t.reversed;
+        }
+    }
+    return MULLS_OK;
+}
+int mulls_omp_ndt_batch(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *targets, const mulls_cloud_view *sources,
+                        float ndt_resolution, int use_direct_search, const double *initial_guesses, int apply_intersection_filter,
+                        float fitness_score_thre, const double *target_bounds, const double *source_bounds, mulls_ndt_result *out,
+                        mulls_ndt_iter *trace, int trace_cap) {
+    return front_call(ctx, [&](uint64_t &launches) {
+        return ndt_batch_impl(ctx, n_pairs, targets, sources, ndt_resolution, use_direct_search, initial_guesses,
+                              apply_intersection_filter, fitness_score_thre, target_bounds, source_bounds, out, trace, trace_cap,
+                              launches);
     });
 }
 

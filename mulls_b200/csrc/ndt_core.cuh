@@ -450,63 +450,92 @@ struct NdtIter {
     int reversed; // computeStepLengthMT turned the direction around (-g.d > 0)
 };
 
-// computeTransformation from the derivatives at p = 0: `eval(p, T, out43)` evaluates at the float transform T of p and
-// fills score, gradient, Hessian. Returns the iteration count; T_final the float transform; converged; trace (cap
-// entries) records every iteration.
-template <class Eval>
-int ndt_walk(Eval eval, float T_final[12], int &converged, NdtIter *trace, int cap) {
-    double p[6] = {0, 0, 0, 0, 0, 0}, r[kNdtTerms];
+// computeTransformation from the derivatives at p = 0, as a state that advances one evaluation at a time, so that one
+// walk (ndt_walk) and a batch of walks in lockstep (mulls_omp_ndt_batch) run the same code. The owner evaluates score,
+// gradient and Hessian at the pose vector `q` and its float transform `T` into `r`, then calls ndt_walk_advance, until
+// that returns false. `T` is then the final float transform, `nr` the iteration count.
+struct NdtWalk {
+    double p[6], q[6], d[6], a; // pose, the pose being evaluated, the step direction and length
+    double r[kNdtTerms];        // score, gradient, Hessian at q
+    float T[12];                // the float transform of q
+    int nr, converged, reversed;
+    int in_step;                // r holds the evaluation of the current iteration's step
+};
+
+inline void ndt_walk_start(NdtWalk &W) {
     const float I[12] = {1.f, 0.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, 1.f, 0.f};
-    for (int i = 0; i < 12; ++i) T_final[i] = I[i];
-    eval(p, T_final, r);
-    int nr = 0;
-    converged = 0;
+    for (int i = 0; i < 6; ++i) W.p[i] = W.q[i] = 0.0;
+    for (int i = 0; i < 12; ++i) W.T[i] = I[i];
+    W.nr = W.converged = W.reversed = W.in_step = 0;
+    W.a = 0.0;
+}
+
+// consumes the evaluation of W.q: true when the next one is wanted (at W.q, W.T), false when the walk has ended. trace
+// (cap entries) records every iteration.
+inline bool ndt_walk_advance(NdtWalk &W, NdtIter *trace, int cap) {
     for (;;) {
-        double b[6], d[6];
-        for (int i = 0; i < 6; ++i) b[i] = -r[1 + i];
-        ndt_svd_solve(r + 7, b, d);
+        if (W.in_step) { // the end of an iteration: the step is taken
+            W.in_step = 0;
+            for (int i = 0; i < 6; ++i) W.p[i] = W.p[i] + W.d[i] * W.a;
+            if (trace && W.nr < cap) {
+                for (int i = 0; i < 6; ++i) trace[W.nr].p[i] = W.p[i];
+                trace[W.nr].step = W.a, trace[W.nr].score = W.r[0], trace[W.nr].reversed = W.reversed;
+            }
+            const bool stop = W.nr > kNdtMaxIterations || (W.nr && fabs(W.a) < kNdtEpsilon);
+            ++W.nr;
+            if (stop) {
+                W.converged = 1;
+                return false;
+            }
+        }
+        double b[6], *d = W.d;
+        for (int i = 0; i < 6; ++i) b[i] = -W.r[1 + i];
+        ndt_svd_solve(W.r + 7, b, d);
         double sq = 0.0;
         for (int i = 0; i < 6; ++i) sq += d[i] * d[i];
         const double norm = sqrt(sq);
         if (norm == 0 || norm != norm) {
-            converged = norm == norm;
-            return nr;
+            W.converged = norm == norm;
+            return false;
         }
         for (int i = 0; i < 6; ++i) d[i] /= norm; // normalize(): /= sqrt(squaredNorm)
         // computeStepLengthMT
         double d_phi_0 = 0.0;
-        for (int i = 0; i < 6; ++i) d_phi_0 += r[1 + i] * d[i];
+        for (int i = 0; i < 6; ++i) d_phi_0 += W.r[1 + i] * d[i];
         d_phi_0 = -d_phi_0;
-        double a = 0.0;
+        W.a = 0.0;
+        W.reversed = 0;
+        W.in_step = 1;
         bool step = true;
-        int reversed = 0;
         if (d_phi_0 >= 0) {
             if (d_phi_0 == 0) step = false;
             else {
                 for (int i = 0; i < 6; ++i) d[i] = -d[i];
-                reversed = 1;
+                W.reversed = 1;
             }
         }
         if (step) {
-            a = norm < kNdtStepMax ? norm : kNdtStepMax;
-            a = a > kNdtStepMin ? a : kNdtStepMin;
-            double xt[6];
-            for (int i = 0; i < 6; ++i) xt[i] = p[i] + d[i] * a;
-            ndt_step_transform(xt, T_final);
-            eval(xt, T_final, r);
+            double a = norm < kNdtStepMax ? norm : kNdtStepMax;
+            W.a = a > kNdtStepMin ? a : kNdtStepMin;
+            for (int i = 0; i < 6; ++i) W.q[i] = W.p[i] + d[i] * W.a;
+            ndt_step_transform(W.q, W.T);
+            return true;
         }
-        for (int i = 0; i < 6; ++i) p[i] = p[i] + d[i] * a;
-        if (trace && nr < cap) {
-            for (int i = 0; i < 6; ++i) trace[nr].p[i] = p[i];
-            trace[nr].step = a, trace[nr].score = r[0], trace[nr].reversed = reversed;
-        }
-        const bool stop = nr > kNdtMaxIterations || (nr && fabs(a) < kNdtEpsilon);
-        ++nr;
-        if (stop) {
-            converged = 1;
-            return nr;
-        }
+        // no step: the iteration ends without an evaluation, on the same derivatives
     }
+}
+
+// the whole walk: `eval(q, T, out43)` evaluates at the float transform T of q and fills score, gradient, Hessian.
+// Returns the iteration count; T_final the float transform; converged; trace (cap entries) records every iteration.
+template <class Eval>
+int ndt_walk(Eval eval, float T_final[12], int &converged, NdtIter *trace, int cap) {
+    NdtWalk W;
+    ndt_walk_start(W);
+    do eval(W.q, W.T, W.r);
+    while (ndt_walk_advance(W, trace, cap));
+    for (int i = 0; i < 12; ++i) T_final[i] = W.T[i];
+    converged = W.converged;
+    return W.nr;
 }
 
 // ---- the prologue and epilogue (host) ----------------------------------------------------------------------------

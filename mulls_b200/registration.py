@@ -43,6 +43,8 @@ class CloudBlock:
     local_bound: tuple = (0.0, 0.0, 0.0, 0.0, 0.0, 0.0)
     # centerpoint_t local_station (utility.hpp:92-99): the scanner position, pivot of the 4-DoF global search
     local_station: tuple = (0.0, 0.0, 0.0)
+    # pc_down: the down-sampled cloud the baseline registrations (omp_ndt) work on
+    pc_down: np.ndarray = field(default_factory=_empty)
 
     def clone_feature(self, get_feature_down: bool):
         """cloudblock_t::clone_feature (utility.hpp:524-550): the six clouds mm_lls_icp works on."""
@@ -82,6 +84,28 @@ class Constraint:
     information_matrix: np.ndarray = field(default_factory=lambda: np.eye(6))
     sigma: float = float(np.finfo(np.float32).max)
     confidence: float = 0.0
+
+
+def _xyz_rows(c):
+    """(n, 3) xyz rows are accepted too where only positions are read (NDT)"""
+    c = np.asarray(c, np.float32)
+    if c.ndim == 2 and c.shape[1] == 3:
+        c = np.concatenate([c, np.zeros((len(c), 9), np.float32)], axis=1)
+    return abi.as_aos48(c)
+
+
+def _ndt_out(res, tr, first, trace_cap):
+    """the dict omp_ndt returns, from a mulls_ndt_result and its trace rows tr[first:first + trace_cap]"""
+    out = dict(code=res.code, trans=np.array(res.trans[:], np.float64).reshape(4, 4), iterations=res.iterations,
+               converged=bool(res.converged), fitness=res.fitness, n_target=res.n_target, n_source=res.n_source)
+    if trace_cap > 0:
+        k = min(res.iterations, int(trace_cap))
+        rows = [tr[first + i] for i in range(k)]
+        out["trace"] = dict(p=np.array([r.p[:] for r in rows], np.float64).reshape(k, 6),
+                            step=np.array([r.step for r in rows], np.float64),
+                            score=np.array([r.score for r in rows], np.float64),
+                            reversed=np.array([r.reversed for r in rows], np.int32))
+    return out
 
 
 class Context:
@@ -373,13 +397,7 @@ class Context:
         the fitness exceeds fitness_score_thre), trans (Trans1_2, (4, 4) float64), iterations, converged, fitness,
         n_target / n_source after the intersection filter, and with trace_cap > 0 `trace`: per iteration the pose vector
         p (6), the step length, the score and whether the direction was reversed. use_direct_search=False (KDTREE) raises. Replaces the resident batch."""
-        def aos48(c):  # (n, 3) xyz rows are accepted too: NDT reads positions only
-            c = np.asarray(c, np.float32)
-            if c.ndim == 2 and c.shape[1] == 3:
-                c = np.concatenate([c, np.zeros((len(c), 9), np.float32)], axis=1)
-            return abi.as_aos48(c)
-
-        t, s = aos48(target), aos48(source)
+        t, s = _xyz_rows(target), _xyz_rows(source)
         g = np.ascontiguousarray(np.eye(4) if initial_guess is None else initial_guess, np.float64).reshape(16).copy()
         tb = np.ascontiguousarray(target_bound, np.float64).reshape(6).copy()
         sb = np.ascontiguousarray(source_bound, np.float64).reshape(6).copy()
@@ -390,15 +408,33 @@ class Context:
                                            int(bool(use_direct_search)), g.ctypes.data_as(dp), int(bool(apply_intersection_filter)),
                                            float(fitness_score_thre), tb.ctypes.data_as(dp), sb.ctypes.data_as(dp), C.byref(res),
                                            tr, int(trace_cap)))
-        out = dict(code=res.code, trans=np.array(res.trans[:], np.float64).reshape(4, 4), iterations=res.iterations,
-                   converged=bool(res.converged), fitness=res.fitness, n_target=res.n_target, n_source=res.n_source)
-        if trace_cap > 0:
-            k = min(res.iterations, int(trace_cap))
-            out["trace"] = dict(p=np.array([tr[i].p[:] for i in range(k)], np.float64).reshape(k, 6),
-                                step=np.array([tr[i].step for i in range(k)], np.float64),
-                                score=np.array([tr[i].score for i in range(k)], np.float64),
-                                reversed=np.array([tr[i].reversed for i in range(k)], np.int32))
-        return out
+        return _ndt_out(res, tr, 0, trace_cap)
+
+    def omp_ndt_batch(self, targets, sources, target_bounds, source_bounds, ndt_resolution: float = 1.0,
+                      use_direct_search: bool = True, initial_guesses=None, apply_intersection_filter: bool = True,
+                      fitness_score_thre: float = 10.0, trace_cap: int = 0):
+        """omp_ndt for P pairs in one call (mulls_omp_ndt_batch): targets / sources / target_bounds / source_bounds are
+        sequences of P clouds and bounds, initial_guesses None or P (4, 4) matrices; the other parameters are shared.
+        Returns one dict per pair, equal bit for bit to what omp_ndt returns for that pair alone. Needs a context made
+        for at least P pairs. Replaces the resident batch."""
+        ts, ss = [_xyz_rows(t) for t in targets], [_xyz_rows(s) for s in sources]
+        n = len(ts)
+        if len(ss) != n or len(target_bounds) != n or len(source_bounds) != n or (initial_guesses is not None and len(initial_guesses) != n):
+            raise ValueError("omp_ndt_batch: targets, sources, bounds and initial guesses must have one entry per pair")
+        g = np.ascontiguousarray([np.eye(4)] * n if initial_guesses is None else initial_guesses, np.float64).reshape(16 * n).copy()
+        tb = np.ascontiguousarray(target_bounds, np.float64).reshape(6 * n).copy()
+        sb = np.ascontiguousarray(source_bounds, np.float64).reshape(6 * n).copy()
+        tv = (abi.CloudView * max(n, 1))(*[abi.cloud_view(t) for t in ts])
+        sv = (abi.CloudView * max(n, 1))(*[abi.cloud_view(s) for s in ss])
+        res = (abi.NdtResult * max(n, 1))()
+        cap = int(trace_cap)
+        tr = (abi.NdtIter * max(n * cap, 1))()
+        dp = C.POINTER(C.c_double)
+        self._check(self.lib.mulls_omp_ndt_batch(self.handle, n, tv, sv, float(ndt_resolution), int(bool(use_direct_search)),
+                                                 g.ctypes.data_as(dp), int(bool(apply_intersection_filter)),
+                                                 float(fitness_score_thre), tb.ctypes.data_as(dp), sb.ctypes.data_as(dp), res,
+                                                 tr, cap))
+        return [_ndt_out(res[i], tr, i * cap, cap) for i in range(n)]
 
     def omp_gicp(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, max_iter_num: int = 20,
                  dis_thre_unit: float = 1.5, using_voxel_gicp: bool = True, voxel_size: float = 1.0, initial_guess=None,
@@ -621,6 +657,26 @@ class CRegistration:
         r = self._ctx.omp_ndt(target, source, target_bound, source_bound, ndt_resolution, use_direct_search, initial_guess,
                               apply_intersection_filter, fitness_score_thre)
         return r["code"], r["trans"]
+
+    def omp_ndt_batch(self, registration_cons, ndt_resolution: float = 1.0, use_direct_search: bool = True,
+                      initial_guesses=None, apply_intersection_filter: bool = True, fitness_score_thre: float = 10.0):
+        """omp_ndt for every Constraint of registration_cons in one call (block1 = target, block2 = source, their pc_down
+        and local_bounds; initial_guesses None or one (4, 4) per constraint): each one's Trans1_2 is written as
+        omp_ndt writes it. Returns the codes, one per constraint."""
+        n = len(registration_cons)
+        if self._batch_ctx is None or self._batch_ctx.max_pairs < n or self._batch_cap < (self._max_src, self._max_tgt):
+            if self._batch_ctx is not None:
+                self._batch_ctx.close()
+            self._batch_ctx = Context(self._device, max(n, 1), self._max_src, self._max_tgt)
+            self._batch_cap = (self._max_src, self._max_tgt)
+        res = self._batch_ctx.omp_ndt_batch([c.block1.pc_down for c in registration_cons],
+                                            [c.block2.pc_down for c in registration_cons],
+                                            [c.block1.local_bound for c in registration_cons],
+                                            [c.block2.local_bound for c in registration_cons], ndt_resolution,
+                                            use_direct_search, initial_guesses, apply_intersection_filter, fitness_score_thre)
+        for c, r in zip(registration_cons, res):
+            c.Trans1_2 = r["trans"]
+        return [r["code"] for r in res]
 
     def omp_gicp(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, max_iter_num: int = 20,
                  dis_thre_unit: float = 1.5, using_voxel_gicp: bool = True, voxel_size: float = 1.0, initial_guess=None,
