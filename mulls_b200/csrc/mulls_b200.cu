@@ -2,6 +2,7 @@
 // CUDA runtime only: no torch, no PCL/Eigen. One context = one device, one stream.
 #include <algorithm>
 #include <atomic>
+#include <cassert>
 #include <memory>
 #include <cmath>
 #include <cstdio>
@@ -84,10 +85,18 @@ int nccl_allreduce_hook(void *user, void *buf, size_t count, int dtype, int op, 
 
 struct mulls_map;
 
-// a device buffer of the context that only grows (grow_scratch)
+// a device buffer of the context that only grows (grow_scratch); freed with the context
 struct Scratch {
     void *p = nullptr;
     size_t bytes = 0;
+    Scratch() = default;
+    Scratch(const Scratch &) = delete;
+    Scratch &operator=(const Scratch &) = delete;
+    ~Scratch() { release(); }
+    void release() {
+        if (p) cudaFree(p);
+        p = nullptr, bytes = 0;
+    }
 };
 
 struct mulls_ctx {
@@ -186,8 +195,7 @@ struct mulls_ctx {
 static int grow_scratch(mulls_ctx *ctx, Scratch &s, size_t bytes) {
     bytes = std::max<size_t>(bytes, 16);
     if (bytes <= s.bytes) return MULLS_OK;
-    if (s.p) cudaFree(s.p);
-    s = Scratch{};
+    s.release();
     CK(cudaMalloc(&s.p, bytes));
     s.bytes = bytes;
     return MULLS_OK;
@@ -214,19 +222,33 @@ static void drop_iteration_graph(mulls_ctx *ctx) {
     if (ctx->graph) cudaGraphDestroy(ctx->graph), ctx->graph = nullptr;
 }
 
-// The device arrays of one call in one Scratch: take() hands out 256-byte aligned offsets, grow() makes the Scratch
-// hold them all and sets `base`, from which each array is at its offset.
+// The device arrays of one call in one Scratch: take(p, count) reserves `count` elements of *p's type at the next
+// 256-byte boundary and remembers p; grow() makes the Scratch hold them all and points each p at its array.
 struct ScratchLayout {
-    size_t bytes = 0;
-    size_t take(size_t n) {
-        const size_t o = bytes;
-        bytes += ceil_div(std::max<size_t>(n, 1), 256) * 256;
-        return o;
-    }
-    int grow(mulls_ctx *ctx, Scratch &s, char *&base) const {
+    size_t bytes = 0; // the arrays taken so far
+    template <typename T> void take(T *&p, size_t count) { add(&p, count * sizeof(T), &bind<T>); }
+    void take_bytes(void *&p, size_t n) { add(&p, n, &bind<void>); }
+    int grow(mulls_ctx *ctx, Scratch &s) const {
         const int rc = grow_scratch(ctx, s, bytes);
-        base = (char *)s.p;
+        if (rc == MULLS_OK)
+            for (int i = 0; i < n_slots; ++i) slots[i].bind(slots[i].p, (char *)s.p + slots[i].off);
         return rc;
+    }
+
+  private:
+    template <typename T> static void bind(void *p, char *at) { *(T **)p = (T *)at; }
+    struct Slot {
+        void *p; // the T * to set
+        void (*bind)(void *, char *);
+        size_t off;
+    };
+    static constexpr int kMaxSlots = 40;
+    Slot slots[kMaxSlots];
+    int n_slots = 0;
+    void add(void *p, size_t n, void (*b)(void *, char *)) {
+        assert(n_slots < kMaxSlots);
+        slots[n_slots++] = Slot{p, b, bytes};
+        bytes += ceil_div(std::max<size_t>(n, 1), 256) * 256;
     }
 };
 
@@ -267,9 +289,6 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     for (void *p : ctx->allocs) cudaFree(p);
     if (ctx->cub_temp) cudaFree(ctx->cub_temp);
-    for (Scratch *s : {&ctx->pca_buf, &ctx->cls_buf, &ctx->gf_buf, &ctx->gf_cell_buf, &ctx->vx_buf, &ctx->ext_buf, &ctx->sor_buf, &ctx->raw_buf, &ctx->ncc_buf, &ctx->rc_buf, &ctx->nms_buf,
-                        &ctx->ndt_buf, &ctx->gicp_buf})
-        if (s->p) cudaFree(s->p);
     if (ctx->rc_host) cudaFreeHost(ctx->rc_host);
     if (ctx->h_results) cudaFreeHost(ctx->h_results);
     if (ctx->h_flags) cudaFreeHost(ctx->h_flags);
@@ -286,7 +305,7 @@ void mulls_destroy(mulls_ctx *ctx) {
     if (ctx->ev_end) cudaEventDestroy(ctx->ev_end);
     if (ctx->ev_h2d0) cudaEventDestroy(ctx->ev_h2d0);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx; // frees the Scratch buffers, with ctx->device current
 }
 
 mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t max_tgt_pts) {
@@ -1409,26 +1428,20 @@ static int pca_on_device(mulls_ctx *ctx, mulls_cloud_view cloud, bool cloud_on_d
     if (rc != MULLS_OK) return rc;
     const size_t n = cloud.n;
     ScratchLayout L;
-    const size_t o_ev = L.take(3 * n * sizeof(float)), o_pr = L.take(3 * n * sizeof(float)),
-                 o_nr = L.take(3 * n * sizeof(float)), o_num = L.take(n * sizeof(int)), outputs = L.bytes;
+    L.take(args.eigenvalues, 3 * n), L.take(args.principal, 3 * n), L.take(args.normal, 3 * n), L.take(args.pt_num, n);
+    const size_t outputs = L.bytes;
     // k within the list capacity (the reference uses 20..50): the neighbour lists, and with them pcl::PCA's float mean /
     // covariance accumulated in radiusSearch order — bit-reproducible against the CPU path; larger or unlimited k: fp64
     // warp reduction
-    const bool lists = k >= 1 && k <= kPcaListCap;
-    const size_t o_nbr = lists ? L.take(n * (size_t)k * sizeof(uint32_t)) : 0;
-    char *base;
-    if ((rc = L.grow(ctx, ctx->pca_buf, base)) != MULLS_OK) return rc;
+    args.nbr = nullptr;
+    if (k >= 1 && k <= kPcaListCap) L.take(args.nbr, n * (size_t)k);
+    if ((rc = L.grow(ctx, ctx->pca_buf)) != MULLS_OK) return rc;
     args.radius = radius;
     args.r2 = (float)((double)radius * (double)radius);
     args.k = k;
     args.stride = stride;
-    args.eigenvalues = (float *)(base + o_ev);
-    args.principal = (float *)(base + o_pr);
-    args.normal = (float *)(base + o_nr);
-    args.pt_num = (int *)(base + o_num);
-    args.nbr = lists ? (uint32_t *)(base + o_nbr) : nullptr;
     cudaStream_t st = ctx->stream;
-    CK(cudaMemsetAsync(base, 0, outputs, st));
+    CK(cudaMemsetAsync(args.eigenvalues, 0, outputs, st)); // the four outputs, from the layout's start
     if (n && adaptive) {
         PcaAdaptiveArgs aa;
         static_cast<PcaArgs &>(aa) = args;
@@ -1496,13 +1509,12 @@ static int sor_filter_impl(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, d
                    " neighbours wanted per point";
         return MULLS_E_ARG;
     }
+    float *d_dist;
+    uint32_t *d_keep;
+    mulls_sor_stats *d_stats;
     ScratchLayout L;
-    const size_t o_dist = L.take(n * sizeof(float)), o_keep = L.take(ceil_div(n, 32) * 4), o_stats = L.take(sizeof(mulls_sor_stats));
-    char *base;
-    if ((rc = L.grow(ctx, ctx->sor_buf, base)) != MULLS_OK) return rc;
-    float *d_dist = (float *)(base + o_dist);
-    uint32_t *d_keep = (uint32_t *)(base + o_keep);
-    mulls_sor_stats *d_stats = (mulls_sor_stats *)(base + o_stats);
+    L.take(d_dist, n), L.take(d_keep, ceil_div(n, 32)), L.take(d_stats, 1);
+    if ((rc = L.grow(ctx, ctx->sor_buf)) != MULLS_OK) return rc;
     cudaStream_t st = ctx->stream;
     CK(cudaMemsetAsync(d_dist, 0, n * sizeof(float), st)); // non-finite points: distance 0, as PCL
     const unsigned nb = (unsigned)ceil_div((size_t)n_valid, kSorBlock);
@@ -1534,11 +1546,9 @@ int mulls_sor_filter(mulls_ctx *ctx, mulls_cloud_view cloud, int mean_k, double 
 static int raw_upload(mulls_ctx *ctx, const mulls_cloud_view *clouds, int n_clouds, size_t n_total, int out_floats,
                       float **d_rows, float **d_out, TsState **d_st) {
     ScratchLayout L;
-    const size_t o_rows = L.take(n_total * 48), o_out = L.take(n_total * out_floats * sizeof(float)), o_st = L.take(sizeof(TsState));
-    char *base;
-    int rc = L.grow(ctx, ctx->raw_buf, base);
+    L.take(*d_rows, n_total * 12), L.take(*d_out, n_total * out_floats), L.take(*d_st, 1);
+    int rc = L.grow(ctx, ctx->raw_buf);
     if (rc != MULLS_OK) return rc;
-    *d_rows = (float *)(base + o_rows), *d_out = (float *)(base + o_out), *d_st = (TsState *)(base + o_st);
     size_t at = 0;
     for (int c = 0; c < n_clouds; ++c) {
         if (clouds[c].n)
@@ -1679,26 +1689,28 @@ static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, in
         return MULLS_E_CAPACITY;
     }
     cudaStream_t st = ctx->stream;
+    float *d_rows, *d_desc, *d_range;
+    TsState *d_ts;
     ScratchLayout L;
-    const size_t o_rows = L.take(n_all * 48), o_desc = L.take(n_all * kNccDim * sizeof(float)), o_ts = L.take(sizeof(TsState)),
-                 o_range = L.take(2 * sizeof(float));
-    size_t o_rowkey = 0, o_colmin = 0, o_cand = 0, o_keep = 0, o_sel = 0, o_out = 0, o_num = 0, o_gath = 0, o_sorted = 0, o_tmp = 0;
+    L.take(d_rows, n_all * 12), L.take(d_desc, n_all * kNccDim), L.take(d_ts, 1), L.take(d_range, 2);
+    unsigned long long *d_rowkey = nullptr, *d_cand = nullptr, *d_out = nullptr, *d_gath = nullptr, *d_sorted = nullptr;
+    uint32_t *d_colmin = nullptr;
+    uint8_t *d_keep = nullptr;
+    int *d_num = nullptr;
+    NccSelect *d_sel = nullptr;
+    void *d_tmp;
     size_t tmp_bytes = 0;
     if (!fixed_num_corr) {
-        o_rowkey = L.take(nt * 8), o_colmin = L.take(ns * 4), o_cand = L.take(nt * 8), o_keep = L.take(nt), o_out = L.take(nt * 8);
-        o_num = L.take(sizeof(int));
+        L.take(d_rowkey, nt), L.take(d_colmin, ns), L.take(d_cand, nt), L.take(d_keep, nt), L.take(d_out, nt), L.take(d_num, 1);
         CK(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, (unsigned long long *)nullptr, (uint8_t *)nullptr,
                                       (unsigned long long *)nullptr, (int *)nullptr, (int)nt, st));
     } else {
-        o_sel = L.take(sizeof(NccSelect)), o_gath = L.take(K * 8), o_sorted = L.take(K * 8);
+        L.take(d_sel, 1), L.take(d_gath, K), L.take(d_sorted, K);
         CK(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr,
                                           (int)std::max<size_t>(K, 1), 0, 64, st));
     }
-    o_tmp = L.take(tmp_bytes);
-    char *base;
-    if ((rc = L.grow(ctx, ctx->ncc_buf, base)) != MULLS_OK) return rc;
-    float *d_rows = (float *)(base + o_rows), *d_desc = (float *)(base + o_desc), *d_range = (float *)(base + o_range);
-    TsState *d_ts = (TsState *)(base + o_ts);
+    L.take_bytes(d_tmp, tmp_bytes);
+    if ((rc = L.grow(ctx, ctx->ncc_buf)) != MULLS_OK) return rc;
     CK(cudaMemcpyAsync(d_rows, tk.aos48, nt * 48, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync((char *)d_rows + nt * 48, sk.aos48, ns * 48, cudaMemcpyHostToDevice, st));
     TsState ts0{};
@@ -1714,11 +1726,6 @@ static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, in
     const dim3 grid((unsigned)ceil_div(nt, kNccTileT), (unsigned)gy);
     std::vector<std::pair<int32_t, int32_t>> res;
     if (!fixed_num_corr) {
-        unsigned long long *d_rowkey = (unsigned long long *)(base + o_rowkey), *d_cand = (unsigned long long *)(base + o_cand),
-                           *d_out = (unsigned long long *)(base + o_out);
-        uint32_t *d_colmin = (uint32_t *)(base + o_colmin);
-        uint8_t *d_keep = (uint8_t *)(base + o_keep);
-        int *d_num = (int *)(base + o_num);
         k_ncc_init<<<(unsigned)ceil_div(std::max(nt, ns), kRawBlock), kRawBlock, 0, st>>>(d_rowkey, (uint32_t)nt, d_colmin, (uint32_t)ns);
         if (reciprocal_on)
             k_ncc_pairs<kNccRowCol><<<grid, kNccBlock, 0, st>>>(P, d_rowkey, d_colmin, nullptr, 0, nullptr, 0);
@@ -1727,7 +1734,7 @@ static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, in
         k_ncc_pick<<<nbt, kRawBlock, 0, st>>>(d_rowkey, d_colmin, (uint32_t)nt, reciprocal_on ? 1 : 0, d_cand, d_keep);
         launches += 3;
         size_t tb = tmp_bytes;
-        CK(cub::DeviceSelect::Flagged(base + o_tmp, tb, d_cand, d_keep, d_out, d_num, (int)nt, st));
+        CK(cub::DeviceSelect::Flagged(d_tmp, tb, d_cand, d_keep, d_out, d_num, (int)nt, st));
         std::vector<unsigned long long> h(nt);
         int n_kept = 0;
         CK(cudaMemcpyAsync(&n_kept, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1737,8 +1744,6 @@ static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, in
         res.reserve(n_kept);
         for (int k = 0; k < n_kept; ++k) res.emplace_back((int32_t)(h[k] >> 32), (int32_t)(uint32_t)h[k]);
     } else if (K > 0) {
-        NccSelect *d_sel = (NccSelect *)(base + o_sel);
-        unsigned long long *d_gath = (unsigned long long *)(base + o_gath), *d_sorted = (unsigned long long *)(base + o_sorted);
         NccSelect s0{};
         s0.rank = (uint32_t)(K - 1);
         s0.E = 0xffffffffu;
@@ -1764,7 +1769,7 @@ static int ncc_impl(mulls_ctx *ctx, mulls_cloud_view tk, mulls_cloud_view sk, in
         }
         k_ncc_pairs<kNccGather><<<grid, kNccBlock, 0, st>>>(P, nullptr, nullptr, d_sel, 0, d_gath, K);
         size_t tb = tmp_bytes;
-        CK(cub::DeviceRadixSort::SortKeys(base + o_tmp, tb, d_gath, d_sorted, (int)K, 0, 64, st));
+        CK(cub::DeviceRadixSort::SortKeys(d_tmp, tb, d_gath, d_sorted, (int)K, 0, 64, st));
         launches += 1;
         std::vector<unsigned long long> h(K);
         unsigned long long gathered = 0;
@@ -1842,20 +1847,17 @@ static int ransac_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv,
     int hyps = 0;
     if (N > 0) { // an empty correspondence list returns before the rejector runs (getCorrespondences)
         cudaStream_t st = ctx->stream;
+        float *d_corr, *d_best, *d_T[2];
+        int *d_samp[2], *d_cnt[2];
+        RcRefineArgs A{};
         ScratchLayout L;
-        const size_t o_corr = L.take(N * 6 * sizeof(float)), o_samp = L.take(2 * kRcChunk * 3 * sizeof(int)),
-                     o_T = L.take(2 * (size_t)kRcChunk * 12 * sizeof(float)), o_cnt = L.take(2 * kRcChunk * sizeof(int)),
-                     o_best = L.take(12 * sizeof(float)), o_fa = L.take(N), o_fb = L.take(N), o_err = L.take(N * sizeof(float)),
-                     o_out = L.take(sizeof(RcRefineOut));
-        char *base;
-        if ((rc = L.grow(ctx, ctx->rc_buf, base)) != MULLS_OK) return rc;
+        L.take(d_corr, N * 6), L.take(d_samp[0], 3 * kRcChunk), L.take(d_samp[1], 3 * kRcChunk);
+        L.take(d_T[0], 12 * kRcChunk), L.take(d_T[1], 12 * kRcChunk), L.take(d_cnt[0], kRcChunk), L.take(d_cnt[1], kRcChunk);
+        L.take(d_best, 12), L.take(A.flag_a, N), L.take(A.flag_b, N), L.take(A.err, N), L.take(A.out, 1);
+        if ((rc = L.grow(ctx, ctx->rc_buf)) != MULLS_OK) return rc;
         if (!ctx->rc_host) CK(cudaMallocHost(&ctx->rc_host, 2 * kRcChunk * 4 * sizeof(int)));
-        float *d_corr = (float *)(base + o_corr), *d_best = (float *)(base + o_best);
         int *h_samp[2] = {(int *)ctx->rc_host, (int *)ctx->rc_host + 3 * kRcChunk};
         int *h_cnt[2] = {(int *)ctx->rc_host + 6 * kRcChunk, (int *)ctx->rc_host + 7 * kRcChunk};
-        int *d_samp[2] = {(int *)(base + o_samp), (int *)(base + o_samp) + 3 * kRcChunk};
-        float *d_T[2] = {(float *)(base + o_T), (float *)(base + o_T) + 12 * (size_t)kRcChunk};
-        int *d_cnt[2] = {(int *)(base + o_cnt), (int *)(base + o_cnt) + kRcChunk};
         // the correspondences i <-> i: source x y z, target x y z
         std::vector<float> c6(N * 6);
         for (size_t i = 0; i < N; ++i)
@@ -1916,8 +1918,7 @@ static int ransac_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv,
         if (W.best < 0) { // computeModel failed: every correspondence, identity
             n_final = N;
         } else {
-            RcRefineArgs A{d_corr, (int)N, d_best, (double)noise_bound, (uint8_t *)(base + o_fa), (uint8_t *)(base + o_fb),
-                           (float *)(base + o_err), (RcRefineOut *)(base + o_out)};
+            A.corr = d_corr, A.n = (int)N, A.T_best = d_best, A.threshold = (double)noise_bound;
             k_ransac_refine<<<1, kRcLanes, 0, st>>>(A);
             launches += 1;
             RcRefineOut o;
@@ -2054,22 +2055,19 @@ static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, fl
     cudaStream_t st = ctx->stream;
     size_t cub_bytes = 0;
     if ((rc = sort_runs_bytes(ctx, nt, cub_bytes)) != MULLS_OK) return rc;
+    float4 *d_t, *d_s;
+    uint64_t *d_ka, *d_kb, *d_uk;
+    uint32_t *d_va, *d_vb;
+    int *d_cnt, *d_off, *d_nr;
+    NdtLeaf *d_lv;
+    double *d_ts, *d_out;
+    float *d_d2;
+    void *d_cub;
     ScratchLayout L;
-    const size_t o_t = L.take(nt * sizeof(float4)), o_s = L.take(ns * sizeof(float4)), o_ka = L.take(nt * 8ull),
-                 o_kb = L.take(nt * 8ull), o_va = L.take(nt * 4ull), o_vb = L.take(nt * 4ull), o_uk = L.take(nt * 8ull),
-                 o_cnt = L.take(nt * 4ull), o_off = L.take(nt * 4ull), o_nr = L.take(sizeof(int)),
-                 o_lv = L.take(nt * sizeof(NdtLeaf)), o_ts = L.take((size_t)tiles * kNdtTerms * 8),
-                 o_out = L.take(kNdtTerms * 8), o_d2 = L.take(ns * sizeof(float)), o_cub = L.take(cub_bytes);
-    char *base;
-    if ((rc = L.grow(ctx, ctx->ndt_buf, base)) != MULLS_OK) return rc;
-    float4 *d_t = (float4 *)(base + o_t), *d_s = (float4 *)(base + o_s);
-    uint64_t *d_ka = (uint64_t *)(base + o_ka), *d_kb = (uint64_t *)(base + o_kb), *d_uk = (uint64_t *)(base + o_uk);
-    uint32_t *d_va = (uint32_t *)(base + o_va), *d_vb = (uint32_t *)(base + o_vb);
-    int *d_cnt = (int *)(base + o_cnt), *d_off = (int *)(base + o_off), *d_nr = (int *)(base + o_nr);
-    NdtLeaf *d_lv = (NdtLeaf *)(base + o_lv);
-    double *d_ts = (double *)(base + o_ts), *d_out = (double *)(base + o_out);
-    float *d_d2 = (float *)(base + o_d2);
-    void *d_cub = base + o_cub;
+    L.take(d_t, nt), L.take(d_s, ns), L.take(d_ka, nt), L.take(d_kb, nt), L.take(d_va, nt), L.take(d_vb, nt), L.take(d_uk, nt);
+    L.take(d_cnt, nt), L.take(d_off, nt), L.take(d_nr, 1), L.take(d_lv, nt), L.take(d_ts, (size_t)tiles * kNdtTerms);
+    L.take(d_out, kNdtTerms), L.take(d_d2, ns), L.take_bytes(d_cub, cub_bytes);
+    if ((rc = L.grow(ctx, ctx->ndt_buf)) != MULLS_OK) return rc;
     if (nt) CK(cudaMemcpyAsync(d_t, tgt.data(), nt * sizeof(float4), cudaMemcpyHostToDevice, st));
     if (ns) CK(cudaMemcpyAsync(d_s, src.data(), ns * sizeof(float4), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(d_nr, 0, sizeof(int), st));
@@ -2213,26 +2211,22 @@ static int ndt_batch_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view
     size_t cub_bytes = 0;
     int rc;
     if ((rc = sort_runs_bytes(ctx, nt_leaf, cub_bytes)) != MULLS_OK) return rc;
+    NdtPairDev *d_pd;
+    NdtLiveSlot *d_sl;
+    float *d_T, *d_d2;
+    float4 *d_t, *d_s;
+    uint64_t *d_ka, *d_kb, *d_uk;
+    uint32_t *d_va, *d_vb;
+    int *d_cnt, *d_off, *d_nr;
+    NdtLeaf *d_lv;
+    double *d_ts, *d_out;
+    void *d_cub;
     ScratchLayout L;
-    const size_t o_pd = L.take(P * sizeof(NdtPairDev)), o_sl = L.take(P * sizeof(NdtLiveSlot)), o_T = L.take(P * 12 * sizeof(float)),
-                 o_t = L.take(nt_leaf * sizeof(float4)), o_s = L.take(ns_all * sizeof(float4)), o_ka = L.take(nt_leaf * 8ull),
-                 o_kb = L.take(nt_leaf * 8ull), o_va = L.take(nt_leaf * 4ull), o_vb = L.take(nt_leaf * 4ull),
-                 o_uk = L.take(nt_leaf * 8ull), o_cnt = L.take(nt_leaf * 4ull), o_off = L.take(nt_leaf * 4ull),
-                 o_nr = L.take(sizeof(int)), o_lv = L.take(nt_leaf * sizeof(NdtLeaf)),
-                 o_ts = L.take((size_t)tiles_all * kNdtTerms * 8), o_out = L.take((size_t)P * kNdtTerms * 8),
-                 o_d2 = L.take(ns_all * sizeof(float)), o_cub = L.take(cub_bytes);
-    char *base;
-    if ((rc = L.grow(ctx, ctx->ndt_buf, base)) != MULLS_OK) return rc;
-    NdtPairDev *d_pd = (NdtPairDev *)(base + o_pd);
-    NdtLiveSlot *d_sl = (NdtLiveSlot *)(base + o_sl);
-    float *d_T = (float *)(base + o_T), *d_d2 = (float *)(base + o_d2);
-    float4 *d_t = (float4 *)(base + o_t), *d_s = (float4 *)(base + o_s);
-    uint64_t *d_ka = (uint64_t *)(base + o_ka), *d_kb = (uint64_t *)(base + o_kb), *d_uk = (uint64_t *)(base + o_uk);
-    uint32_t *d_va = (uint32_t *)(base + o_va), *d_vb = (uint32_t *)(base + o_vb);
-    int *d_cnt = (int *)(base + o_cnt), *d_off = (int *)(base + o_off), *d_nr = (int *)(base + o_nr);
-    NdtLeaf *d_lv = (NdtLeaf *)(base + o_lv);
-    double *d_ts = (double *)(base + o_ts), *d_out = (double *)(base + o_out);
-    void *d_cub = base + o_cub;
+    L.take(d_pd, P), L.take(d_sl, P), L.take(d_T, P * 12), L.take(d_t, nt_leaf), L.take(d_s, ns_all), L.take(d_ka, nt_leaf);
+    L.take(d_kb, nt_leaf), L.take(d_va, nt_leaf), L.take(d_vb, nt_leaf), L.take(d_uk, nt_leaf), L.take(d_cnt, nt_leaf);
+    L.take(d_off, nt_leaf), L.take(d_nr, 1), L.take(d_lv, nt_leaf), L.take(d_ts, (size_t)tiles_all * kNdtTerms);
+    L.take(d_out, (size_t)P * kNdtTerms), L.take(d_d2, ns_all), L.take_bytes(d_cub, cub_bytes);
+    if ((rc = L.grow(ctx, ctx->ndt_buf)) != MULLS_OK) return rc;
     for (int p = 0; p < P; ++p) {
         if (pd[p].n_tgt)
             CK(cudaMemcpyAsync(d_t + pd[p].tgt_off, B[p].tgt.data(), pd[p].n_tgt * sizeof(float4), cudaMemcpyHostToDevice, st));
@@ -2386,23 +2380,19 @@ static int gicp_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, i
     cudaStream_t st = ctx->stream;
     size_t cub_bytes = 0;
     if ((rc = sort_runs_bytes(ctx, nt, cub_bytes)) != MULLS_OK) return rc;
+    float4 *d_t, *d_s;
+    float *d_ct, *d_cs, *d_d2; // covariances: 9 floats per point
+    uint64_t *d_ka, *d_kb, *d_uk;
+    uint32_t *d_va, *d_vb;
+    int *d_cnt, *d_off, *d_nr;
+    GicpVoxel *d_vx;
+    double *d_ts, *d_out;
+    void *d_cub;
     ScratchLayout L;
-    const size_t o_t = L.take(nt * sizeof(float4)), o_s = L.take(ns * sizeof(float4)), o_ct = L.take(nt * 36ull),
-                 o_cs = L.take(ns * 36ull), o_ka = L.take(nt * 8ull), o_kb = L.take(nt * 8ull), o_va = L.take(nt * 4ull),
-                 o_vb = L.take(nt * 4ull), o_uk = L.take(nt * 8ull), o_cnt = L.take(nt * 4ull), o_off = L.take(nt * 4ull),
-                 o_nr = L.take(sizeof(int)), o_vx = L.take(nt * sizeof(GicpVoxel)),
-                 o_ts = L.take((size_t)tiles * kGicpTerms * 8), o_out = L.take(kGicpTerms * 8),
-                 o_d2 = L.take(ns * sizeof(float)), o_cub = L.take(cub_bytes);
-    char *base;
-    if ((rc = L.grow(ctx, ctx->gicp_buf, base)) != MULLS_OK) return rc;
-    float4 *d_t = (float4 *)(base + o_t), *d_s = (float4 *)(base + o_s);
-    float *d_ct = (float *)(base + o_ct), *d_cs = (float *)(base + o_cs), *d_d2 = (float *)(base + o_d2);
-    uint64_t *d_ka = (uint64_t *)(base + o_ka), *d_kb = (uint64_t *)(base + o_kb), *d_uk = (uint64_t *)(base + o_uk);
-    uint32_t *d_va = (uint32_t *)(base + o_va), *d_vb = (uint32_t *)(base + o_vb);
-    int *d_cnt = (int *)(base + o_cnt), *d_off = (int *)(base + o_off), *d_nr = (int *)(base + o_nr);
-    GicpVoxel *d_vx = (GicpVoxel *)(base + o_vx);
-    double *d_ts = (double *)(base + o_ts), *d_out = (double *)(base + o_out);
-    void *d_cub = base + o_cub;
+    L.take(d_t, nt), L.take(d_s, ns), L.take(d_ct, nt * 9ull), L.take(d_cs, ns * 9ull), L.take(d_ka, nt), L.take(d_kb, nt);
+    L.take(d_va, nt), L.take(d_vb, nt), L.take(d_uk, nt), L.take(d_cnt, nt), L.take(d_off, nt), L.take(d_nr, 1), L.take(d_vx, nt);
+    L.take(d_ts, (size_t)tiles * kGicpTerms), L.take(d_out, kGicpTerms), L.take(d_d2, ns), L.take_bytes(d_cub, cub_bytes);
+    if ((rc = L.grow(ctx, ctx->gicp_buf)) != MULLS_OK) return rc;
     CK(cudaMemcpyAsync(d_t, tgt.data(), nt * sizeof(float4), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_s, src.data(), ns * sizeof(float4), cudaMemcpyHostToDevice, st));
     // G1: the source's covariances, then the target's (its grid stays for the fitness)
@@ -2873,19 +2863,21 @@ static int nms_impl(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int32_
     const uint32_t slots = nms_hash_slots(n, r2);
     size_t cub_bytes = 0;
     CK(cub::DeviceRadixSort::SortKeys(nullptr, cub_bytes, (uint64_t *)nullptr, (uint64_t *)nullptr, (int)n, 0, 64, st));
-    ScratchLayout L;
-    const size_t o_in = L.take(n * 48), o_srt = L.take(n * 48), o_sel = L.take(n * sizeof(float4)), o_idx = L.take(n * sizeof(int32_t)),
-                 o_ord = L.take(n * sizeof(uint32_t)), o_ka = L.take(n * sizeof(uint64_t)), o_kb = L.take(n * sizeof(uint64_t)),
-                 o_hash = L.take((size_t)slots * sizeof(NmsSlot)), o_next = L.take(slots ? n * sizeof(int32_t) : 0),
-                 o_cnt = L.take(sizeof(NmsCounts)), o_cub = L.take(cub_bytes);
-    char *base;
-    if ((rc = L.grow(ctx, ctx->nms_buf, base)) != MULLS_OK) return rc;
-    NmsCounts *d_cnt = (NmsCounts *)(base + o_cnt);
-    hc = NmsCounts{(uint32_t)n, 0, 0, 0};
-    CK(cudaMemcpyAsync(d_cnt, &hc, sizeof(hc), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(base + o_in, cloud.aos48, n * 48, cudaMemcpyDefault, st));
     NmsArgs N;
     std::memset(&N, 0, sizeof(N));
+    float4 *d_in;
+    NmsSlot *d_hash;
+    int32_t *d_next;
+    NmsCounts *d_cnt;
+    void *d_cub;
+    ScratchLayout L;
+    L.take(d_in, 3 * n), L.take(N.sorted[0], 3 * n), L.take(N.sel[0], n), L.take(N.kept_idx[0], n), L.take(N.order, n);
+    L.take(N.keys_a, n), L.take(N.keys_b, n), L.take(d_hash, slots), L.take(d_next, slots ? n : 0), L.take(d_cnt, 1);
+    L.take_bytes(d_cub, cub_bytes);
+    if ((rc = L.grow(ctx, ctx->nms_buf)) != MULLS_OK) return rc;
+    hc = NmsCounts{(uint32_t)n, 0, 0, 0};
+    CK(cudaMemcpyAsync(d_cnt, &hc, sizeof(hc), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_in, cloud.aos48, n * 48, cudaMemcpyDefault, st));
     N.n_clouds = 1;
     N.on_mask = 1;
     N.n = &d_cnt->n;
@@ -2893,20 +2885,11 @@ static int nms_impl(mulls_ctx *ctx, mulls_cloud_view cloud, float radius, int32_
     N.ran = &d_cnt->ran;
     N.r2 = r2;
     N.inv_cell = nms_inv_cell(r2);
-    N.in[0] = (const float4 *)(base + o_in);
-    N.sorted[0] = (float4 *)(base + o_srt);
-    N.kept_idx[0] = (int32_t *)(base + o_idx);
-    N.sel[0] = (float4 *)(base + o_sel);
-    if (slots) {
-        N.hash[0] = (NmsSlot *)(base + o_hash);
-        N.next[0] = (int32_t *)(base + o_next);
-    }
+    N.in[0] = d_in;
+    if (slots) N.hash[0] = d_hash, N.next[0] = d_next;
     N.hash_mask = slots - 1;
     N.total = (uint32_t)n;
-    N.keys_a = (uint64_t *)(base + o_ka);
-    N.keys_b = (uint64_t *)(base + o_kb);
-    N.order = (uint32_t *)(base + o_ord);
-    if ((rc = launch_nms(ctx, N, base + o_cub, cub_bytes, launches)) != MULLS_OK) return rc;
+    if ((rc = launch_nms(ctx, N, d_cub, cub_bytes, launches)) != MULLS_OK) return rc;
     // all n entries: one copy instead of a count read-back first; the ones past the kept count are unspecified
     CK(cudaMemcpyAsync(kept_idx, N.kept_idx[0], n * sizeof(int32_t), cudaMemcpyDefault, st));
     CK(cudaMemcpyAsync(&hc, d_cnt, sizeof(hc), cudaMemcpyDeviceToHost, st));
@@ -2985,47 +2968,31 @@ static int classify_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_
     if (sample_in) n = (size_t)P.unground_down_fixed_num;
     const int stride = P.pca_down_rate > 0 ? P.pca_down_rate : 1;
     const size_t row_b = 48;
+    ClsArgs C;
+    std::memset(&C, 0, sizeof(C));
+    float4 *d_in, *d_sel;
+    uint32_t *d_ord;
+    NmsSlot *d_hash;
+    int32_t *d_next;
     ScratchLayout L;
-    const size_t o_in = L.take(n0 * row_b), o_rows = L.take(n0 * row_b);
-    size_t o_cls[4], o_srt[4], o_dn[4], o_dn2[4];
+    L.take(d_in, 3 * n0), L.take(C.rows, 3 * n0);
     for (int c = 0; c < 4; ++c)
-        o_cls[c] = L.take(n0 * row_b), o_srt[c] = L.take(n0 * row_b), o_dn[c] = L.take(n0 * row_b), o_dn2[c] = L.take(n0 * row_b);
-    const size_t o_sect = L.take(2 * n0 * row_b), o_vrows = L.take(n0 * row_b), o_vertex = L.take(n0 * row_b);
-    const size_t o_sel = L.take(4 * n0 * sizeof(float4)), o_ord = L.take(n0 * sizeof(uint32_t));
+        L.take(C.cls[c], 3 * n0), L.take(C.cls_sorted[c], 3 * n0), L.take(C.down[c], 3 * n0), L.take(C.down2[c], 3 * n0);
+    L.take(C.sect, 6 * n0), L.take(C.vrows, 3 * n0), L.take(C.vertex, 3 * n0), L.take(d_sel, 4 * n0), L.take(d_ord, n0);
     // non_max_suppress(cloud, cloud_down, 0.25 * neighbor_searching_radius) (:2236-2255) on the four class clouds
     const float nms_radius = (float)(0.25 * (double)P.neighbor_searching_radius);
     const float nms_r2 = (float)((double)nms_radius * (double)nms_radius);
     const uint32_t nms_slots = nms_hash_slots(n, nms_r2);
-    const size_t o_hash = L.take(4 * (size_t)nms_slots * sizeof(NmsSlot)), o_next = L.take(nms_slots ? 4 * n0 * sizeof(int32_t) : 0);
-    const size_t o_l0 = L.take(n0), o_l = L.take(n0), o_df = L.take(n0), o_s4 = L.take(n0), o_vf = L.take(n0),
-                 o_st = L.take(sizeof(ClsState));
-    char *base;
-    if (const int rc = L.grow(ctx, ctx->cls_buf, base); rc != MULLS_OK) return rc;
-    ClsArgs C;
-    std::memset(&C, 0, sizeof(C));
+    L.take(d_hash, 4 * (size_t)nms_slots), L.take(d_next, nms_slots ? 4 * n0 : 0);
+    L.take(C.label0, n0), L.take(C.label, n0), L.take(C.downflag, n0), L.take(C.st4, n0), L.take(C.vflag, n0), L.take(C.st, 1);
+    if (const int rc = L.grow(ctx, ctx->cls_buf); rc != MULLS_OK) return rc;
     C.P = P;
     C.n = (uint32_t)n;
     C.stride = stride;
-    C.rows = (float4 *)(base + o_rows);
-    for (int c = 0; c < 4; ++c) {
-        C.cls[c] = (float4 *)(base + o_cls[c]);
-        C.cls_sorted[c] = (float4 *)(base + o_srt[c]);
-        C.down[c] = (float4 *)(base + o_dn[c]);
-        C.down2[c] = (float4 *)(base + o_dn2[c]);
-    }
-    C.sect = (float4 *)(base + o_sect);
-    C.vrows = (float4 *)(base + o_vrows);
-    C.vertex = (float4 *)(base + o_vertex);
-    C.label0 = (uint8_t *)(base + o_l0);
-    C.label = (uint8_t *)(base + o_l);
-    C.downflag = (uint8_t *)(base + o_df);
-    C.st4 = (uint8_t *)(base + o_s4);
-    C.vflag = (uint8_t *)(base + o_vf);
-    C.st = (ClsState *)(base + o_st);
     CK(cudaMemsetAsync(C.st, 0, sizeof(ClsState), st));
     if (sample_in) {
-        CK(cudaMemcpyAsync(base + o_in, cloud_in.aos48, n0 * row_b, cudaMemcpyDefault, st)); // host or device rows
-        k_rows_sample<<<1, kClsBlock, 0, st>>>((const float4 *)(base + o_in), (uint32_t)n0, P.unground_down_fixed_num, P.random_seed,
+        CK(cudaMemcpyAsync(d_in, cloud_in.aos48, n0 * row_b, cudaMemcpyDefault, st)); // host or device rows
+        k_rows_sample<<<1, kClsBlock, 0, st>>>(d_in, (uint32_t)n0, P.unground_down_fixed_num, P.random_seed,
                                                18u, C.rows);
         ++launches;
     } else {
@@ -3062,16 +3029,16 @@ static int classify_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_
             N.total = (uint32_t)n;
             N.keys_a = ctx->A.keys_a;
             N.keys_b = ctx->A.keys_b;
-            N.order = (uint32_t *)(base + o_ord);
+            N.order = d_ord;
             for (int c = 0; c < 4; ++c) {
                 if (fixed[c] > 0) N.on_mask |= 1u << c;
                 N.in[c] = C.cls[c];
                 N.sorted[c] = C.cls_sorted[c];
                 N.kept_rows[c] = C.down[c];
-                N.sel[c] = (float4 *)(base + o_sel) + (size_t)c * n0;
+                N.sel[c] = d_sel + (size_t)c * n0;
                 if (nms_slots) {
-                    N.hash[c] = (NmsSlot *)(base + o_hash) + (size_t)c * nms_slots;
-                    N.next[c] = (int32_t *)(base + o_next) + (size_t)c * n0;
+                    N.hash[c] = d_hash + (size_t)c * nms_slots;
+                    N.next[c] = d_next + (size_t)c * n0;
                 }
             }
             if (const int rc = launch_nms(ctx, N, ctx->cub_temp, ctx->cub_temp_bytes, launches); rc != MULLS_OK) return rc;
@@ -3187,36 +3154,18 @@ static int ground_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_gr
     cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, st);
     // per-point scratch
     const size_t row_b = 48;
-    ScratchLayout L;
-    const size_t o_rows = L.take(n * row_b), o_g = L.take(n * row_b), o_gd = L.take(n * row_b), o_u = L.take(n * row_b);
-    const size_t o_key = L.take(4 * n), o_idx = L.take(4 * n), o_keys = L.take(4 * n), o_idxs = L.take(4 * n),
-                 o_call = L.take(4 * n);
-    const size_t o_hf = L.take(4 * n), o_hp = L.take(4 * n), o_dec = L.take(n), o_cand = L.take(16 * n), o_shuf = L.take(4 * n),
-                 o_inl = L.take(n);
-    const size_t o_st = L.take(sizeof(GfState)), o_draws = L.take(kSacDraws * sizeof(uint32_t));
-    const size_t o_tmp = L.take(std::max(sort_bytes, scan_bytes));
-    char *base;
-    if (const int rc = L.grow(ctx, ctx->gf_buf, base); rc != MULLS_OK) return rc;
+    const size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
     GfArgs A;
     std::memset(&A, 0, sizeof(A));
+    void *tmp;
+    ScratchLayout L;
+    L.take(A.rows, 3 * n), L.take(A.out_ground, 3 * n), L.take(A.out_ground_down, 3 * n);
+    L.take(A.out_unground, 3 * n), L.take(A.key, n), L.take(A.idx, n), L.take(A.key_s, n), L.take(A.idx_s, n);
+    L.take(A.cell_all, n), L.take(A.high_flag, n), L.take(A.high_pos, n), L.take(A.decision, n), L.take(A.cand, n);
+    L.take(A.shuf, n), L.take(A.inl, n), L.take(A.st, 1), L.take(A.draws, kSacDraws), L.take_bytes(tmp, tmp_bytes);
+    if (const int rc = L.grow(ctx, ctx->gf_buf); rc != MULLS_OK) return rc;
     A.P = P;
     A.n = (uint32_t)n;
-    A.rows = (const float4 *)(base + o_rows);
-    A.out_ground = (float4 *)(base + o_g);
-    A.out_ground_down = (float4 *)(base + o_gd);
-    A.out_unground = (float4 *)(base + o_u);
-    A.key = (uint32_t *)(base + o_key), A.idx = (uint32_t *)(base + o_idx);
-    A.key_s = (uint32_t *)(base + o_keys), A.idx_s = (uint32_t *)(base + o_idxs);
-    A.cell_all = (int *)(base + o_call);
-    A.high_flag = (uint32_t *)(base + o_hf), A.high_pos = (uint32_t *)(base + o_hp);
-    A.decision = (uint8_t *)(base + o_dec);
-    A.cand = (float4 *)(base + o_cand);
-    A.shuf = (int *)(base + o_shuf);
-    A.inl = (uint8_t *)(base + o_inl);
-    A.st = (GfState *)(base + o_st);
-    A.draws = (const uint32_t *)(base + o_draws);
-    void *tmp = base + o_tmp;
-    size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
     CK(cudaMemcpyAsync((void *)A.rows, cloud_in.aos48, n * row_b, cudaMemcpyDefault, st)); // host or device rows
     CK(cudaMemcpyAsync((void *)A.draws, sac_draw_table(), kSacDraws * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     GfState hs;
@@ -3238,23 +3187,14 @@ static int ground_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, const mulls_gr
     const int num_grid = hs.num_grid;
     if (num_grid > 0) { // (a degenerate cloud with zero extent along x or y has no cell: every point fails the id test)
         const size_t g = (size_t)num_grid;
-        ScratchLayout CL;
-        const size_t c_start = CL.take(4 * g), c_end = CL.take(4 * g), c_minz = CL.take(4 * g), c_nb = CL.take(4 * g),
-                     c_oth = CL.take(4 * g);
-        const size_t c_rel = CL.take(4 * g), c_nrm = CL.take(16 * g), c_ng = CL.take(4 * g), c_nu = CL.take(4 * g),
-                     c_og = CL.take(4 * g), c_ou = CL.take(4 * g);
         size_t cscan = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, cscan, (uint32_t *)nullptr, (uint32_t *)nullptr, num_grid, st);
-        const size_t c_tmp = CL.take(cscan);
-        char *cb;
-        if (const int rc = CL.grow(ctx, ctx->gf_cell_buf, cb); rc != MULLS_OK) return rc;
-        A.cell_start = (uint32_t *)(cb + c_start), A.cell_end = (uint32_t *)(cb + c_end);
-        A.min_z = (float *)(cb + c_minz), A.neighbor_min_z = (float *)(cb + c_nb), A.outlier_thre = (float *)(cb + c_oth);
-        A.reliable = (int *)(cb + c_rel);
-        A.cell_normal = (float4 *)(cb + c_nrm);
-        A.cell_ng = (uint32_t *)(cb + c_ng), A.cell_nu = (uint32_t *)(cb + c_nu);
-        A.cell_og = (uint32_t *)(cb + c_og), A.cell_ou = (uint32_t *)(cb + c_ou);
-        void *ctmp = cb + c_tmp;
+        void *ctmp;
+        ScratchLayout CL;
+        CL.take(A.cell_start, g), CL.take(A.cell_end, g), CL.take(A.min_z, g), CL.take(A.neighbor_min_z, g);
+        CL.take(A.outlier_thre, g), CL.take(A.reliable, g), CL.take(A.cell_normal, g), CL.take(A.cell_ng, g);
+        CL.take(A.cell_nu, g), CL.take(A.cell_og, g), CL.take(A.cell_ou, g), CL.take_bytes(ctmp, cscan);
+        if (const int rc = CL.grow(ctx, ctx->gf_cell_buf); rc != MULLS_OK) return rc;
         CK(cudaMemsetAsync(A.cell_start, 0, 4 * g, st));
         CK(cudaMemsetAsync(A.cell_end, 0, 4 * g, st));
         const unsigned wb = (unsigned)ceil_div(g * 32, kGfBlock), cbk = (unsigned)ceil_div(g, kGfBlock);
@@ -3329,24 +3269,15 @@ static int voxel_impl(mulls_ctx *ctx, mulls_cloud_view cloud_in, float voxel_siz
     cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr,
                                     (uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, 0, 64, st);
     cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, st);
-    ScratchLayout L;
-    const size_t o_rows = L.take(n * row_b), o_out = L.take(n * row_b), o_key = L.take(8 * n), o_keys = L.take(8 * n);
-    const size_t o_idx = L.take(4 * n), o_idxs = L.take(4 * n), o_head = L.take(4 * n), o_pos = L.take(4 * n),
-                 o_st = L.take(sizeof(VxState));
-    const size_t o_tmp = L.take(std::max(sort_bytes, scan_bytes));
-    char *base;
-    if (const int rc = L.grow(ctx, ctx->vx_buf, base); rc != MULLS_OK) return rc;
+    const size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
     VxArgs V;
     V.n = (uint32_t)n;
     V.voxel_size = voxel_size;
-    V.rows = (const float4 *)(base + o_rows);
-    V.out = (float4 *)(base + o_out);
-    V.key = (unsigned long long *)(base + o_key), V.key_s = (unsigned long long *)(base + o_keys);
-    V.idx = (uint32_t *)(base + o_idx), V.idx_s = (uint32_t *)(base + o_idxs);
-    V.head = (uint32_t *)(base + o_head), V.pos = (uint32_t *)(base + o_pos);
-    V.st = (VxState *)(base + o_st);
-    void *tmp = base + o_tmp;
-    const size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
+    void *tmp;
+    ScratchLayout L;
+    L.take(V.rows, 3 * n), L.take(V.out, 3 * n), L.take(V.key, n), L.take(V.key_s, n), L.take(V.idx, n), L.take(V.idx_s, n);
+    L.take(V.head, n), L.take(V.pos, n), L.take(V.st, 1), L.take_bytes(tmp, tmp_bytes);
+    if (const int rc = L.grow(ctx, ctx->vx_buf); rc != MULLS_OK) return rc;
     VxState hs;
     std::memset(&hs, 0, sizeof(hs));
     for (int d = 0; d < 3; ++d) hs.bb[d] = host_ord(FLT_MAX), hs.bb[3 + d] = host_ord(-FLT_MAX);
@@ -3393,9 +3324,11 @@ static int extract_impl(mulls_ctx *ctx, mulls_cloud_view pc_raw, const mulls_ext
     }
     // the clouds handed from stage to stage stay in HBM: pc_down and the ground filter's cloud_unground
     const size_t row_b = 48;
-    int rc = grow_scratch(ctx, ctx->ext_buf, 2 * n * row_b);
+    float *d_down, *d_ung;
+    ScratchLayout L;
+    L.take(d_down, 12 * n), L.take(d_ung, 12 * n);
+    int rc = L.grow(ctx, ctx->ext_buf);
     if (rc != MULLS_OK) return rc;
-    float *d_down = (float *)ctx->ext_buf.p, *d_ung = (float *)((char *)ctx->ext_buf.p + n * row_b);
     // :2346 voxel_downsample(pc_raw, pc_down) (pc_sketch, :2348, is not a feature cloud and is not produced)
     size_t n_down = 0;
     rc = voxel_impl(ctx, pc_raw, params->vf_downsample_resolution, d_down, n, &n_down, launches);
