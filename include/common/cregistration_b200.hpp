@@ -393,6 +393,49 @@ int omp_gicp(constraint_t &registration_cons, float voxel_size = 1.0, Eigen::Mat
     return res.code;
 }
 
+// lo::CRegistration<PointT>::omp_gicp (cregistration.hpp:1024-1098) with using_voxel_gicp = false (point-wise GICP with
+// PCL's BFGS, test/mulls_slam.cpp:637-639 and :674-676 with --voxel_gicp_on=false), the reference's arguments and
+// defaults but using_voxel_gicp and voxel_size, which this mode does not read: target = block1->pc_down, source =
+// block2->pc_down, their local_bounds, on the device (mulls_omp_gicp_pcl, readings in abi.h). max_iter_num caps the BFGS
+// steps of each outer iteration; dis_thre_unit has no effect, as in the reference. Returns 1, or -3 when the fitness
+// exceeds fitness_score_thre, and writes Trans1_2, as the reference does. When the library refuses the call
+// (MULLS_E_UNSUPPORTED: fewer than 20 points in a cloud) *unsupported is set and nothing else is done, so that the
+// caller can run the reference member. Any other library error is logged and returns -3 with Trans1_2 left as it was.
+template <typename PointT>
+int omp_gicp_pcl(constraint_t &registration_cons, int max_iter_num = 20, float dis_thre_unit = 1.5,
+                 Eigen::Matrix4d initial_guess = Eigen::Matrix4d::Identity(), bool apply_intersection_filter = false,
+                 float fitness_score_thre = 10.0, bool *unsupported = nullptr) {
+    (void)dis_thre_unit;
+    const typename pcl::PointCloud<PointT>::Ptr &t = registration_cons.block1->pc_down, &s = registration_cons.block2->pc_down;
+    double guess[16], tb[6], sb[6];
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) guess[4 * r + c] = initial_guess(r, c);
+    const bounds_t &b1 = registration_cons.block1->local_bound, &b2 = registration_cons.block2->local_bound;
+    const double tb_[6] = {b1.min_x, b1.min_y, b1.min_z, b1.max_x, b1.max_y, b1.max_z};
+    const double sb_[6] = {b2.min_x, b2.min_y, b2.min_z, b2.max_x, b2.max_y, b2.max_z};
+    std::memcpy(tb, tb_, sizeof(tb));
+    std::memcpy(sb, sb_, sizeof(sb));
+    if (unsupported) *unsupported = false;
+    mulls_gicp_pcl_result res;
+    // both clouds go through the ingest: both count against the context's target capacity
+    mulls_ctx *ctx = thread_context(s->points.size(), std::max(t->points.size(), s->points.size()));
+    const int rc = ctx ? mulls_omp_gicp_pcl(ctx, view_of<PointT>(t), view_of<PointT>(s), max_iter_num, guess,
+                                            apply_intersection_filter ? 1 : 0, fitness_score_thre, tb, sb, &res, nullptr, 0)
+                       : MULLS_E_CUDA;
+    if (rc == MULLS_E_UNSUPPORTED && unsupported) {
+        *unsupported = true;
+        return -3;
+    }
+    if (rc != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return -3;
+    }
+    LOG(INFO) << "fitness score: " << res.fitness; // base_align, :779
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) registration_cons.Trans1_2(r, c) = res.trans[4 * r + c];
+    return res.code;
+}
+
 } // namespace b200
 } // namespace lo
 #endif

@@ -42,6 +42,8 @@
  *   mulls_omp_ndt            <- lo::CRegistration<PointT>::omp_ndt with use_direct_search (DIRECT7), cregistration.hpp:945-1021
  *   mulls_omp_ndt_batch      <- P independent omp_ndt calls with shared parameters, in one call
  *   mulls_omp_gicp           <- lo::CRegistration<PointT>::omp_gicp with using_voxel_gicp (FastVGICP), cregistration.hpp:1024-1098
+ *   mulls_omp_gicp_pcl       <- lo::CRegistration<PointT>::omp_gicp without using_voxel_gicp (point-wise GICP with PCL's BFGS),
+ *                               cregistration.hpp:1024-1098
  *                               (mulls_voxel_downsample, mulls_fast_ground_filter and mulls_classify_nground also accept
  *                                device pointers for their input rows and output buffers)
  *
@@ -706,6 +708,45 @@ int mulls_omp_gicp(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view sou
                    const double initial_guess[16] /* row-major */, int apply_intersection_filter, float fitness_score_thre,
                    const double target_bound[6], const double source_bound[6], mulls_gicp_result *out, mulls_gicp_iter *trace,
                    int trace_cap);
+
+/* Point-wise GICP registration: lo::CRegistration<PointT>::omp_gicp(reg_con, max_iter_num, dis_thre_unit,
+ * using_voxel_gicp = false, voxel_size, initial_guess, apply_intersection_filter, fitness_score_thre)
+ * (cregistration.hpp:1024-1098), i.e. koide_reg::GeneralizedIterativeClosestPoint (include/baseline_reg/gicp_omp.h,
+ * gicp_omp_impl.hpp) with PCL's BFGS solver: the mode mulls_slam runs with --voxel_gicp_on=false. target = block1->pc_down,
+ * source = block2->pc_down, target_bound / source_bound = block1 / block2 ->local_bound. The readings of the reference
+ * and of PCL's bfgs.h are listed in mulls_b200/csrc/gicp_pcl_core.cuh (P1-P8, B1-B7, C1-C3); in short:
+ *   - prologue, fitness and epilogue: mulls_omp_gicp's; points with a non-finite coordinate are dropped from both clouds;
+ *   - each cloud's covariances from its 20 nearest neighbours (the point itself included), summed in double and
+ *     rebuilt from the SVD's U with (1, 1, 1e-3);
+ *   - up to 200 outer iterations: every source point's exact nearest target, kept within 5 m, with
+ *     M = (R C_src R^T + C_tgt)^-1; then PCL's BFGS over (tx ty tz, X Y Z angles) for at most max_iter_num steps
+ *     (setMaximumOptimizerIterations(max_iter_num), the one argument of omp_gicp this class reads; with
+ *     max_iter_num <= 0 one step is still taken, and a walk that has not finished then ends the loop);
+ *   - the loop stops when the transformation changes by less than rotation / translation epsilons 2e-3 / 5e-4, or
+ *     ends early, unconverged, when fewer than 4 correspondences are found or the solver did not finish;
+ *   - fitness = getFitnessScore(); code -3 when fitness > fitness_score_thre, else 1; Trans1_2 = final * initial_guess
+ *     when the guess moved the source, else final.
+ * Each outer iteration runs one match kernel, an order-preserving compaction and one 4-byte download; each functor call
+ * of the solver runs one evaluation and one tile-sum kernel and downloads 8, 96 or 104 bytes. The solver runs on the
+ * host. The call replaces the resident batch (both clouds go through the ingest). The result has mulls_ndt_result's
+ * fields: iterations = nr_iterations_, converged = converged_. trace (may be NULL with trace_cap 0) receives up to
+ * trace_cap outer iterations. dis_thre_unit and voxel_size have no effect on this class and are not parameters.
+ * Refusals: fewer than 20 points in either cloud after the prologue: MULLS_E_UNSUPPORTED (the reference reads
+ * covariances it never computed there). A NULL output or matrix, NULL rows with n > 0, or trace_cap > 0 without a
+ * trace: MULLS_E_ARG. Either cloud above max_tgt_pts: MULLS_E_CAPACITY. */
+typedef mulls_ndt_result mulls_gicp_pcl_result;
+typedef struct mulls_gicp_pcl_iter {
+    double x[6];       /* the solver's state after the outer iteration: tx ty tz, then the X Y Z angles */
+    double delta;      /* the largest epsilon-scaled change of a transformation entry (converged when < 1) */
+    int n_corr;        /* correspondences of the iteration */
+    int inner_iterations; /* BFGS steps taken (at most max_iter_num, at least 1) */
+    int status;        /* the BFGS status the steps ended on: 0 success, 1 no progress, -1 still running (step cap) */
+    int evaluations;   /* functor calls of the iteration (operator(), df and fdf together) */
+} mulls_gicp_pcl_iter;
+int mulls_omp_gicp_pcl(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view source, int max_iter_num,
+                       const double initial_guess[16] /* row-major */, int apply_intersection_filter, float fitness_score_thre,
+                       const double target_bound[6], const double source_bound[6], mulls_gicp_pcl_result *out,
+                       mulls_gicp_pcl_iter *trace, int trace_cap);
 
 /* The wire format the library ships host clouds in when the "host_pack" tunable is on (csrc/host_pack.h): the 28 of the
  * 48 bytes of a pcl::PointXYZINormal row (utility.hpp:40) that the path reads, repacked on the host cores into pinned

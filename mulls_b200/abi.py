@@ -144,6 +144,22 @@ class GicpIter(C.Structure):
     _fields_ = [("x", C.c_float * 6), ("delta", C.c_float * 6), ("n_corr", C.c_int), ("random_step", C.c_int)]
 
 
+GicpPclResult = NdtResult  # mulls_gicp_pcl_result is a typedef of mulls_ndt_result
+
+
+class GicpPclIter(C.Structure):
+    """mulls_gicp_pcl_iter: one outer iteration of the point-wise GICP (the solver's state after it, the change of the
+    transformation, correspondences, BFGS steps, the BFGS status, functor calls)."""
+    _fields_ = [
+        ("x", C.c_double * 6),
+        ("delta", C.c_double),
+        ("n_corr", C.c_int),
+        ("inner_iterations", C.c_int),
+        ("status", C.c_int),
+        ("evaluations", C.c_int),
+    ]
+
+
 class SorStats(C.Structure):
     """mulls_sor_stats: what pcl::StatisticalOutlierRemoval computed (mean, stddev, threshold) and the point counts."""
     _fields_ = [
@@ -333,6 +349,7 @@ EXPORTED_SYMBOLS = (
     "mulls_omp_ndt",
     "mulls_omp_ndt_batch",
     "mulls_omp_gicp",
+    "mulls_omp_gicp_pcl",
     "mulls_scan_probe",
     "mulls_scan_read",
     "mulls_pose_write",
@@ -430,6 +447,10 @@ def load_library() -> C.CDLL:
     lib.mulls_omp_gicp.argtypes = [vp, CloudView, CloudView, C.c_int, C.c_float, C.POINTER(C.c_double), C.c_int, C.c_float,
                                    C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(GicpResult), C.POINTER(GicpIter),
                                    C.c_int]
+    lib.mulls_omp_gicp_pcl.restype = C.c_int
+    lib.mulls_omp_gicp_pcl.argtypes = [vp, CloudView, CloudView, C.c_int, C.POINTER(C.c_double), C.c_int, C.c_float,
+                                       C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(GicpPclResult),
+                                       C.POINTER(GicpPclIter), C.c_int]
     lib.mulls_pack_rows.restype = C.c_int
     lib.mulls_pack_rows.argtypes = [C.POINTER(C.c_float), C.c_size_t, C.c_int, C.POINTER(C.c_float)]
     lib.mulls_scan_probe.restype = C.c_int

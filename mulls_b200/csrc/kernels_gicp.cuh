@@ -21,9 +21,10 @@ namespace mulls {
 
 constexpr int kGicpCovBlock = 128;
 
-// the raw covariance (6 floats) into cov[9 * input index]; k_gicp_plane regularises it in place
-__global__ void __launch_bounds__(kGicpCovBlock) k_gicp_cov(DeviceArrays A, float *__restrict__ cov) {
-    const int i = blockIdx.x * kGicpCovBlock + threadIdx.x;
+// point i of the ingested cloud (in the grid's order): its kGicpK nearest neighbours (knn_search, FLANN's order), handed
+// to fin(input index, nb) with nb(t, p) the t-th neighbour's x y z. Shared by the covariances of both GICP variants.
+template <class Fin>
+__device__ __forceinline__ void gicp_cov_neighbours(const DeviceArrays &A, int i, Fin fin) {
     const PairConst &pc = A.pc[0];
     const PairState &ps = A.ps[0];
     if (i >= ps.n_tgt[0] || A.hash_used[1]) return;
@@ -31,14 +32,21 @@ __global__ void __launch_bounds__(kGicpCovBlock) k_gicp_cov(DeviceArrays A, floa
     const float4 p = g.pos[i];
     KnnList<kGicpK> kl;
     knn_search(g, p.x, p.y, p.z, kSorStartLevel, kGicpK, kl);
-    float c[6];
-    gicp_raw_covariance([&](int t, float q[3]) {
+    fin(knn_orig(g, i), [&](int t, float q[3]) {
         const float4 v = g.pos[kl.j[t]];
         q[0] = v.x, q[1] = v.y, q[2] = v.z;
-    }, c);
-    float *o = cov + 9 * (size_t)knn_orig(g, i);
+    });
+}
+
+// the raw covariance (6 floats) into cov[9 * input index]; k_gicp_plane regularises it in place
+__global__ void __launch_bounds__(kGicpCovBlock) k_gicp_cov(DeviceArrays A, float *__restrict__ cov) {
+    gicp_cov_neighbours(A, blockIdx.x * kGicpCovBlock + threadIdx.x, [&](int orig, auto nb) {
+        float c[6];
+        gicp_raw_covariance(nb, c);
+        float *o = cov + 9 * (size_t)orig;
 #pragma unroll
-    for (int a = 0; a < 6; ++a) o[a] = c[a];
+        for (int a = 0; a < 6; ++a) o[a] = c[a];
+    });
 }
 
 __global__ void __launch_bounds__(kGicpCovBlock) k_gicp_plane(float *__restrict__ cov, int n) {

@@ -15,6 +15,7 @@
 #include <cub/device/device_run_length_encode.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
 
 #include <dlfcn.h>
 #include <mutex>
@@ -34,6 +35,7 @@
 #include "kernels_ransac.cuh"
 #include "kernels_ndt.cuh"
 #include "kernels_gicp.cuh"
+#include "kernels_gicp_pcl.cuh"
 
 using namespace mulls;
 
@@ -174,6 +176,7 @@ struct mulls_ctx {
     Scratch nms_buf;             // keypoint NMS: rows, sorted rows, keys, sort scratch, cell hash, kept indices
     Scratch ndt_buf;             // NDT: clouds, leaf keys and sort scratch, leaves, tile sums, fitness distances
     Scratch gicp_buf;            // GICP: clouds, covariances, voxel keys and sort scratch, voxels, tile sums, distances
+    Scratch gicp_pcl_buf;        // point-wise GICP: clouds, covariances, correspondences, tile sums, distances
     void *rc_host = nullptr;     // pinned: two chunks of sample triples and their counts
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
@@ -2450,6 +2453,122 @@ int mulls_omp_gicp(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view sou
     return front_call(ctx, [&](uint64_t &launches) {
         return gicp_impl(ctx, target, source, using_voxel_gicp, voxel_size, initial_guess, apply_intersection_filter,
                          fitness_score_thre, target_bound, source_bound, out, trace, trace_cap, launches);
+    });
+}
+
+// ================================================================================================
+// Point-wise GICP registration (CRegistration::omp_gicp without using_voxel_gicp, GeneralizedIterativeClosestPoint with
+// PCL's BFGS): gicp_pcl_core.cuh, kernels_gicp_pcl.cuh
+// ================================================================================================
+static int gicp_pcl_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, int max_iter_num, const double *guess,
+                         int apply_filter, float fitness_thre, const double *tbound, const double *sbound,
+                         mulls_gicp_pcl_result *out, mulls_gicp_pcl_iter *trace, int trace_cap, uint64_t &launches) {
+    if (!out || !guess || !tbound || !sbound || (tv.n && !tv.aos48) || (sv.n && !sv.aos48) || (trace_cap > 0 && !trace))
+        return MULLS_E_ARG;
+    const char *fn = "mulls_omp_gicp_pcl";
+    int rc;
+    // both clouds go through the ingest (their k-nearest covariances)
+    if ((rc = check_capacity(ctx, tv.n, fn)) != MULLS_OK || (rc = check_capacity(ctx, sv.n, fn)) != MULLS_OK) return rc;
+    std::vector<float4> tgt, src;
+    bool moved = false;
+    ndt_prologue(tv.aos48, tv.n, sv.aos48, sv.n, guess, apply_filter, tbound, sbound, tgt, src, moved);
+    gicp_keep_finite(src); // (the prologue keeps the target's finite points only)
+    const int nt = (int)tgt.size(), ns = (int)src.size();
+    if (nt < kGicpK || ns < kGicpK) { // P8
+        ctx->err = std::string(fn) + ": " + std::to_string(nt) + " target and " + std::to_string(ns) +
+                   " source points after the prologue; the covariances need " + std::to_string(kGicpK) + " in each";
+        return MULLS_E_UNSUPPORTED;
+    }
+    cudaStream_t st = ctx->stream;
+    const thrust::counting_iterator<int> iota(0);
+    size_t cub_bytes = 0;
+    CK(cub::DeviceSelect::Flagged(nullptr, cub_bytes, iota, (const int *)nullptr, (int *)nullptr, (int *)nullptr, ns));
+    const int max_tiles = (int)ceil_div((size_t)ns, kNdtTile);
+    float4 *d_t, *d_s;
+    double *d_ct, *d_cs, *d_ts, *d_out; // covariances: 9 doubles per point
+    int *d_flag, *d_tix, *d_list, *d_m;
+    float *d_maha, *d_d2;
+    void *d_cub;
+    ScratchLayout L;
+    L.take(d_t, nt), L.take(d_s, ns), L.take(d_ct, nt * 9ull), L.take(d_cs, ns * 9ull), L.take(d_flag, ns), L.take(d_tix, ns);
+    L.take(d_list, ns), L.take(d_m, 1), L.take(d_maha, ns * 9ull), L.take(d_ts, (size_t)max_tiles * kGicpPclMaxTerms);
+    L.take(d_out, kGicpPclMaxTerms), L.take(d_d2, ns), L.take_bytes(d_cub, cub_bytes);
+    if ((rc = L.grow(ctx, ctx->gicp_pcl_buf)) != MULLS_OK) return rc;
+    CK(cudaMemcpyAsync(d_t, tgt.data(), nt * sizeof(float4), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_s, src.data(), ns * sizeof(float4), cudaMemcpyHostToDevice, st));
+    // P3: the source's covariances, then the target's (its grid stays for the matches and the fitness)
+    DeviceArrays A;
+    if ((rc = ingest_points(ctx, src, A, launches)) != MULLS_OK) return rc;
+    k_gicp_pcl_cov<<<(unsigned)ceil_div(ns, kGicpCovBlock), kGicpCovBlock, 0, st>>>(A, d_cs);
+    k_gicp_pcl_plane<<<(unsigned)ceil_div(ns, kGicpCovBlock), kGicpCovBlock, 0, st>>>(d_cs, ns);
+    if ((rc = ingest_points(ctx, tgt, A, launches)) != MULLS_OK) return rc;
+    k_gicp_pcl_cov<<<(unsigned)ceil_div(nt, kGicpCovBlock), kGicpCovBlock, 0, st>>>(A, d_ct);
+    k_gicp_pcl_plane<<<(unsigned)ceil_div(nt, kGicpCovBlock), kGicpCovBlock, 0, st>>>(d_ct, nt);
+    launches += 4;
+    int err = MULLS_OK;
+    auto fail = [&](cudaError_t e) {
+        if (e == cudaSuccess || err != MULLS_OK) return;
+        ctx->err = std::string(fn) + ": " + cudaGetErrorString(e);
+        err = MULLS_E_CUDA;
+    };
+    int m = 0; // the current correspondences
+    auto match = [&](const float T[12], const double R[9]) {
+        if (err != MULLS_OK) return 0;
+        GicpPclMatchConst MC;
+        std::memcpy(MC.T, T, sizeof(MC.T));
+        std::memcpy(MC.R, R, sizeof(MC.R));
+        k_gicp_pcl_match<<<(unsigned)ceil_div(ns, 128), 128, 0, st>>>(A, d_s, ns, d_cs, d_ct, MC, d_flag, d_tix, d_maha);
+        size_t b = cub_bytes;
+        cudaError_t e = cub::DeviceSelect::Flagged(d_cub, b, iota, (const int *)d_flag, d_list, d_m, ns, st);
+        launches += 2;
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&m, d_m, sizeof(int), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        fail(e);
+        return err == MULLS_OK ? m : 0;
+    };
+    NdtEvalConst E;
+    auto eval = [&](int method, const float T[12], double *r) {
+        const int terms = gicp_pcl_terms(method);
+        for (int c = 0; c < terms; ++c) r[c] = 0.0;
+        if (err != MULLS_OK) return;
+        std::memcpy(E.T, T, sizeof(E.T));
+        const int tiles = (int)ceil_div((size_t)m, kNdtTile);
+        const GicpPclEvalArgs EA{d_s, d_t, d_list, d_tix, d_maha, m, d_ts};
+        if (method == kGicpPclF) k_gicp_pcl_eval<kGicpPclF><<<(unsigned)tiles, kNdtTile, 0, st>>>(EA, E);
+        else if (method == kGicpPclDf) k_gicp_pcl_eval<kGicpPclDf><<<(unsigned)tiles, kNdtTile, 0, st>>>(EA, E);
+        else k_gicp_pcl_eval<kGicpPclFdf><<<(unsigned)tiles, kNdtTile, 0, st>>>(EA, E);
+        k_gicp_pcl_tiles<<<1, 32, 0, st>>>(d_ts, tiles, terms, d_out);
+        launches += 2;
+        cudaError_t e = cudaMemcpyAsync(r, d_out, terms * sizeof(double), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        fail(e);
+    };
+    std::vector<GicpPclIter> tr(trace_cap > 0 ? trace_cap : 0);
+    float T[12];
+    int converged = 0;
+    const int iters = gicp_pcl_walk(max_iter_num, match, eval, T, converged, tr.data(), (int)tr.size());
+    if (err != MULLS_OK) return err;
+    if ((rc = baseline_finish(ctx, &A, d_s, ns, d_d2, T, guess, moved, fitness_thre, out->trans, out->code, out->fitness,
+                              launches)) != MULLS_OK)
+        return rc;
+    out->iterations = iters;
+    out->converged = converged;
+    out->n_target = nt;
+    out->n_source = ns;
+    for (int i = 0; i < std::min(iters, trace_cap); ++i) {
+        for (int c = 0; c < 6; ++c) trace[i].x[c] = tr[i].x[c];
+        trace[i].delta = tr[i].delta, trace[i].n_corr = tr[i].n_corr, trace[i].inner_iterations = tr[i].inner;
+        trace[i].status = tr[i].status, trace[i].evaluations = tr[i].evaluations;
+    }
+    return MULLS_OK;
+}
+int mulls_omp_gicp_pcl(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view source, int max_iter_num,
+                       const double initial_guess[16], int apply_intersection_filter, float fitness_score_thre,
+                       const double target_bound[6], const double source_bound[6], mulls_gicp_pcl_result *out,
+                       mulls_gicp_pcl_iter *trace, int trace_cap) {
+    return front_call(ctx, [&](uint64_t &launches) {
+        return gicp_pcl_impl(ctx, target, source, max_iter_num, initial_guess, apply_intersection_filter, fitness_score_thre,
+                             target_bound, source_bound, out, trace, trace_cap, launches);
     });
 }
 

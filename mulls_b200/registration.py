@@ -108,6 +108,16 @@ def _ndt_out(res, tr, first, trace_cap):
     return out
 
 
+
+def _gicp_pcl_trace(tr, k):
+    """the first k rows of a mulls_gicp_pcl_iter array as numpy arrays"""
+    return dict(x=np.array([tr[i].x[:] for i in range(k)], np.float64).reshape(k, 6),
+                delta=np.array([tr[i].delta for i in range(k)], np.float64),
+                n_corr=np.array([tr[i].n_corr for i in range(k)], np.int32),
+                inner_iterations=np.array([tr[i].inner_iterations for i in range(k)], np.int32),
+                status=np.array([tr[i].status for i in range(k)], np.int32),
+                evaluations=np.array([tr[i].evaluations for i in range(k)], np.int32))
+
 class Context:
     """Thin RAII wrapper of a mulls_ctx (one CUDA device, one stream)."""
 
@@ -476,6 +486,42 @@ class Context:
                                 random_step=np.array([tr[i].random_step for i in range(k)], np.int32))
         return out
 
+    def omp_gicp_pcl(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, max_iter_num: int = 20,
+                     dis_thre_unit: float = 1.5, initial_guess=None, apply_intersection_filter: bool = False,
+                     fitness_score_thre: float = 10.0, trace_cap: int = 0):
+        """CRegistration::omp_gicp with using_voxel_gicp=False (cregistration.hpp:1024-1098, point-wise GICP with PCL's
+        BFGS) on the GPU: target / source are block1 / block2 ->pc_down ((n, 3), (n, 7) or (n, 12) rows), the bounds
+        their local_bound. max_iter_num caps the BFGS steps of each outer iteration, as setMaximumOptimizerIterations
+        does; dis_thre_unit is accepted and ignored, as the reference ignores it. Returns a dict: code (1, or -3 when
+        the fitness exceeds fitness_score_thre), trans (Trans1_2, (4, 4) float64), iterations, converged, fitness,
+        n_target / n_source after the prologue, and with trace_cap > 0 `trace`: per outer iteration the solver's state
+        x (6: tx ty tz, X Y Z angles), delta, the correspondence count, the BFGS steps, the BFGS status and the functor
+        calls. Replaces the resident batch."""
+        del dis_thre_unit  # not read by GeneralizedIterativeClosestPoint
+
+        def aos48(c):  # (n, 3) xyz rows are accepted too: GICP reads positions only
+            c = np.asarray(c, np.float32)
+            if c.ndim == 2 and c.shape[1] == 3:
+                c = np.concatenate([c, np.zeros((len(c), 9), np.float32)], axis=1)
+            return abi.as_aos48(c)
+
+        t, s = aos48(target), aos48(source)
+        g = np.ascontiguousarray(np.eye(4) if initial_guess is None else initial_guess, np.float64).reshape(16).copy()
+        tb = np.ascontiguousarray(target_bound, np.float64).reshape(6).copy()
+        sb = np.ascontiguousarray(source_bound, np.float64).reshape(6).copy()
+        res = abi.GicpPclResult()
+        tr = (abi.GicpPclIter * max(int(trace_cap), 1))()
+        dp = C.POINTER(C.c_double)
+        self._check(self.lib.mulls_omp_gicp_pcl(self.handle, abi.cloud_view(t), abi.cloud_view(s), int(max_iter_num),
+                                                g.ctypes.data_as(dp), int(bool(apply_intersection_filter)),
+                                                float(fitness_score_thre), tb.ctypes.data_as(dp), sb.ctypes.data_as(dp),
+                                                C.byref(res), tr, int(trace_cap)))
+        out = dict(code=res.code, trans=np.array(res.trans[:], np.float64).reshape(4, 4), iterations=res.iterations,
+                   converged=bool(res.converged), fitness=res.fitness, n_target=res.n_target, n_source=res.n_source)
+        if trace_cap > 0:
+            out["trace"] = _gicp_pcl_trace(tr, min(res.iterations, int(trace_cap)))
+        return out
+
     def non_max_suppress(self, cloud: np.ndarray, non_max_radius: float):
         """CFilter::non_max_suppress(cloud_in_out, non_max_radius) (cfilter.hpp:1183-1240) on the GPU. Returns
         (kept_idx, performed): kept_idx is an int32 array of the input rows the reference leaves in the cloud, in its
@@ -685,6 +731,15 @@ class CRegistration:
         block2 = source with their local_bounds. Only the voxelized GICP (using_voxel_gicp=True) runs here."""
         r = self._ctx.omp_gicp(target, source, target_bound, source_bound, max_iter_num, dis_thre_unit, using_voxel_gicp,
                                voxel_size, initial_guess, apply_intersection_filter, fitness_score_thre)
+        return r["code"], r["trans"]
+
+    def omp_gicp_pcl(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, max_iter_num: int = 20,
+                     dis_thre_unit: float = 1.5, initial_guess=None, apply_intersection_filter: bool = False,
+                     fitness_score_thre: float = 10.0):
+        """lo::CRegistration::omp_gicp with using_voxel_gicp=False (cregistration.hpp:1024-1098): returns
+        (code, Trans1_2) for block1 = target and block2 = source with their local_bounds."""
+        r = self._ctx.omp_gicp_pcl(target, source, target_bound, source_bound, max_iter_num, dis_thre_unit, initial_guess,
+                                   apply_intersection_filter, fitness_score_thre)
         return r["code"], r["trans"]
 
     def mm_lls_icp_4dof_global(self, registration_con: Constraint, heading_step_d: float, max_iter_num: int = 20,
