@@ -54,6 +54,21 @@ struct ClsFeat { // pca_feature_t (pca.hpp:23-54): eigenvalues and ratios are do
     float pdir[3], ndir[3];
 };
 
+// The ratios divide by l1, which is 0 for a neighbourhood of identical points. x86 SSE answers 0/0 with the default
+// NaN (0xfff8000000000000, sign set); the device's canonical NaN has the sign clear. The reference's x86 build defines
+// the value, so the device writes that one.
+__device__ __forceinline__ double cls_ratio(double num, double den) {
+    return (num == 0.0 && den == 0.0) ? __longlong_as_double((long long)0xfff8000000000000ull) : num / den;
+}
+
+// (float) of a ratio as cvtsd2ss converts it: a NaN keeps its sign and the top of its payload (0xfff8... -> 0xffc00000).
+// The device's double-to-float conversion is not relied on to keep a NaN's sign.
+__device__ __forceinline__ float cls_to_float(double v) {
+    if (!isnan(v)) return (float)v;
+    const unsigned long long b = (unsigned long long)__double_as_longlong(v);
+    return __uint_as_float(((unsigned)(b >> 32) & 0x80000000u) | 0x7fc00000u | ((unsigned)(b >> 29) & 0x3fffffu));
+}
+
 __device__ __forceinline__ ClsFeat cls_feat(const PcaArgs &F, uint32_t i) {
     ClsFeat f;
     f.pt_num = F.pt_num[i];
@@ -61,9 +76,9 @@ __device__ __forceinline__ ClsFeat cls_feat(const PcaArgs &F, uint32_t i) {
     for (int d = 0; d < 3; ++d) f.pdir[d] = f.ndir[d] = 0.f;
     if (f.pt_num > 3) { // get_pca_feature, pca.hpp:390-434
         const double l1 = F.eigenvalues[3 * (size_t)i], l2 = F.eigenvalues[3 * (size_t)i + 1], l3 = F.eigenvalues[3 * (size_t)i + 2];
-        f.curvature = ((l1 + l2 + l3) == 0) ? 0 : l3 / (l1 + l2 + l3);
-        f.linear_2 = (l1 - l2) / l1;
-        f.planar_2 = (l2 - l3) / l1;
+        f.curvature = ((l1 + l2 + l3) == 0) ? 0 : l3 / (l1 + l2 + l3); // the guard leaves no 0/0
+        f.linear_2 = cls_ratio(l1 - l2, l1);
+        f.planar_2 = cls_ratio(l2 - l3, l1);
         for (int d = 0; d < 3; ++d) f.pdir[d] = F.principal[3 * (size_t)i + d], f.ndir[d] = F.normal[3 * (size_t)i + d];
     }
     return f;
@@ -78,7 +93,7 @@ __global__ void __launch_bounds__(256) k_cls_label(ClsArgs C) {
     float4 *row = C.rows + 3 * (size_t)i;
     const float z = row[0].z;
     float4 nb = row[1];
-    if (f.pt_num > 1) nb = make_float4(f.ndir[0], f.ndir[1], f.ndir[2], (float)f.planar_2);
+    if (f.pt_num > 1) nb = make_float4(f.ndir[0], f.ndir[1], f.ndir[2], cls_to_float(f.planar_2)); // a NaN lands here
     int label = 0, down = 0;
     if (f.pt_num > P.neigh_k_min) {
         if (f.linear_2 > (double)P.edge_thre) {
@@ -87,7 +102,7 @@ __global__ void __launch_bounds__(256) k_cls_label(ClsArgs C) {
                 label = 1;
             else if (az < P.linear_vertical_sin_low_thre && z < P.beam_height_max)
                 label = 2;
-            if (label) nb = make_float4(f.pdir[0], f.pdir[1], f.pdir[2], (float)f.linear_2);
+            if (label) nb = make_float4(f.pdir[0], f.pdir[1], f.pdir[2], cls_to_float(f.linear_2));
             if (!P.sharpen_with_nms && f.linear_2 > (double)P.edge_thre_down) down = label;
         } else if (f.planar_2 > (double)P.planar_thre) {
             const float az = fabsf(f.ndir[2]);
@@ -95,7 +110,7 @@ __global__ void __launch_bounds__(256) k_cls_label(ClsArgs C) {
                 label = 4;
             else if (az < P.planar_vertical_sin_low_thre)
                 label = 3;
-            if (label) nb = make_float4(f.ndir[0], f.ndir[1], f.ndir[2], (float)f.planar_2);
+            if (label) nb = make_float4(f.ndir[0], f.ndir[1], f.ndir[2], cls_to_float(f.planar_2));
             if (!P.sharpen_with_nms && f.planar_2 > (double)P.planar_thre_down) down = label;
         }
     }
@@ -209,6 +224,7 @@ __global__ void __launch_bounds__(256) k_cls_promote_apply(ClsArgs C) {
     const uint8_t s = C.st4[i];
     if (s < 3) return;
     const ClsFeat f = cls_feat(C.F, i);
+    // the curvature is never NaN (cls_feat): the plain conversion is the x86 one
     C.rows[3 * (size_t)i + 1] = make_float4(f.pdir[0], f.pdir[1], f.pdir[2], (float)(5.0 * f.curvature));
     if (s == 4) C.label[i] = 1;
     if (s == 5) C.label[i] = 2;
@@ -278,7 +294,7 @@ __global__ void __launch_bounds__(256) k_cls_encode(ClsArgs C) {
             const int descriptor_2 = r[1] * 1000000 + r[2] * 10000 + r[3] * 100 + r[4];
             const float4 *row = C.rows + 3 * (size_t)i;
             float4 ra = row[0], rb = row[1], rc = row[2];
-            rb.w = (float)f.curvature;
+            rb.w = (float)f.curvature; // never NaN (cls_feat)
             rc.y = (float)descriptor;
             rb.x = (float)descriptor_1;
             rb.y = (float)descriptor_2;
@@ -418,7 +434,10 @@ __global__ void __launch_bounds__(kClsBlock) k_cls_fixed(ClsArgs C) {
                     bool mine = false;
                     if (i < n) {
                         const float4 nb = in[3 * (size_t)i + 1];
-                        double ang = atan2((double)nb.y, (double)nb.x);
+                        // std::atan2(float, float) is the float overload: the angle is rounded to float before the
+                        // double wrap. On a boundary that decides the sector: (+-0, -1) is float(+-pi), sector 2 / 1,
+                        // and (0, -1) is -float(pi / 2), whose wrap lies below 270 degrees, sector 2.
+                        double ang = (double)(float)atan2((double)nb.y, (double)nb.x);
                         if (ang < 0) ang += 2 * M_PI;
                         ang *= (180.0 / M_PI);
                         int sid = (int)(ang / angle_per_sector);

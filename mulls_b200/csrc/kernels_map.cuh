@@ -295,6 +295,8 @@ __global__ void __launch_bounds__(kMapBlock) k_map_revector(const float4 *in, ui
         if (i < n && F.pt_num[i] >= k_min) {
             // pca_feature_t keeps the eigenvalues and the ratios as double (pca.hpp:23-44, :425)
             const double l1 = F.eigenvalues[3 * (size_t)i], l2 = F.eigenvalues[3 * (size_t)i + 1];
+            // identical neighbours give l1 == 0 and a NaN here whose bits differ from the x86 build's; it cannot reach
+            // an output, because a NaN fails the `>` below (the classification writes its ratios: kernels_classify.cuh)
             const double linear_2 = (l1 - l2) / l1;
             const float pz = fabsf(F.principal[3 * (size_t)i + 2]);
             if (linear_2 > (double)min_linearity && (pz > sin_high || pz < sin_low)) {
