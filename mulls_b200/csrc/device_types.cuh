@@ -12,6 +12,11 @@ constexpr int kNumClasses = MULLS_NUM_CLASSES;
 constexpr int kNumSegs = 2 * kNumClasses; // seg = side*6 + class; side 0 = target, 1 = source
 constexpr int kIterBlock = 128;           // threads (= source points) per iteration-kernel block
 constexpr int kIngestBlock = 256;         // input points per ingest block
+constexpr int kSortDigitBits = 9;         // the segment sort: four 9-bit digits of the 36-bit Morton code
+constexpr int kSortBins = 1 << kSortDigitBits;
+constexpr int kSortPasses = 4;
+constexpr int kSortItems = 16;            // points per thread of a sort tile
+constexpr int kSortTile = kIngestBlock * kSortItems;
 constexpr int kTerms = 28;                // 21 lower-tri ATPA + 6 ATPb (+1 pad) per class partial
 constexpr int kMaxLevels = 12;
 constexpr int kCoordBits = 12;            // Morton bits per axis
@@ -126,8 +131,12 @@ struct LoopCtl {
 // All device pointers of a context, passed by value to the kernels.
 struct DeviceArrays {
     const float4 *in_aos;   // input clouds, 3 float4 per point (pcl::PointXYZINormal)
-    uint64_t *keys_a, *keys_b;
-    uint32_t *vals_a, *vals_b;
+    uint64_t *keys_a, *keys_b;       // Morton keys in input order (k_make_keys); the sort passes alternate between the
+                                     // two and leave the sorted keys [pair*12+seg | morton36] in keys_a
+    ChunkDesc *sort_tiles;           // kSortTile input points of one segment per entry, in (pair, segment) order
+    uint32_t *digit_hist;            // [pair][seg][kSortPasses][kSortBins]: digit counts, then each bin's segment offset
+    uint64_t *sort_status;           // [tile][kSortBins]: look-back words of the current sort pass
+    uint32_t *sort_ctr;              // [kSortPasses]: tile fetch counter of each pass
     float4 *tgt_pos, *tgt_nrm;       // target SoA, Morton-sorted inside each (pair,class) slice
     float4 *src_pos[2], *src_nrm[2]; // source SoA ping-pong
     int *src_prevj[2];               // previous NN target (seeds the next search with a real candidate)

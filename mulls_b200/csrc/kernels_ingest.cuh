@@ -10,7 +10,7 @@ namespace mulls {
 // ---- load_input_point: input point `local` of segment `seg`, read from whichever of the three layouts is behind
 //      in_ptr (block-uniform): the caller's 48-byte rows, or the host-packed wire formats (host_pack.h). A source point
 //      gets the motion undistortion and the initial guess (double math, float store,
-//      pcl::transformPointCloudWithNormals semantics). The bbox pass, k_make_keys and k_gather each recompute the point
+//      pcl::transformPointCloudWithNormals semantics). The bbox pass, k_make_keys and the last sort pass each recompute the point
 //      here instead of reading a staged copy: one function, so every recomputation gives the same bits.
 // kUndistort = false: the instantiation for batches in which no pair asks for motion undistortion (no slerp code).
 // kNormals = false: position only (nrm untouched); the position does not depend on the normal, so its bits are the same.
@@ -208,44 +208,71 @@ __global__ void k_pair_setup(DeviceArrays A, int n_pairs) {
     }
 }
 
-// ---- k_make_keys: intersection filter (cfilter.hpp:950-981: strictly inside) + 64-bit sort key
-//      [pair*12+seg | morton36(cell)]; filtered-out points sort to the very end.
+// Morton code of the level-0 cell of p. Targets are inside the grid by construction; sources may stick out (clamped:
+// the source key only orders threads for locality, it never enters a distance decision).
+__device__ __forceinline__ uint64_t cell_morton(const PairState &ps, const float4 &p) {
+    const int hi = (1 << kCoordBits) - 1;
+    const int cx = (int)floorf((p.x - ps.origin[0]) * ps.inv_h0);
+    const int cy = (int)floorf((p.y - ps.origin[1]) * ps.inv_h0);
+    const int cz = (int)floorf((p.z - ps.origin[2]) * ps.inv_h0);
+    return morton36((uint32_t)min(max(cx, 0), hi), (uint32_t)min(max(cy, 0), hi), (uint32_t)min(max(cz, 0), hi));
+}
+
+// ---- digit histograms of the segment sort: a block counts into shared memory (one atomic per warp and distinct digit),
+//      then adds its non-empty bins to the segment's global histogram. Every lane of the warp calls digit_hist_add.
+__device__ __forceinline__ uint32_t *digit_hist_of(const DeviceArrays &A, uint32_t pair, uint32_t seg) {
+    return A.digit_hist + (size_t)(pair * kNumSegs + seg) * (kSortPasses * kSortBins);
+}
+__device__ __forceinline__ void digit_hist_add(uint32_t (*s_hist)[kSortBins], bool on, uint64_t m) {
+    const unsigned lt = (1u << (threadIdx.x & 31)) - 1u;
+#pragma unroll
+    for (int d = 0; d < kSortPasses; ++d) {
+        const uint32_t b = on ? (uint32_t)(m >> (kSortDigitBits * d)) & (kSortBins - 1) : kSortBins;
+        const unsigned peers = __match_any_sync(0xffffffffu, b);
+        if (on && (peers & lt) == 0) atomicAdd(&s_hist[d][b], (unsigned)__popc(peers));
+    }
+}
+__device__ __forceinline__ void digit_hist_flush(uint32_t (*s_hist)[kSortBins], uint32_t *g, bool subtract) {
+    for (int i = threadIdx.x; i < kSortPasses * kSortBins; i += blockDim.x) {
+        const uint32_t c = s_hist[i / kSortBins][i % kSortBins];
+        if (c) atomicAdd(&g[i], subtract ? 0u - c : c);
+    }
+}
+
+// ---- k_make_keys: one block per sort tile. Intersection filter (cfilter.hpp:950-981: strictly inside) + the point's
+//      Morton code into keys_a (~0: filtered out, the point leaves the sort), and the digit histograms of the segment.
 // kFiniteOnly: points with a non-finite coordinate are filtered out as well.
 template <bool kUndistort, bool kFiniteOnly = false>
 __global__ void __launch_bounds__(kIngestBlock) k_make_keys(DeviceArrays A) {
-    const ChunkDesc cd = A.in_chunks[blockIdx.x];
-    const PairConst &pc = A.pc[cd.pair];
-    PairState &ps = A.ps[cd.pair];
-    const uint32_t seg = cd.seg;
-    const uint32_t local = cd.first + threadIdx.x;
-    const bool valid = local < pc.in_n[seg];
-    bool inside = false;
-    if (valid) {
-        const size_t gi = (size_t)pc.in_off[seg] + local;
-        float4 p, unused;
-        load_input_point<kUndistort, false>(pc, seg, local, p, unused);
-        const double *b = ps.ibb;
-        inside = (double)p.x > b[0] && (double)p.x < b[3] && (double)p.y > b[1] && (double)p.y < b[4] &&
-                 (double)p.z > b[2] && (double)p.z < b[5];
-        if (kFiniteOnly) inside = inside && finite_xyz(p);
-        uint64_t key = ~0ull;
-        if (inside) {
-            const int hi = (1 << kCoordBits) - 1;
-            int cx = (int)floorf((p.x - ps.origin[0]) * ps.inv_h0);
-            int cy = (int)floorf((p.y - ps.origin[1]) * ps.inv_h0);
-            int cz = (int)floorf((p.z - ps.origin[2]) * ps.inv_h0);
-            // targets are inside the grid by construction; sources may stick out (clamped: the
-            // source key only orders threads for locality, it never enters a distance decision)
-            cx = min(max(cx, 0), hi);
-            cy = min(max(cy, 0), hi);
-            cz = min(max(cz, 0), hi);
-            key = ((uint64_t)(cd.pair * kNumSegs + seg) << 36) | morton36((uint32_t)cx, (uint32_t)cy, (uint32_t)cz);
+    const ChunkDesc td = A.sort_tiles[blockIdx.x];
+    const PairConst &pc = A.pc[td.pair];
+    PairState &ps = A.ps[td.pair];
+    const uint32_t seg = td.seg;
+    __shared__ uint32_t s_hist[kSortPasses][kSortBins];
+    for (int i = threadIdx.x; i < kSortPasses * kSortBins; i += kIngestBlock) s_hist[i / kSortBins][i % kSortBins] = 0;
+    __syncthreads();
+    unsigned kept = 0;
+#pragma unroll 1
+    for (int k = 0; k < kSortItems; ++k) {
+        const uint32_t local = td.first + k * kIngestBlock + threadIdx.x;
+        bool inside = false;
+        uint64_t m = 0;
+        if (local < pc.in_n[seg]) {
+            float4 p, unused;
+            load_input_point<kUndistort, false>(pc, seg, local, p, unused);
+            const double *b = ps.ibb;
+            inside = (double)p.x > b[0] && (double)p.x < b[3] && (double)p.y > b[1] && (double)p.y < b[4] &&
+                     (double)p.z > b[2] && (double)p.z < b[5];
+            if (kFiniteOnly) inside = inside && finite_xyz(p);
+            if (inside) m = cell_morton(ps, p);
+            A.keys_a[(size_t)pc.in_off[seg] + local] = inside ? m : ~0ull;
         }
-        A.keys_a[gi] = key;
-        A.vals_a[gi] = (uint32_t)gi;
+        digit_hist_add(s_hist, inside, m);
+        kept += (unsigned)__popc(__ballot_sync(0xffffffffu, inside));
     }
-    const unsigned ballot = __ballot_sync(0xffffffffu, inside);
-    if ((threadIdx.x & 31) == 0 && ballot) atomicAdd(&ps.seg_count[seg], (unsigned)__popc(ballot));
+    if ((threadIdx.x & 31) == 0 && kept) atomicAdd(&ps.seg_count[seg], kept);
+    __syncthreads();
+    digit_hist_flush(s_hist, digit_hist_of(A, td.pair, seg), false);
 }
 
 // ---- keep_less_source_pts (cregistration.hpp:2866-2892) -> random_downsample_pcl (cfilter.hpp:606-628) --------
@@ -333,7 +360,8 @@ __global__ void k_keepless_step(DeviceArrays A, int n_pairs, int pass) {
     }
 }
 
-// drop the points whose key exceeds the k-th smallest one (keys are a bijection of the index: exactly k remain)
+// drop the points whose key exceeds the k-th smallest one (keys are a bijection of the index: exactly k remain); their
+// digits leave the segment's histograms
 __global__ void __launch_bounds__(kIngestBlock) k_keepless_mark(DeviceArrays A) {
     const ChunkDesc cd = A.in_chunks[blockIdx.x];
     const PairConst &pc = A.pc[cd.pair];
@@ -341,17 +369,66 @@ __global__ void __launch_bounds__(kIngestBlock) k_keepless_mark(DeviceArrays A) 
     const uint32_t seg = cd.seg;
     const int keep = ps.kl_keep[seg];
     if (keep < 0) return;
+    __shared__ uint32_t s_hist[kSortPasses][kSortBins];
+    for (int i = threadIdx.x; i < kSortPasses * kSortBins; i += kIngestBlock) s_hist[i / kSortBins][i % kSortBins] = 0;
+    __syncthreads();
     const uint32_t local = cd.first + threadIdx.x;
     bool drop = false;
+    uint64_t m = 0;
     if (local < pc.in_n[seg]) {
         const size_t gi = (size_t)pc.in_off[seg] + local;
-        if (A.keys_a[gi] != ~0ull) {
+        m = A.keys_a[gi];
+        if (m != ~0ull) {
             drop = (keep == 0) || sample_key(pc.random_seed, seg, local) > ps.kl_prefix[seg];
             if (drop) A.keys_a[gi] = ~0ull;
         }
     }
+    digit_hist_add(s_hist, drop, m);
     const unsigned b = __ballot_sync(0xffffffffu, drop);
     if ((threadIdx.x & 31) == 0 && b) atomicSub(&ps.seg_count[seg], (unsigned)__popc(b));
+    __syncthreads();
+    digit_hist_flush(s_hist, digit_hist_of(A, cd.pair, seg), true);
+}
+
+// Exclusive scan over a block of kThreads threads (a multiple of 32, at most 1024); *total = the sum of all v.
+template <int kThreads>
+__device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t *s_warp, uint32_t &total) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    uint32_t incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_warp[w] = incl;
+    __syncthreads();
+    if (w == 0) {
+        const uint32_t x = lane < kThreads / 32 ? s_warp[lane] : 0u;
+        uint32_t xi = x;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, xi, o);
+            if (lane >= o) xi += t;
+        }
+        if (lane < kThreads / 32) s_warp[lane] = xi - x;
+        if (lane == 31) s_warp[32] = xi;
+    }
+    __syncthreads();
+    total = s_warp[32];
+    const uint32_t r = s_warp[w] + incl - v;
+    __syncthreads(); // s_warp may be reused
+    return r;
+}
+
+// ---- k_digit_scan: one block per (pair, segment): each digit's counts -> the bin's first position inside the segment
+__global__ void __launch_bounds__(kSortBins) k_digit_scan(DeviceArrays A) {
+    __shared__ uint32_t s_warp[33];
+    uint32_t *h = A.digit_hist + (size_t)blockIdx.x * (kSortPasses * kSortBins);
+    for (int d = 0; d < kSortPasses; ++d) {
+        uint32_t total;
+        const uint32_t v = h[d * kSortBins + threadIdx.x];
+        h[d * kSortBins + threadIdx.x] = block_exclusive_scan<kSortBins>(v, s_warp, total);
+    }
 }
 
 // ---- k_seg_offsets: single block; exclusive scan of the valid counts in (pair, seg) order gives the
@@ -419,11 +496,179 @@ __device__ __forceinline__ int cell_top(const uint64_t *keys, uint32_t i, uint64
     return (63 - __clzll((long long)diff)) / 3;
 }
 
-// ---- k_gather: sorted order -> final SoA slices (targets, and source buffer 0), each point recomputed from the input
-//      by load_input_point (normal .w = the point's index in its input cloud). Also counts the grid cells of every
-//      (pair, class) -> PairState::hash_entries, from which k_hash_layout sizes the tables.
-template <bool kUndistort>
-__global__ void __launch_bounds__(256) k_gather(DeviceArrays A, const uint64_t *keys, const uint32_t *vals, uint32_t n_total) {
+// ---- k_sort_pass: pass kPass of the Morton sort inside every (pair, segment), a stable LSD radix sort by 9-bit digit.
+// The batch is already grouped by segment, so a pass scatters inside the segment's own range: bin b of a tile goes to
+// the segment's start + the bin's offset in the segment (k_digit_scan) + what the segment's earlier tiles put into b.
+// The last comes from a decoupled look-back over those tiles (consecutive in sort_tiles; a block fetches its tile from a
+// counter, so every earlier tile is held by a running block). A tile ranks its points in input order, so equal keys keep
+// the order in which they came: pass 0 reads the keys k_make_keys wrote in input order, the points it keeps are what
+// CUB's stable sort of [pair*12+seg | morton36] ordered. Passes 0-2 write the segment compacted to the front of its input
+// range, each point as one word: the digits still to sort above its 31-bit index in the input cloud. Pass 3 writes the
+// sorted order: the keys [pair*12+seg | morton36] (~0 for the filtered-out points, at the tail) and the SoA slices
+// (targets, and source buffer 0), each point recomputed from the input by load_input_point (normal .w = its index in the
+// input cloud). Look-back word: (2 * epoch + inclusive) << 32 | count; older passes carry smaller epochs.
+struct SortSmem {
+    union {
+        uint32_t warp_bin[kIngestBlock / 32][kSortBins]; // ranking: per warp and bin, its points, then the warps' offsets
+        struct {
+            uint64_t item[kSortTile];                    // the tile in sorted order
+            uint16_t bin[kSortTile];
+        } stage;
+    } u;
+    uint32_t tile_start[kSortBins]; // first position of each bin in the tile's sorted order
+    uint32_t out_base[kSortBins];   // destination of tile position p of bin b: out_base[b] + p
+    uint32_t warp_sum[33];
+    uint32_t tile, n_tile;
+};
+
+template <int kPass>
+__device__ __forceinline__ uint32_t sort_digit(uint64_t e) {
+    return (uint32_t)(kPass == 0 ? e : e >> 31) & (kSortBins - 1);
+}
+
+template <int kPass, bool kUndistort>
+__global__ void __launch_bounds__(kIngestBlock, 3) k_sort_pass(DeviceArrays A, const uint64_t *in, uint64_t *out, int n_pairs,
+                                                            uint32_t epoch) {
+    constexpr bool kLast = kPass == kSortPasses - 1;
+    __shared__ SortSmem s;
+    if (threadIdx.x == 0) s.tile = atomicAdd(&A.sort_ctr[kPass], 1u);
+    for (int i = threadIdx.x; i < (kIngestBlock / 32) * kSortBins; i += kIngestBlock) (&s.u.warp_bin[0][0])[i] = 0;
+    __syncthreads();
+    const uint32_t t = s.tile;
+    const ChunkDesc td = A.sort_tiles[t];
+    const PairConst &pc = A.pc[td.pair];
+    const PairState &ps = A.ps[td.pair];
+    const uint32_t seg = td.seg;
+    const uint32_t n = kPass == 0 ? pc.in_n[seg] : ps.seg_count[seg]; // points of the segment in `in`
+    if (kLast) { // filtered-out points: ~0 keys after the last kept point of the batch
+        const PairState &pl = A.ps[n_pairs - 1];
+        const uint32_t kept = pl.seg_start[kNumSegs - 1] + pl.seg_count[kNumSegs - 1];
+        const uint32_t tail = kept + (pc.in_off[seg] - ps.seg_start[seg]) - n;
+        for (uint32_t i = max(td.first, n) + threadIdx.x; i < min(td.first + kSortTile, pc.in_n[seg]); i += kIngestBlock)
+            out[tail + i] = ~0ull;
+    }
+    if (td.first >= n) return; // block-uniform; no later tile of the segment has points either: nobody looks back here
+    const uint64_t *src = in + pc.in_off[seg];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const unsigned lt = (1u << lane) - 1u;
+    // rank: warp w takes the tile's w-th slice; item j of the lanes is a coalesced row, rows in input order
+    uint64_t item[kSortItems];
+    uint32_t rb[kSortItems]; // rank among the warp's points of the same bin | bin << 16 (bin kSortBins: no point)
+#pragma unroll
+    for (int j = 0; j < kSortItems; ++j) {
+        const uint32_t idx = td.first + (w * kSortItems + j) * 32 + lane;
+        uint64_t e = idx < n ? src[idx] : ~0ull;
+        const bool valid = e != ~0ull; // (no packed word is ~0: it has at most 27 + 31 bits)
+        const uint32_t b = valid ? sort_digit<kPass>(e) : kSortBins;
+        const unsigned peers = __match_any_sync(0xffffffffu, b);
+        uint32_t r = 0;
+        if (valid) r = s.u.warp_bin[w][b] + (uint32_t)__popc(peers & lt);
+        __syncwarp();
+        if (valid && (peers & lt) == 0) s.u.warp_bin[w][b] += (uint32_t)__popc(peers);
+        __syncwarp();
+        if (kPass == 0) e = ((e >> kSortDigitBits) << 31) | idx;
+        else if (!kLast) e = ((e >> (31 + kSortDigitBits)) << 31) | (e & 0x7fffffffu);
+        else e &= 0x7fffffffu;
+        item[j] = e;
+        rb[j] = r | (b << 16);
+    }
+    __syncthreads();
+    // bins 2 tid and 2 tid + 1: the warps' offsets, the tile's counts and their scan
+    uint32_t cnt[2];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        const int b = 2 * threadIdx.x + q;
+        uint32_t run = 0;
+#pragma unroll
+        for (int v = 0; v < kIngestBlock / 32; ++v) {
+            const uint32_t c = s.u.warp_bin[v][b];
+            s.u.warp_bin[v][b] = run;
+            run += c;
+        }
+        cnt[q] = run;
+    }
+    uint32_t n_tile;
+    const uint32_t ex = block_exclusive_scan<kIngestBlock>(cnt[0] + cnt[1], s.warp_sum, n_tile);
+    s.tile_start[2 * threadIdx.x] = ex;
+    s.tile_start[2 * threadIdx.x + 1] = ex + cnt[0];
+    // look-back: publish the tile's counts, add up the earlier tiles' counts until one carries its inclusive prefix
+    volatile uint64_t *status = A.sort_status;
+    const uint64_t agg = (uint64_t)(2u * epoch) << 32, inc = (uint64_t)(2u * epoch + 1u) << 32;
+#pragma unroll
+    for (int q = 0; q < 2; ++q) status[(size_t)t * kSortBins + 2 * threadIdx.x + q] = (td.first == 0 ? inc : agg) | cnt[q];
+    const uint32_t *dig = digit_hist_of(A, td.pair, seg) + kPass * kSortBins;
+    const uint32_t base = kLast ? ps.seg_start[seg] : pc.in_off[seg];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        const int b = 2 * threadIdx.x + q;
+        uint32_t prefix = 0;
+        if (td.first != 0) {
+            for (uint32_t k = t - 1;; --k) {
+                uint64_t v;
+                do v = status[(size_t)k * kSortBins + b];
+                while ((uint32_t)(v >> 32) < 2u * epoch);
+                prefix += (uint32_t)v;
+                if ((uint32_t)(v >> 32) & 1u) break;
+            }
+            status[(size_t)t * kSortBins + b] = inc | (prefix + cnt[q]);
+        }
+        s.out_base[b] = base + dig[b] + prefix - s.tile_start[b];
+    }
+    __syncthreads();
+    uint32_t pos[kSortItems];
+#pragma unroll
+    for (int j = 0; j < kSortItems; ++j) {
+        const uint32_t b = rb[j] >> 16;
+        pos[j] = b < kSortBins ? s.tile_start[b] + s.u.warp_bin[w][b] + (rb[j] & 0xffffu) : 0u;
+    }
+    __syncthreads(); // warp_bin gives way to the staged tile
+#pragma unroll
+    for (int j = 0; j < kSortItems; ++j) {
+        const uint32_t b = rb[j] >> 16;
+        if (b < kSortBins) {
+            s.u.stage.item[pos[j]] = item[j];
+            s.u.stage.bin[pos[j]] = (uint16_t)b;
+        }
+    }
+    __syncthreads();
+    if (!kLast) {
+        for (uint32_t p = threadIdx.x; p < n_tile; p += kIngestBlock) out[s.out_base[s.u.stage.bin[p]] + p] = s.u.stage.item[p];
+        return;
+    }
+    const uint32_t sg = td.pair * kNumSegs + seg;
+    // kGather points per thread at a time: their input rows are all loaded before any of them is stored
+    constexpr int kGather = 4;
+    const uint32_t dst_base = seg < kNumClasses ? pc.tgt_base[seg] : pc.src_base[seg - kNumClasses];
+    const int index_shift = (seg >= kNumClasses && pc.sharded) ? (int)pc.src_index_base[seg - kNumClasses] : 0;
+    float4 *dst_pos = seg < kNumClasses ? A.tgt_pos : A.src_pos[0];
+    float4 *dst_nrm = seg < kNumClasses ? A.tgt_nrm : A.src_nrm[0];
+    // (src_prevj and src_cert need no initial value: iteration 0 reads no previous match, and a certificate is read only
+    // after k_search<1> has written it, kernels_iterate.cuh)
+    for (uint32_t p0 = threadIdx.x; p0 < n_tile; p0 += kGather * kIngestBlock) {
+        float4 pt[kGather], nrm[kGather];
+#pragma unroll
+        for (int g = 0; g < kGather; ++g) {
+            const uint32_t p = p0 + g * kIngestBlock;
+            if (p < n_tile) load_input_point<kUndistort, true>(pc, seg, (uint32_t)s.u.stage.item[p], pt[g], nrm[g]);
+        }
+#pragma unroll
+        for (int g = 0; g < kGather; ++g) {
+            const uint32_t p = p0 + g * kIngestBlock;
+            if (p >= n_tile) break;
+            const uint32_t i = s.out_base[s.u.stage.bin[p]] + p;
+            out[i] = ((uint64_t)sg << 36) | cell_morton(ps, pt[g]);
+            const uint32_t d = dst_base + (i - ps.seg_start[seg]);
+            nrm[g].w = __int_as_float(__float_as_int(nrm[g].w) + index_shift);
+            dst_pos[d] = pt[g];
+            dst_nrm[d] = nrm[g];
+        }
+    }
+}
+
+// ---- k_cell_count: the grid cells of every (pair, class) in the sorted keys -> PairState::hash_entries, from which
+//      k_hash_layout sizes the tables. (Not part of the last sort pass: a cell boundary needs the key before it, and a
+//      tile of that pass does not hold the key before the first point of each of its bins.)
+__global__ void __launch_bounds__(256) k_cell_count(DeviceArrays A, const uint64_t *keys, uint32_t n_total) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const uint64_t key = i < n_total ? keys[i] : ~0ull;
     const uint32_t sg = (uint32_t)(key >> 36);
@@ -439,23 +684,20 @@ __global__ void __launch_bounds__(256) k_gather(DeviceArrays A, const uint64_t *
     } else if (cnt > 0) {
         atomicAdd(&A.ps[pair].hash_entries[seg], (unsigned)cnt);
     }
-    if (key == ~0ull) return;
-    const PairConst &pc = A.pc[pair];
-    float4 pos, nrm;
-    load_input_point<kUndistort, true>(pc, seg, vals[i] - pc.in_off[seg], pos, nrm);
-    const uint32_t local = i - A.ps[pair].seg_start[seg];
-    if (seg < kNumClasses) {
-        const uint32_t d = pc.tgt_base[seg] + local;
-        A.tgt_pos[d] = pos;
-        A.tgt_nrm[d] = nrm;
-    } else {
-        const uint32_t d = pc.src_base[seg - kNumClasses] + local;
-        if (pc.sharded) nrm.w = __int_as_float(__float_as_int(nrm.w) + (int)pc.src_index_base[seg - kNumClasses]);
-        A.src_pos[0][d] = pos;
-        A.src_nrm[0][d] = nrm;
-        // (src_prevj and src_cert need no initial value: iteration 0 reads no previous match, and a certificate is read
-        // only after k_search<1> has written it, kernels_iterate.cuh)
-    }
+}
+
+// Launches sort pass `pass` (k_sort_pass) over the batch's n_tiles sort tiles: keys_a -> keys_b -> keys_a -> keys_b ->
+// keys_a, so the sorted keys end in keys_a. `epoch` counts the context's passes (the look-back words).
+inline void enqueue_sort_pass(const DeviceArrays &A, cudaStream_t st, int pass, unsigned n_tiles, int n_pairs, bool undistort,
+                              uint32_t &epoch) {
+    const uint64_t *in = (pass & 1) ? A.keys_b : A.keys_a;
+    uint64_t *out = (pass & 1) ? A.keys_a : A.keys_b;
+    ++epoch;
+    if (pass == 0) k_sort_pass<0, false><<<n_tiles, kIngestBlock, 0, st>>>(A, in, out, n_pairs, epoch);
+    else if (pass == 1) k_sort_pass<1, false><<<n_tiles, kIngestBlock, 0, st>>>(A, in, out, n_pairs, epoch);
+    else if (pass == 2) k_sort_pass<2, false><<<n_tiles, kIngestBlock, 0, st>>>(A, in, out, n_pairs, epoch);
+    else if (undistort) k_sort_pass<3, true><<<n_tiles, kIngestBlock, 0, st>>>(A, in, out, n_pairs, epoch);
+    else k_sort_pass<3, false><<<n_tiles, kIngestBlock, 0, st>>>(A, in, out, n_pairs, epoch);
 }
 
 // ---- hashed multi-level grid over a target class --------------------------------------------

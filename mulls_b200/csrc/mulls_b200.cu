@@ -104,7 +104,7 @@ struct Scratch {
 struct mulls_ctx {
     int device = 0;
     size_t max_pairs = 0, max_src = 0, max_tgt = 0;
-    size_t cap_src = 0, cap_tgt = 0, cap_in = 0, cap_it_chunks = 0, cap_in_chunks = 0;
+    size_t cap_src = 0, cap_tgt = 0, cap_in = 0, cap_it_chunks = 0, cap_in_chunks = 0, cap_sort_tiles = 0;
     cudaStream_t stream = nullptr;
     DeviceArrays A{};
     void *cub_temp = nullptr;
@@ -116,7 +116,8 @@ struct mulls_ctx {
     std::vector<cudaEvent_t> ev_done;      // one per iteration (launch-loop flow control)
     mulls_icp_trace *d_trace = nullptr;
     std::vector<PairConst> h_pc;
-    std::vector<ChunkDesc> h_in_chunks, h_it_chunks;
+    std::vector<ChunkDesc> h_in_chunks, h_it_chunks, h_sort_tiles;
+    uint32_t sort_epoch = 0; // sort passes run on the context (k_sort_pass look-back words)
     size_t n_pairs = 0, n_in = 0, n_src_total = 0, n_tgt_total = 0;
     int max_iter_max = 0;
     bool uploaded = false;
@@ -346,6 +347,7 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     // every cloud adds at most one partial chunk
     ctx->cap_it_chunks = ceil_div(cs, kIterBlock) + max_pairs * (kNumClasses + 1);
     ctx->cap_in_chunks = ceil_div(cin, kIngestBlock) + max_pairs * kNumSegs;
+    ctx->cap_sort_tiles = ceil_div(cin, kSortTile) + max_pairs * kNumSegs;
     DeviceArrays &A = ctx->A;
     float4 *in = nullptr;
 #define ALLOC(ptr, n)                                                   \
@@ -354,8 +356,10 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     A.in_aos = in;
     ALLOC(A.keys_a, cin);
     ALLOC(A.keys_b, cin);
-    ALLOC(A.vals_a, cin);
-    ALLOC(A.vals_b, cin);
+    ALLOC(A.sort_tiles, ctx->cap_sort_tiles);
+    ALLOC(A.digit_hist, max_pairs * kNumSegs * kSortPasses * kSortBins);
+    ALLOC(A.sort_status, ctx->cap_sort_tiles * kSortBins);
+    ALLOC(A.sort_ctr, kSortPasses);
     ALLOC(A.tgt_pos, ct + kScanOverrun); // (walk_scan_leaf's last group reads past a cell)
     ALLOC(A.tgt_nrm, ct);
     for (int b = 0; b < 2; ++b) {
@@ -418,11 +422,10 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
         return fail("pinned results", e);
     if ((e = cudaMallocHost((void **)&ctx->h_flags, 4 * sizeof(uint32_t))) != cudaSuccess) return fail("pinned flags", e);
     if ((e = cudaMallocHost((void **)&ctx->h_ctl, sizeof(LoopCtl))) != cudaSuccess) return fail("pinned control block", e);
-    // radix-sort temp storage for the largest possible sort
+    // radix-sort temp storage of the keypoint suppression (launch_nms), whose keys live in keys_a / keys_b
     {
         size_t bytes = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, bytes, A.keys_a, A.keys_b, A.vals_a, A.vals_b, (int)cin, 0, 64,
-                                        ctx->stream);
+        cub::DeviceRadixSort::SortKeys(nullptr, bytes, A.keys_a, A.keys_b, (int)cin, 0, 64, ctx->stream);
         ctx->cub_temp_bytes = bytes;
         if ((e = cudaMalloc(&ctx->cub_temp, std::max<size_t>(bytes, 16))) != cudaSuccess) return fail("cub temp", e);
     }
@@ -434,6 +437,9 @@ mulls_ctx *mulls_create(int device, size_t max_pairs, size_t max_src_pts, size_t
     ctx->ev_search.resize(2 * MULLS_MAX_TRACE_ITERS);
     for (auto &ev : ctx->ev_search) cudaEventCreate(&ev);
     if ((e = cudaMemsetAsync(A.ps, 0, max_pairs * sizeof(PairState), ctx->stream)) != cudaSuccess) return fail("memset", e);
+    // look-back words of epoch 0: older than any pass
+    if ((e = cudaMemsetAsync(A.sort_status, 0, ctx->cap_sort_tiles * kSortBins * sizeof(uint64_t), ctx->stream)) != cudaSuccess)
+        return fail("memset", e);
     if ((e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess) return fail("sync", e);
     return ctx;
 }
@@ -627,6 +633,7 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
     ctx->h_pc.assign(n_pairs, PairConst());
     ctx->h_in_chunks.clear();
     ctx->h_it_chunks.clear();
+    ctx->h_sort_tiles.clear();
     size_t in_off = 0, s_off = 0, t_off = 0;
     int max_iter_max = 0;
     bool any_keep_less = false, any_shoot = false, any_undistort = false;
@@ -654,6 +661,8 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
             pc.in_n[s] = (uint32_t)v.n;
             for (size_t f = 0; f < v.n; f += kIngestBlock)
                 ctx->h_in_chunks.push_back(ChunkDesc{(uint32_t)p, (uint32_t)s, (uint32_t)f});
+            for (size_t f = 0; f < v.n; f += kSortTile)
+                ctx->h_sort_tiles.push_back(ChunkDesc{(uint32_t)p, (uint32_t)s, (uint32_t)f});
             in_off += v.n;
         }
         pc.chunk_begin = (uint32_t)ctx->h_it_chunks.size();
@@ -675,7 +684,8 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
         pc.chunk_end = (uint32_t)ctx->h_it_chunks.size();
         pc.sharded = src_index_base ? 1 : 0;
     }
-    if (ctx->h_in_chunks.size() > ctx->cap_in_chunks || ctx->h_it_chunks.size() > ctx->cap_it_chunks) {
+    if (ctx->h_in_chunks.size() > ctx->cap_in_chunks || ctx->h_it_chunks.size() > ctx->cap_it_chunks ||
+        ctx->h_sort_tiles.size() > ctx->cap_sort_tiles) {
         ctx->err = "internal: chunk table capacity";
         return MULLS_E_CAPACITY;
     }
@@ -741,6 +751,9 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
         if (ce == cudaSuccess && !ctx->h_it_chunks.empty())
             ce = cudaMemcpyAsync(ctx->A.it_chunks, ctx->h_it_chunks.data(), ctx->h_it_chunks.size() * sizeof(ChunkDesc),
                                  cudaMemcpyHostToDevice, ctx->stream);
+        if (ce == cudaSuccess && !ctx->h_sort_tiles.empty())
+            ce = cudaMemcpyAsync(ctx->A.sort_tiles, ctx->h_sort_tiles.data(), ctx->h_sort_tiles.size() * sizeof(ChunkDesc),
+                                 cudaMemcpyHostToDevice, ctx->stream);
         tables_sent = true; // (every job is waited for even after an error: the jobs point at `pending`)
         if (ce == cudaSuccess && cudaEventRecord(ctx->ev_h2d0, ctx->stream) == cudaSuccess) ctx->h2d_timed = true;
         const double t_pack0 = wall_ms();
@@ -778,6 +791,9 @@ static int upload_impl(mulls_ctx *ctx, size_t n_pairs, const mulls_cloud_view *t
                                cudaMemcpyHostToDevice, ctx->stream));
         if (!ctx->h_it_chunks.empty())
             CK(cudaMemcpyAsync(ctx->A.it_chunks, ctx->h_it_chunks.data(), ctx->h_it_chunks.size() * sizeof(ChunkDesc),
+                               cudaMemcpyHostToDevice, ctx->stream));
+        if (!ctx->h_sort_tiles.empty())
+            CK(cudaMemcpyAsync(ctx->A.sort_tiles, ctx->h_sort_tiles.data(), ctx->h_sort_tiles.size() * sizeof(ChunkDesc),
                                cudaMemcpyHostToDevice, ctx->stream));
     }
     // The tables above live in pageable vectors: cudaMemcpyAsync has already staged them when it returns. The clouds,
@@ -832,10 +848,13 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
     }
     k_pair_setup<<<(unsigned)ceil_div(np, 128), 128, 0, st>>>(A, np);
     ++launches;
+    const unsigned n_tiles = (unsigned)ctx->h_sort_tiles.size();
     if (n_inc) {
-        if (ctx->any_undistort) k_make_keys<true><<<n_inc, kIngestBlock, 0, st>>>(A);
-        else if (finite_only) k_make_keys<false, true><<<n_inc, kIngestBlock, 0, st>>>(A);
-        else k_make_keys<false><<<n_inc, kIngestBlock, 0, st>>>(A);
+        CK(cudaMemsetAsync(A.digit_hist, 0, (size_t)np * kNumSegs * kSortPasses * kSortBins * sizeof(uint32_t), st));
+        CK(cudaMemsetAsync(A.sort_ctr, 0, kSortPasses * sizeof(uint32_t), st));
+        if (ctx->any_undistort) k_make_keys<true><<<n_tiles, kIngestBlock, 0, st>>>(A);
+        else if (finite_only) k_make_keys<false, true><<<n_tiles, kIngestBlock, 0, st>>>(A);
+        else k_make_keys<false><<<n_tiles, kIngestBlock, 0, st>>>(A);
         ++launches;
         if (ctx->any_keep_less) { // random down-sampling of :2866-2892: radix select of the k-th sampling key
             const unsigned pb = (unsigned)ceil_div(np, 64);
@@ -847,12 +866,11 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
             k_keepless_mark<<<n_inc, kIngestBlock, 0, st>>>(A);
             launches += 18;
         }
-        int seg_bits = 1;
-        while ((1ull << seg_bits) <= (uint64_t)np * kNumSegs) ++seg_bits;
-        size_t bytes = ctx->cub_temp_bytes;
-        CK(cub::DeviceRadixSort::SortPairs(ctx->cub_temp, bytes, A.keys_a, A.keys_b, A.vals_a, A.vals_b, (int)n_in, 0,
-                                           36 + seg_bits, st));
-        // (CUB's radix-sort kernels are library launches and are not counted in kernel_launches)
+        // the Morton order inside every segment: digit offsets, then sort passes 0-2 (pass 3 needs the segment starts)
+        k_digit_scan<<<(unsigned)(np * kNumSegs), kSortBins, 0, st>>>(A);
+        for (int pass = 0; pass < kSortPasses - 1; ++pass)
+            enqueue_sort_pass(A, st, pass, n_tiles, np, ctx->any_undistort, ctx->sort_epoch);
+        launches += kSortPasses;
     }
     k_seg_offsets<<<1, 256, 0, st>>>(A, np);
     ++launches;
@@ -864,12 +882,12 @@ static int launch_ingest(mulls_ctx *ctx, DeviceArrays &A, bool trace, uint64_t &
     }
     if (n_in) {
         const unsigned nb = (unsigned)ceil_div(n_in, 256);
-        if (ctx->any_undistort) k_gather<true><<<nb, 256, 0, st>>>(A, A.keys_b, A.vals_b, n_in);
-        else k_gather<false><<<nb, 256, 0, st>>>(A, A.keys_b, A.vals_b, n_in);
+        enqueue_sort_pass(A, st, kSortPasses - 1, n_tiles, np, ctx->any_undistort, ctx->sort_epoch);
+        k_cell_count<<<nb, 256, 0, st>>>(A, A.keys_a, n_in);
         k_hash_layout<<<1, 32, 0, st>>>(A, np);
         k_hash_clear<<<1184, 256, 0, st>>>(A);
-        k_hash_build<<<nb, 256, 0, st>>>(A, A.keys_b, n_in);
-        launches += 4;
+        k_hash_build<<<nb, 256, 0, st>>>(A, A.keys_a, n_in);
+        launches += 5;
     } else {
         k_hash_layout<<<1, 32, 0, st>>>(A, np);
         ++launches;

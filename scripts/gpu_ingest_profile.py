@@ -20,8 +20,8 @@ runs = int(sys.argv[2]) if len(sys.argv) > 2 else 5
 out_path = sys.argv[3] if len(sys.argv) > 3 else None
 
 # the kernels that run before the iteration loop (launch_ingest), CUB's sort kernels and the claim-table memset included
-INGEST = ("k_state_init", "k_ingest", "k_pair_setup", "k_make_keys", "k_keepless", "k_seg_offsets", "k_gather", "k_hash",
-          "DeviceRadixSort", "Memset")
+INGEST = ("k_state_init", "k_ingest", "k_pair_setup", "k_make_keys", "k_keepless", "k_digit_scan", "k_sort_pass",
+          "k_seg_offsets", "k_cell_count", "k_gather", "k_hash", "DeviceRadixSort", "Memset")
 
 
 def _gen(a):
