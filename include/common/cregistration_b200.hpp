@@ -309,6 +309,45 @@ int omp_ndt(constraint_t &registration_cons, float ndt_resolution = 1.0, Eigen::
     return res.code;
 }
 
+// lo::CRegistration<PointT>::omp_ndt with use_direct_search = false (KDTREE, test/mulls_slam.cpp:634-636 and :671-673
+// with --ndt_searching_method=false), the reference's arguments and defaults but use_direct_search: target =
+// block1->pc_down, source = block2->pc_down, their local_bounds, on the device (mulls_omp_ndt_kdtree, readings in abi.h).
+// Returns 1, or -3 when the fitness exceeds fitness_score_thre, and writes Trans1_2, as the reference does. When the
+// library refuses the call (MULLS_E_UNSUPPORTED) *unsupported is set and nothing else is done, so that the caller can
+// run the reference member. Any other library error is logged and returns -3 with Trans1_2 left as it was.
+template <typename PointT>
+int omp_ndt_kdtree(constraint_t &registration_cons, float ndt_resolution = 1.0,
+                   Eigen::Matrix4d initial_guess = Eigen::Matrix4d::Identity(), bool apply_intersection_filter = true,
+                   float fitness_score_thre = 10.0, bool *unsupported = nullptr) {
+    const typename pcl::PointCloud<PointT>::Ptr &t = registration_cons.block1->pc_down, &s = registration_cons.block2->pc_down;
+    double guess[16], tb[6], sb[6];
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) guess[4 * r + c] = initial_guess(r, c);
+    const bounds_t &b1 = registration_cons.block1->local_bound, &b2 = registration_cons.block2->local_bound;
+    const double tb_[6] = {b1.min_x, b1.min_y, b1.min_z, b1.max_x, b1.max_y, b1.max_z};
+    const double sb_[6] = {b2.min_x, b2.min_y, b2.min_z, b2.max_x, b2.max_y, b2.max_z};
+    std::memcpy(tb, tb_, sizeof(tb));
+    std::memcpy(sb, sb_, sizeof(sb));
+    if (unsupported) *unsupported = false;
+    mulls_ndt_result res;
+    mulls_ctx *ctx = thread_context(s->points.size(), t->points.size());
+    const int rc = ctx ? mulls_omp_ndt_kdtree(ctx, view_of<PointT>(t), view_of<PointT>(s), ndt_resolution, guess,
+                                              apply_intersection_filter ? 1 : 0, fitness_score_thre, tb, sb, &res, nullptr, 0)
+                       : MULLS_E_CUDA;
+    if (rc == MULLS_E_UNSUPPORTED && unsupported) {
+        *unsupported = true;
+        return -3;
+    }
+    if (rc != MULLS_OK) {
+        LOG(ERROR) << "mulls_b200: " << mulls_last_error(ctx);
+        return -3;
+    }
+    LOG(INFO) << "fitness score: " << res.fitness; // base_align, :779
+    for (int r = 0; r < 4; ++r)
+        for (int c = 0; c < 4; ++c) registration_cons.Trans1_2(r, c) = res.trans[4 * r + c];
+    return res.code;
+}
+
 // omp_ndt over every constraint of registration_cons in one call (mulls_omp_ndt_batch), with the arguments of the
 // reference's omp_ndt in its order and with its defaults, shared by all constraints. Each Trans1_2 is written and each
 // code returned as omp_ndt above would for that constraint alone. A library error (use_direct_search = false included:

@@ -40,6 +40,7 @@
  *   mulls_coarse_reg_ransac  <- lo::CRegistration<PointT>::coarse_reg_ransac, cregistration.hpp:604-661
  *   mulls_non_max_suppress   <- lo::CFilter<PointT>::non_max_suppress(cloud_in_out, non_max_radius), cfilter.hpp:1183-1240
  *   mulls_omp_ndt            <- lo::CRegistration<PointT>::omp_ndt with use_direct_search (DIRECT7), cregistration.hpp:945-1021
+ *   mulls_omp_ndt_kdtree     <- lo::CRegistration<PointT>::omp_ndt without use_direct_search (KDTREE), cregistration.hpp:945-1021
  *   mulls_omp_ndt_batch      <- P independent omp_ndt calls with shared parameters, in one call
  *   mulls_omp_gicp           <- lo::CRegistration<PointT>::omp_gicp with using_voxel_gicp (FastVGICP), cregistration.hpp:1024-1098
  *   mulls_omp_gicp_pcl       <- lo::CRegistration<PointT>::omp_gicp without using_voxel_gicp (point-wise GICP with PCL's BFGS),
@@ -625,8 +626,8 @@ int mulls_non_max_suppress(mulls_ctx *ctx, mulls_cloud_view cloud, float non_max
  * The walk runs on the host: one evaluation (a few kernels and one 344-byte download) per iteration. The call replaces
  * the resident batch (the fitness search uses the ingest's grid). iterations = nr_iterations_ (at most 37), converged
  * = converged_. trace (may be NULL with trace_cap 0) receives up to trace_cap iterations: the pose vector after the step,
- * the step length, the score at it and whether the direction was reversed. use_direct_search = 0 (KDTREE): MULLS_E_UNSUPPORTED (the drop-in calls the
- * reference member). A NULL output or matrix, NULL rows with n > 0, or ndt_resolution <= 0: MULLS_E_ARG. A target above
+ * the step length, the score at it and whether the direction was reversed. use_direct_search = 0 (KDTREE): MULLS_E_UNSUPPORTED (mulls_omp_ndt_kdtree runs that
+ * mode; the drop-in calls the reference member). A NULL output or matrix, NULL rows with n > 0, or ndt_resolution <= 0: MULLS_E_ARG. A target above
  * max_tgt_pts or a source above max_src_pts: MULLS_E_CAPACITY. */
 typedef struct mulls_ndt_result {
     double trans[16];  /* Trans1_2, row-major */
@@ -647,6 +648,23 @@ int mulls_omp_ndt(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view sour
                   const double initial_guess[16] /* row-major */, int apply_intersection_filter, float fitness_score_thre,
                   const double target_bound[6], const double source_bound[6], mulls_ndt_result *out, mulls_ndt_iter *trace,
                   int trace_cap);
+
+/* NDT registration with the KDTREE neighbourhood: omp_ndt with use_direct_search = false (test/mulls_slam.cpp with
+ * --ndt_searching_method=false), koide_reg::KDTREE, PCL's original NDT neighbourhood. Everything but the neighbourhood
+ * is mulls_omp_ndt's: the arguments (without use_direct_search), the prologue, the leaves, the walk, the fitness,
+ * Trans1_2, the result and trace types, the codes, the capacities, the refusals and the replaced resident batch. The
+ * readings are K1-K5 in mulls_b200/csrc/ndt_core.cuh; in short:
+ *   - the searchable cloud holds the float centroid (float sum in input order / nr_points) of every leaf with at least
+ *     6 points, in ascending leaf index, including leaves that the eigenvalue check rejects;
+ *   - a source point's neighbours are the centroids at float squared distance d2 < (float)(resolution^2) from its float
+ *     moved position, in (d2, index) order; each contributes with its leaf's double mean and float inverse covariance,
+ *     which is zero for a rejected leaf (it adds -gauss_d1 to the score only);
+ *   - no searchable leaf (empty target, every leaf under 6 points, more than INT32_MAX cells): no neighbours.
+ * Each evaluation runs a radius search kernel per source point before the derivatives. */
+int mulls_omp_ndt_kdtree(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view source, float ndt_resolution,
+                         const double initial_guess[16] /* row-major */, int apply_intersection_filter, float fitness_score_thre,
+                         const double target_bound[6], const double source_bound[6], mulls_ndt_result *out,
+                         mulls_ndt_iter *trace, int trace_cap);
 
 /* A batch of NDT registrations: n_pairs independent mulls_omp_ndt calls in one. ndt_resolution, use_direct_search,
  * apply_intersection_filter and fitness_score_thre are shared by the batch (as the driver's flags are); pair i has its

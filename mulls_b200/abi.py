@@ -347,6 +347,7 @@ EXPORTED_SYMBOLS = (
     "mulls_coarse_reg_ransac",
     "mulls_non_max_suppress",
     "mulls_omp_ndt",
+    "mulls_omp_ndt_kdtree",
     "mulls_omp_ndt_batch",
     "mulls_omp_gicp",
     "mulls_omp_gicp_pcl",
@@ -439,6 +440,10 @@ def load_library() -> C.CDLL:
     lib.mulls_omp_ndt.restype = C.c_int
     lib.mulls_omp_ndt.argtypes = [vp, CloudView, CloudView, C.c_float, C.c_int, C.POINTER(C.c_double), C.c_int, C.c_float,
                                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(NdtResult), C.POINTER(NdtIter), C.c_int]
+    lib.mulls_omp_ndt_kdtree.restype = C.c_int
+    lib.mulls_omp_ndt_kdtree.argtypes = [vp, CloudView, CloudView, C.c_float, C.POINTER(C.c_double), C.c_int, C.c_float,
+                                         C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(NdtResult), C.POINTER(NdtIter),
+                                         C.c_int]
     lib.mulls_omp_ndt_batch.restype = C.c_int
     lib.mulls_omp_ndt_batch.argtypes = [vp, C.c_size_t, C.POINTER(CloudView), C.POINTER(CloudView), C.c_float, C.c_int,
                                         C.POINTER(C.c_double), C.c_int, C.c_float, C.POINTER(C.c_double), C.POINTER(C.c_double),

@@ -8,6 +8,7 @@
 //  - k_ndt_eval: one thread per source point in tiles of kNdtTile: transform, 7 probes, ndt_update per neighbour, then
 //    the tile's sums of the 43 terms in the order of C1 (shuffles inside a warp, then the warps);
 //  - k_ndt_tiles: one thread per term, the tiles' sums in tile order;
+//  - KDTREE (K1-K5): k_ndt_kd_centroids, k_ndt_kd_pack and per evaluation k_ndt_kd_search, k_ndt_eval_kd (below);
 //  - k_ndt_fitness: getFitnessScore's exact unbounded 1-NN squared distance of the moved source (knn_search over the
 //    full-pyramid grid of the target the ingest built), -1 for a point that is not counted.
 #pragma once
@@ -67,6 +68,16 @@ __device__ __forceinline__ int ndt_find_leaf(const uint64_t *keys, int lo, int h
     return (lo < n && keys[lo] == key) ? lo : -1;
 }
 __device__ __forceinline__ int ndt_find_leaf(const uint64_t *keys, int n, uint64_t key) { return ndt_find_leaf(keys, 0, n, key); }
+// the first of keys[0, n) (ascending) that is not below key
+__device__ __forceinline__ int ndt_lower_bound(const uint64_t *keys, int n, uint64_t key) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (keys[mid] < key) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
 
 // N4 for source point p: transform, the 7 probes among the leaves keys[lo, hi) (each key carries `key_hi` above the
 // leaf index: the pair in a batch, 0 for one pair), ndt_update per neighbour into acc
@@ -121,6 +132,124 @@ __global__ void __launch_bounds__(kNdtTile) k_ndt_eval(NdtEvalArgs A, NdtEvalCon
 #pragma unroll
     for (int c = 0; c < kNdtTerms; ++c) acc[c] = 0.0;
     if (i < A.n_src && A.g.ok) ndt_point_terms(A.src[i], A.g, A.leaf_keys, 0, 0, *A.n_leaves, A.leaves, E, acc);
+    tile_tree_store<kNdtTerms>(acc, A.tile_sums);
+}
+
+// ---- KDTREE (mulls_omp_ndt_kdtree, K1-K5 of ndt_core.cuh) --------------------------------------------------------------
+//  - k_ndt_kd_centroids: one thread per leaf (run r, ascending leaf index): the float centroid of a searchable leaf and
+//    the key of its own search cell; other runs and the slots past the last run get the key ~0, which sorts last;
+//  - the (key, run) pairs sorted once per call, k_ndt_kd_pack: the centroids in key order, the run in .w;
+//  - k_ndt_kd_search: one thread per source point per evaluation: the probe box, one contiguous key range per (y, z)
+//    row of it, the exact float test, and the neighbour list in (d2, run) order written to list[k * n_src + i];
+//  - k_ndt_eval_kd: k_ndt_eval's tiles, ndt_update over the point's list in that order.
+constexpr uint64_t kNdtKdNoKey = ~0ull;
+
+__global__ void __launch_bounds__(kNdtKeyBlock) k_ndt_kd_centroids(const float4 *__restrict__ tgt, const uint32_t *__restrict__ order,
+                                                                   const int *__restrict__ offs, const int *__restrict__ counts,
+                                                                   const int *__restrict__ n_runs, int n, NdtGrid g,
+                                                                   float4 *__restrict__ cent, uint64_t *__restrict__ keys,
+                                                                   uint32_t *__restrict__ vals) {
+    const int r = blockIdx.x * kNdtKeyBlock + threadIdx.x;
+    if (r >= n) return;
+    uint64_t key = kNdtKdNoKey;
+    if (r < *n_runs && ndt_kd_searchable(counts[r])) {
+        const int o = offs[r], m = counts[r];
+        float s[3] = {0.f, 0.f, 0.f}, c[3];
+        for (int k = 0; k < m; ++k) {
+            const float4 p = tgt[order[o + k]];
+            s[0] += p.x, s[1] += p.y, s[2] += p.z;
+        }
+        ndt_kd_centroid(s, m, c);
+        cent[r] = make_float4(c[0], c[1], c[2], 0.f);
+        key = (uint64_t)ndt_kd_key(g, ndt_kd_cell(g, c[0], 0), ndt_kd_cell(g, c[1], 1), ndt_kd_cell(g, c[2], 2));
+    }
+    keys[r] = key;
+    vals[r] = (uint32_t)r;
+}
+
+__global__ void __launch_bounds__(kNdtKeyBlock) k_ndt_kd_pack(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ runs,
+                                                              const float4 *__restrict__ cent, int n, float4 *__restrict__ pts) {
+    const int j = blockIdx.x * kNdtKeyBlock + threadIdx.x;
+    if (j >= n || keys[j] == kNdtKdNoKey) return;
+    const float4 c = cent[runs[j]];
+    pts[j] = make_float4(c.x, c.y, c.z, __int_as_float((int)runs[j]));
+}
+
+struct NdtKdArgs {
+    const float4 *src;
+    int n_src;
+    NdtGrid g;
+    float r2, rp;            // K2's r2 and the probe radius r'
+    const uint64_t *keys;    // the sorted centroid keys, kNdtKdNoKey past the searchable ones
+    const float4 *pts;       // the centroids in key order, run index in .w
+    int n_keys;
+    int cap;                 // list entries per point
+    int2 *list;              // [cap][n_src]: (d2 bits, run)
+    int *count;              // [n_src]: the neighbour count, cap or not
+    int *max_count;          // the largest count above cap (0 when every list fits)
+};
+
+__global__ void __launch_bounds__(kNdtTile) k_ndt_kd_search(NdtKdArgs A, NdtEvalConst E) {
+    const int i = blockIdx.x * kNdtTile + threadIdx.x;
+    if (i >= A.n_src) return;
+    int cnt = 0;
+    const float4 p = A.src[i];
+    float t[3];
+    ndt_transform(E.T, p.x, p.y, p.z, t);
+    if (A.g.ok && ndt_finite3(p.x, p.y, p.z) && ndt_finite3(t[0], t[1], t[2])) {
+        int lo[3], hi[3];
+        ndt_kd_box(A.g, A.rp, t, lo, hi);
+        for (int z = lo[2]; z <= hi[2]; ++z)
+            for (int y = lo[1]; y <= hi[1]; ++y) {
+                const uint64_t k0 = (uint64_t)ndt_kd_key(A.g, lo[0], y, z), k1 = (uint64_t)ndt_kd_key(A.g, hi[0], y, z);
+                for (int j = ndt_lower_bound(A.keys, A.n_keys, k0); j < A.n_keys && A.keys[j] <= k1; ++j) {
+                    const float4 c = A.pts[j];
+                    const float d2 = ndt_kd_d2(t, c.x, c.y, c.z);
+                    if (!(d2 < A.r2)) continue;
+                    if (cnt < A.cap) { // insertion in (d2, run) order
+                        const int run = __float_as_int(c.w);
+                        int k = cnt;
+                        for (; k > 0; --k) {
+                            const int2 e = A.list[(size_t)(k - 1) * A.n_src + i];
+                            if (!ndt_kd_before(d2, run, __int_as_float(e.x), e.y)) break;
+                            A.list[(size_t)k * A.n_src + i] = e;
+                        }
+                        A.list[(size_t)k * A.n_src + i] = make_int2(__float_as_int(d2), run);
+                    }
+                    ++cnt;
+                }
+            }
+    }
+    A.count[i] = cnt;
+    if (cnt > A.cap) atomicMax(A.max_count, cnt);
+}
+
+struct NdtKdEvalArgs {
+    const float4 *src;
+    int n_src, cap;
+    const int2 *list;
+    const int *count;
+    const NdtLeaf *leaves;
+    double *tile_sums; // [tiles][kNdtTerms]
+};
+
+__global__ void __launch_bounds__(kNdtTile) k_ndt_eval_kd(NdtKdEvalArgs A, NdtEvalConst E) {
+    const int i = blockIdx.x * kNdtTile + threadIdx.x;
+    double acc[kNdtTerms];
+#pragma unroll
+    for (int c = 0; c < kNdtTerms; ++c) acc[c] = 0.0;
+    if (i < A.n_src) {
+        const int m = min(A.count[i], A.cap);
+        const float4 p = A.src[i];
+        const float x[3] = {p.x, p.y, p.z};
+        float t[3];
+        ndt_transform(E.T, p.x, p.y, p.z, t);
+        for (int k = 0; k < m; ++k) {
+            const NdtLeaf &L = A.leaves[A.list[(size_t)k * A.n_src + i].y];
+            const double xt[3] = {(double)t[0] - L.mean[0], (double)t[1] - L.mean[1], (double)t[2] - L.mean[2]};
+            ndt_update(E, x, xt, L.icov, acc);
+        }
+    }
     tile_tree_store<kNdtTerms>(acc, A.tile_sums);
 }
 

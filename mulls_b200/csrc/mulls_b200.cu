@@ -176,6 +176,7 @@ struct mulls_ctx {
     Scratch rc_buf;              // RANSAC coarse registration: correspondences, hypotheses, counts, refinement state
     Scratch nms_buf;             // keypoint NMS: rows, sorted rows, keys, sort scratch, cell hash, kept indices
     Scratch ndt_buf;             // NDT: clouds, leaf keys and sort scratch, leaves, tile sums, fitness distances
+    Scratch ndt_kd_buf;          // NDT with KDTREE: the per-point neighbour lists, grown to the longest list seen
     Scratch gicp_buf;            // GICP: clouds, covariances, voxel keys and sort scratch, voxels, tile sums, distances
     Scratch gicp_pcl_buf;        // point-wise GICP: clouds, covariances, correspondences, tile sums, distances
     void *rc_host = nullptr;     // pinned: two chunks of sample triples and their counts
@@ -2049,25 +2050,30 @@ static int baseline_finish(mulls_ctx *ctx, const DeviceArrays *A, const float4 *
 }
 
 // ================================================================================================
-// NDT registration (CRegistration::omp_ndt, cregistration.hpp:945-1021, DIRECT7): ndt_core.cuh, kernels_ndt.cuh
+// NDT registration (CRegistration::omp_ndt, cregistration.hpp:945-1021, DIRECT7 or KDTREE): ndt_core.cuh, kernels_ndt.cuh
 // ================================================================================================
-static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, float resolution, int use_direct_search,
+enum class NdtSearch { direct7, kdtree };
+// the neighbour list entries a KDTREE call starts with: most points have fewer; a call whose longest list is longer
+// grows them once, in its first evaluation (tests/test_ndt_kdtree.py's dense_cube scene goes through that path)
+constexpr int kNdtKdListCap = 8;
+
+static bool ndt_args_ok(mulls_cloud_view tv, mulls_cloud_view sv, float resolution, const double *guess, const double *tbound,
+                        const double *sbound, const mulls_ndt_result *out, const mulls_ndt_iter *trace, int trace_cap) {
+    return out && guess && tbound && sbound && (!tv.n || tv.aos48) && (!sv.n || sv.aos48) && resolution > 0.f &&
+           (trace_cap <= 0 || trace);
+}
+
+// the arguments are checked (ndt_args_ok)
+static int ndt_impl(mulls_ctx *ctx, const char *fn, mulls_cloud_view tv, mulls_cloud_view sv, float resolution, NdtSearch search,
                     const double *guess, int apply_filter, float fitness_thre, const double *tbound, const double *sbound,
                     mulls_ndt_result *out, mulls_ndt_iter *trace, int trace_cap, uint64_t &launches) {
-    if (!out || !guess || !tbound || !sbound || (tv.n && !tv.aos48) || (sv.n && !sv.aos48) || !(resolution > 0.f) ||
-        (trace_cap > 0 && !trace))
-        return MULLS_E_ARG;
-    const char *fn = "mulls_omp_ndt";
-    if (!use_direct_search) {
-        ctx->err = std::string(fn) + ": only the DIRECT7 neighbour search runs on the device";
-        return MULLS_E_UNSUPPORTED;
-    }
     int rc;
     if ((rc = check_capacity(ctx, tv.n, fn)) != MULLS_OK) return rc;
     if (sv.n > ctx->max_src) {
         ctx->err = std::string(fn) + ": " + std::to_string(sv.n) + " source points exceed max_src_pts of the context";
         return MULLS_E_CAPACITY;
     }
+    const bool kd = search == NdtSearch::kdtree;
     std::vector<float4> tgt, src;
     bool moved = false;
     ndt_prologue(tv.aos48, tv.n, sv.aos48, sv.n, guess, apply_filter, tbound, sbound, tgt, src, moved);
@@ -2076,10 +2082,10 @@ static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, fl
     cudaStream_t st = ctx->stream;
     size_t cub_bytes = 0;
     if ((rc = sort_runs_bytes(ctx, nt, cub_bytes)) != MULLS_OK) return rc;
-    float4 *d_t, *d_s;
+    float4 *d_t, *d_s, *d_cent, *d_kpts;
     uint64_t *d_ka, *d_kb, *d_uk;
     uint32_t *d_va, *d_vb;
-    int *d_cnt, *d_off, *d_nr;
+    int *d_cnt, *d_off, *d_nr, *d_ncnt;
     NdtLeaf *d_lv;
     double *d_ts, *d_out;
     float *d_d2;
@@ -2088,6 +2094,7 @@ static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, fl
     L.take(d_t, nt), L.take(d_s, ns), L.take(d_ka, nt), L.take(d_kb, nt), L.take(d_va, nt), L.take(d_vb, nt), L.take(d_uk, nt);
     L.take(d_cnt, nt), L.take(d_off, nt), L.take(d_nr, 1), L.take(d_lv, nt), L.take(d_ts, (size_t)tiles * kNdtTerms);
     L.take(d_out, kNdtTerms), L.take(d_d2, ns), L.take_bytes(d_cub, cub_bytes);
+    if (kd) L.take(d_cent, nt), L.take(d_kpts, nt), L.take(d_ncnt, (size_t)ns + 1);
     if ((rc = L.grow(ctx, ctx->ndt_buf)) != MULLS_OK) return rc;
     if (nt) CK(cudaMemcpyAsync(d_t, tgt.data(), nt * sizeof(float4), cudaMemcpyHostToDevice, st));
     if (ns) CK(cudaMemcpyAsync(d_s, src.data(), ns * sizeof(float4), cudaMemcpyHostToDevice, st));
@@ -2097,6 +2104,14 @@ static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, fl
         if ((rc = sort_runs(ctx, d_cub, cub_bytes, nt, d_ka, d_kb, d_va, d_vb, d_uk, d_cnt, d_off, d_nr, st)) != MULLS_OK) return rc;
         k_ndt_leaves<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, d_vb, d_off, d_cnt, d_nr, d_lv);
         launches += 2;
+        if (kd) { // the searchable centroids in the order of their own cells (K1)
+            k_ndt_kd_centroids<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_t, d_vb, d_off, d_cnt, d_nr, nt,
+                                                                                                g, d_cent, d_ka, d_va);
+            size_t b = cub_bytes;
+            CK(cub::DeviceRadixSort::SortPairs(d_cub, b, d_ka, d_kb, d_va, d_vb, nt, 0, 64, st));
+            k_ndt_kd_pack<<<(unsigned)ceil_div(nt, kNdtKeyBlock), kNdtKeyBlock, 0, st>>>(d_kb, d_vb, d_cent, nt, d_kpts);
+            launches += 2;
+        }
     }
     NdtEvalConst E;
     {
@@ -2105,20 +2120,48 @@ static int ndt_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, fl
         E.gauss_d1 = d1, E.gauss_d2 = (float)d2;
     }
     NdtEvalArgs EA{d_s, ns, g, d_uk, d_lv, d_nr, d_ts};
+    // KDTREE: the lists live in their own buffer, so that growing it leaves the leaf tables in place
+    NdtKdArgs KA{d_s, ns, g, ndt_kd_r2(resolution), ndt_kd_probe_radius(resolution), d_kb, d_kpts, nt, 0, nullptr,
+                 d_ncnt, d_ncnt + ns};
+    auto kd_lists = [&](int cap) {
+        const int r = grow_scratch(ctx, ctx->ndt_kd_buf, (size_t)cap * std::max(ns, 1) * sizeof(int2));
+        if (r == MULLS_OK) KA.cap = cap, KA.list = (int2 *)ctx->ndt_kd_buf.p;
+        return r;
+    };
+    if (kd && g.ok && ns > 0 && (rc = kd_lists(kNdtKdListCap)) != MULLS_OK) return rc;
     int err = MULLS_OK;
     auto eval = [&](const double p[6], const float T[12], double r[kNdtTerms]) {
         for (int c = 0; c < kNdtTerms; ++c) r[c] = 0.0;
-        if (err != MULLS_OK || ns == 0) return;
+        if (err != MULLS_OK || ns == 0 || (kd && !g.ok)) return; // K4: no centroids, no neighbours
         std::memcpy(E.T, T, sizeof(E.T));
         ndt_angle_tables(p, E);
-        k_ndt_eval<<<(unsigned)tiles, kNdtTile, 0, st>>>(EA, E);
-        k_ndt_tiles<<<1, 64, 0, st>>>(d_ts, tiles, d_out);
-        launches += 2;
-        cudaError_t e = cudaMemcpyAsync(r, d_out, kNdtTerms * sizeof(double), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) {
-            ctx->err = std::string(fn) + ": " + cudaGetErrorString(e);
-            err = MULLS_E_CUDA;
+        // KDTREE: a point with more neighbours than the lists hold makes the host grow them to the longest list and
+        // evaluate again; the result does not depend on the capacity
+        for (;;) {
+            int longest = 0;
+            cudaError_t e = cudaSuccess;
+            if (!kd) {
+                k_ndt_eval<<<(unsigned)tiles, kNdtTile, 0, st>>>(EA, E);
+                launches += 1;
+            } else {
+                e = cudaMemsetAsync(KA.max_count, 0, sizeof(int), st);
+                k_ndt_kd_search<<<(unsigned)tiles, kNdtTile, 0, st>>>(KA, E);
+                const NdtKdEvalArgs KE{d_s, ns, KA.cap, KA.list, KA.count, d_lv, d_ts};
+                k_ndt_eval_kd<<<(unsigned)tiles, kNdtTile, 0, st>>>(KE, E);
+                launches += 2;
+            }
+            k_ndt_tiles<<<1, 64, 0, st>>>(d_ts, tiles, d_out);
+            launches += 1;
+            if (e == cudaSuccess) e = cudaMemcpyAsync(r, d_out, kNdtTerms * sizeof(double), cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess && kd) e = cudaMemcpyAsync(&longest, KA.max_count, sizeof(int), cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+            if (e != cudaSuccess) {
+                ctx->err = std::string(fn) + ": " + cudaGetErrorString(e);
+                err = MULLS_E_CUDA;
+                return;
+            }
+            if (longest <= KA.cap) return;
+            if ((err = kd_lists(longest)) != MULLS_OK) return;
         }
     };
     std::vector<NdtIter> tr(trace_cap > 0 ? trace_cap : 0);
@@ -2147,8 +2190,25 @@ int mulls_omp_ndt(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view sour
                   const double target_bound[6], const double source_bound[6], mulls_ndt_result *out, mulls_ndt_iter *trace,
                   int trace_cap) {
     return front_call(ctx, [&](uint64_t &launches) {
-        return ndt_impl(ctx, target, source, ndt_resolution, use_direct_search, initial_guess, apply_intersection_filter,
-                        fitness_score_thre, target_bound, source_bound, out, trace, trace_cap, launches);
+        if (!ndt_args_ok(target, source, ndt_resolution, initial_guess, target_bound, source_bound, out, trace, trace_cap))
+            return (int)MULLS_E_ARG;
+        if (!use_direct_search) {
+            ctx->err = "mulls_omp_ndt: only the DIRECT7 neighbour search runs on the device (KDTREE: mulls_omp_ndt_kdtree)";
+            return (int)MULLS_E_UNSUPPORTED;
+        }
+        return ndt_impl(ctx, "mulls_omp_ndt", target, source, ndt_resolution, NdtSearch::direct7, initial_guess,
+                        apply_intersection_filter, fitness_score_thre, target_bound, source_bound, out, trace, trace_cap, launches);
+    });
+}
+int mulls_omp_ndt_kdtree(mulls_ctx *ctx, mulls_cloud_view target, mulls_cloud_view source, float ndt_resolution,
+                         const double initial_guess[16], int apply_intersection_filter, float fitness_score_thre,
+                         const double target_bound[6], const double source_bound[6], mulls_ndt_result *out,
+                         mulls_ndt_iter *trace, int trace_cap) {
+    return front_call(ctx, [&](uint64_t &launches) {
+        if (!ndt_args_ok(target, source, ndt_resolution, initial_guess, target_bound, source_bound, out, trace, trace_cap))
+            return (int)MULLS_E_ARG;
+        return ndt_impl(ctx, "mulls_omp_ndt_kdtree", target, source, ndt_resolution, NdtSearch::kdtree, initial_guess,
+                        apply_intersection_filter, fitness_score_thre, target_bound, source_bound, out, trace, trace_cap, launches);
     });
 }
 

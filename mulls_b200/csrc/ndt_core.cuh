@@ -33,6 +33,43 @@
 //     Newton point.
 //  N6 non-finite coordinates: left out of the min/max, the leaves, the derivatives and the fitness count (PCL's
 //     non-dense branches).
+// With use_direct_search = false omp_ndt selects koide_reg::KDTREE, PCL's original neighbourhood (mulls_omp_ndt_kdtree).
+// Read from the same files and PCL 1.10 / FLANN 1.9, not run, as N1-N6:
+//  K1 the searchable cloud (voxel_grid_covariance_omp_impl.hpp:283-327): one centroid per leaf with nr_points >= 6, in
+//     ascending leaf index (std::map order), pushed before the eigenvalue and infinite-inverse checks, so a leaf rejected
+//     afterwards (nr_points = -1) stays in the kd-tree. Its xyz is the float sum of the leaf's points in input order
+//     divided by (float)nr_points (:175-201, :290), not the double mean_ (ndt_kd_centroid).
+//  K2 the search (voxel_grid_covariance_omp.h:472-499, pcl::KdTreeFLANN::radiusSearch over FLANN's KDTreeSingleIndex with
+//     L2_Simple<float>): the query is the float moved point, xyz only; r2 = (float)((double)resolution * resolution);
+//     d2 = (dx*dx + dy*dy) + dz*dz in float without contraction; a centroid is a neighbour iff d2 < r2; max_nn = 0
+//     returns all neighbours, sorted by (distance, index) (RadiusResultSet's sorted copy, DistanceIndex::operator<), as
+//     kernels_pca.cuh reads radiusSearch. The index is the rank among the searchable leaves, so ascending index is
+//     ascending leaf index.
+//  K3 the contributions (ndt_omp_impl.hpp:233-270): the KDTREE branch never checks nr_points; every neighbour goes
+//     through ndt_update with the leaf's double mean and float icov as the finalisation leaves them. A leaf rejected by
+//     its eigenvalues keeps icov_ = 0 (Leaf(), voxel_grid_covariance_omp.h:98-107): it adds -d1 to the score (gauss_d2
+//     <= 1) and nothing to the gradient or Hessian. DIRECT7 never sees those leaves (6 or more equal points, an exactly
+//     planar leaf whose smallest eigenvalue rounds below zero), so on such targets the score traces of the two modes
+//     differ. The reference's infinite-inverse rejection keeps the computed inverse; ndt_leaf_finish leaves icov zero
+//     there instead, because no float input reaches it: after the eigenvalue check and the inflation every eigenvalue of
+//     the covariance is at least 0.01 of the largest, ev2 > 0, so an inverse entry is at most about 100 / ev2 and
+//     overflows only for ev2 below about 1e-306; a covariance of float points that are not all equal (equal points
+//     give exactly 0 and the eigenvalue rejection) is of the order of their spread squared or of the rounding of
+//     their squares, both above 2^-300 (products of floats are multiples of 2^-298).
+//  K4 no centroids (empty target, every leaf under 6 points, more than INT32_MAX cells): the reference searches an index
+//     it never built (undefined); here no point has neighbours, as DIRECT7's empty-target rule says.
+//  K5 everything else is the DIRECT7 path: the prologue, N1-N2, the walk and its constants (N5), C1, C2, the fitness,
+//     Trans1_2 and the codes. Only the neighbourhood changes.
+// The device search (kernels_ndt.cuh) keys every centroid by the cell of its own float coordinates on the leaf grid,
+// clamped to [min_b, max_b] (ndt_kd_cell), and probes for a query t the cells from ndt_kd_cell(t - r') to
+// ndt_kd_cell(t + r') per axis, r' = resolution (1 + 2^-16) in float. The box holds every neighbour: d2 < r2 gives
+// fl(dx^2) <= d2 < r2 <= r^2 (1 + u) (sums of non-negative terms round to at least each term), so |dx| < r (1 + u) and
+// |t - c| < r (1 + 3u) per axis, u = 2^-24, while r' >= r (1 + 2^-16 - 2^-24) exceeds that (r2 a normal float, i.e. a
+// resolution above 1.1e-19). Then t - r' <= c <= t + r' exactly, and float rounding, the product by inv, floor, the
+// saturating cast and the clamp are all monotone, so the centroid's cell lies in the box on every axis. A box spans 3
+// cells per axis (4 where rounding reaches a face). Each centroid lies in its own leaf up to rounding, and a ball of
+// radius r meets at most 27 cells of edge r, so a list rarely exceeds 27; it has no bound in general (a float sum of
+// many points can drift), so the host grows the list capacity when a count exceeds it and repeats the evaluation.
 // Choices where the reference depends on the machine (OpenMP partial sums, Eigen's vectorised products):
 //  C1 the points' contributions are summed in tiles of kNdtTile points in index order: within a tile a pairwise tree
 //     q[t] += q[t + s] for s = 16 .. 1 inside each group of 32, then over the kNdtTile / 32 group sums for s = 2, 1; then
@@ -263,6 +300,39 @@ GF_HD NdtLeaf ndt_leaf_finish(const double s[3], const double c[9], int n) {
         for (int j = 0; j < 3; ++j) L.icov[3 * i + j] = (float)ic[i][j];
     L.ok = 1;
     return L;
+}
+
+// ---- K1/K2: the KDTREE neighbourhood ---------------------------------------------------------------------------------
+// a leaf of n points (before the checks) is in the searchable cloud
+GF_HD bool ndt_kd_searchable(int n_points) { return n_points >= kNdtMinPoints; }
+
+// K1: the float centroid of a leaf from the float sums of its points in input order
+GF_HD void ndt_kd_centroid(const float s[3], int n, float c[3]) {
+    for (int a = 0; a < 3; ++a) c[a] = s[a] / (float)n;
+}
+
+// K2: the search radius squared, and radiusSearch's float distance of query q to centroid c
+GF_HD float ndt_kd_r2(float resolution) { return (float)((double)resolution * (double)resolution); }
+GF_HD float ndt_kd_d2(const float q[3], float cx, float cy, float cz) {
+    const float dx = q[0] - cx, dy = q[1] - cy, dz = q[2] - cz;
+    return (dx * dx + dy * dy) + dz * dz;
+}
+// (d2, index) order
+GF_HD bool ndt_kd_before(float d2a, int ia, float d2b, int ib) { return d2a < d2b || (d2a == d2b && ia < ib); }
+
+// the search cell of coordinate v on axis a: the leaf grid's cell of v itself, clamped to [min_b, max_b] (monotone in v)
+GF_HD int ndt_kd_cell(const NdtGrid &g, float v, int a) {
+    const int c = ndt_f2i(floorf(v * g.inv));
+    return c < g.min_b[a] ? g.min_b[a] : (c > g.max_b[a] ? g.max_b[a] : c);
+}
+GF_HD int64_t ndt_kd_key(const NdtGrid &g, int c0, int c1, int c2) {
+    return ((int64_t)c0 - g.min_b[0]) * g.divb_mul[0] + ((int64_t)c1 - g.min_b[1]) * g.divb_mul[1] +
+           ((int64_t)c2 - g.min_b[2]) * g.divb_mul[2];
+}
+// the probe box of query t: cells lo[a] .. hi[a] per axis (the header's argument: it holds every c with d2 < r2)
+GF_HD float ndt_kd_probe_radius(float resolution) { return resolution * (1.0f + 1.0f / 65536.0f); }
+GF_HD void ndt_kd_box(const NdtGrid &g, float rp, const float t[3], int lo[3], int hi[3]) {
+    for (int a = 0; a < 3; ++a) lo[a] = ndt_kd_cell(g, t[a] - rp, a), hi[a] = ndt_kd_cell(g, t[a] + rp, a);
 }
 
 // ---- N4: the derivatives ---------------------------------------------------------------------------------------------

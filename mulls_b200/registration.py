@@ -406,7 +406,8 @@ class Context:
         ->pc_down ((n, 3), (n, 7) or (n, 12) rows), the bounds their local_bound (min_x min_y min_z max_x max_y max_z). Returns a dict: code (1, or -3 when
         the fitness exceeds fitness_score_thre), trans (Trans1_2, (4, 4) float64), iterations, converged, fitness,
         n_target / n_source after the intersection filter, and with trace_cap > 0 `trace`: per iteration the pose vector
-        p (6), the step length, the score and whether the direction was reversed. use_direct_search=False (KDTREE) raises. Replaces the resident batch."""
+        p (6), the step length, the score and whether the direction was reversed. use_direct_search=False (KDTREE) raises:
+        omp_ndt_kdtree runs that mode. Replaces the resident batch."""
         t, s = _xyz_rows(target), _xyz_rows(source)
         g = np.ascontiguousarray(np.eye(4) if initial_guess is None else initial_guess, np.float64).reshape(16).copy()
         tb = np.ascontiguousarray(target_bound, np.float64).reshape(6).copy()
@@ -418,6 +419,25 @@ class Context:
                                            int(bool(use_direct_search)), g.ctypes.data_as(dp), int(bool(apply_intersection_filter)),
                                            float(fitness_score_thre), tb.ctypes.data_as(dp), sb.ctypes.data_as(dp), C.byref(res),
                                            tr, int(trace_cap)))
+        return _ndt_out(res, tr, 0, trace_cap)
+
+    def omp_ndt_kdtree(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, ndt_resolution: float = 1.0,
+                       initial_guess=None, apply_intersection_filter: bool = True, fitness_score_thre: float = 10.0,
+                       trace_cap: int = 0):
+        """CRegistration::omp_ndt with use_direct_search=False (KDTREE, mulls_omp_ndt_kdtree) on the GPU: every leaf
+        centroid within ndt_resolution of a moved source point is its neighbour, as PCL's radius search finds them.
+        omp_ndt's arguments without use_direct_search; returns the dict omp_ndt returns. Replaces the resident batch."""
+        t, s = _xyz_rows(target), _xyz_rows(source)
+        g = np.ascontiguousarray(np.eye(4) if initial_guess is None else initial_guess, np.float64).reshape(16).copy()
+        tb = np.ascontiguousarray(target_bound, np.float64).reshape(6).copy()
+        sb = np.ascontiguousarray(source_bound, np.float64).reshape(6).copy()
+        res = abi.NdtResult()
+        tr = (abi.NdtIter * max(int(trace_cap), 1))()
+        dp = C.POINTER(C.c_double)
+        self._check(self.lib.mulls_omp_ndt_kdtree(self.handle, abi.cloud_view(t), abi.cloud_view(s), float(ndt_resolution),
+                                                  g.ctypes.data_as(dp), int(bool(apply_intersection_filter)),
+                                                  float(fitness_score_thre), tb.ctypes.data_as(dp), sb.ctypes.data_as(dp),
+                                                  C.byref(res), tr, int(trace_cap)))
         return _ndt_out(res, tr, 0, trace_cap)
 
     def omp_ndt_batch(self, targets, sources, target_bounds, source_bounds, ndt_resolution: float = 1.0,
@@ -699,9 +719,18 @@ class CRegistration:
                 use_direct_search: bool = True, initial_guess=None, apply_intersection_filter: bool = True,
                 fitness_score_thre: float = 10.0):
         """lo::CRegistration::omp_ndt (cregistration.hpp:945-1021): returns (code, Trans1_2) for block1 = target and
-        block2 = source with their local_bounds. Only the DIRECT7 search (use_direct_search=True) runs here."""
+        block2 = source with their local_bounds. Only the DIRECT7 search (use_direct_search=True) runs here; omp_ndt_kdtree
+        runs KDTREE."""
         r = self._ctx.omp_ndt(target, source, target_bound, source_bound, ndt_resolution, use_direct_search, initial_guess,
                               apply_intersection_filter, fitness_score_thre)
+        return r["code"], r["trans"]
+
+    def omp_ndt_kdtree(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, ndt_resolution: float = 1.0,
+                       initial_guess=None, apply_intersection_filter: bool = True, fitness_score_thre: float = 10.0):
+        """lo::CRegistration::omp_ndt with use_direct_search=False (KDTREE): returns (code, Trans1_2) for block1 = target
+        and block2 = source with their local_bounds."""
+        r = self._ctx.omp_ndt_kdtree(target, source, target_bound, source_bound, ndt_resolution, initial_guess,
+                                     apply_intersection_filter, fitness_score_thre)
         return r["code"], r["trans"]
 
     def omp_ndt_batch(self, registration_cons, ndt_resolution: float = 1.0, use_direct_search: bool = True,
