@@ -11,9 +11,10 @@
 //     CRegistration_reference — every member the reference defines stays available, unchanged;
 //   * lo::CRegistration<PointT> is then defined HERE as a class derived from it whose mm_lls_icp
 //     (cregistration.hpp:1114-1123: same name, argument order, types and defaults) and mm_lls_icp_4dof_global
-//     (:1584-1592), find_feature_correspondence_ncc (:409-411), coarse_reg_ransac (:605-607), omp_ndt (:945-947) and
-//     omp_gicp (:1024-1027) run on the GPU through the C-ABI (include/mulls_b200/abi.h). All other public members the callers use
-//     — determine_source_target_cloud, assign_source_target_cloud, coarse_reg_teaser,
+//     (:1584-1592), find_feature_correspondence_ncc (:409-411), coarse_reg_ransac (:605-607), coarse_reg_teaser
+//     (:664-666), omp_ndt (:945-947) and omp_gicp (:1024-1027) run on the GPU through the C-ABI
+//     (include/mulls_b200/abi.h); coarse_reg_teaser runs whether or not the reference was built with TEASER_ON. All
+//     other public members the callers use — determine_source_target_cloud, assign_source_target_cloud,
 //     ... (SURVEY.md section 8b) — are inherited from the reference; every overload of
 //     coarse_reg_ransac the reference class declares stays visible next to the device one.
 // Differences in contract are listed in INTEGRATION.md (block1->tree_* are not populated: use mulls_nn_query or
@@ -82,6 +83,11 @@ class CRegistration : public CRegistration_reference<PointT> {
     int coarse_reg_ransac(const typename pcl::PointCloud<PointT>::Ptr &target_pts, const typename pcl::PointCloud<PointT>::Ptr &source_pts,
                           Eigen::Matrix4d &tran_mat, float noise_bound = 0.2, int min_inlier_num = 8, int max_iter_num = 20000) {
         return b200::coarse_reg_ransac<PointT>(target_pts, source_pts, tran_mat, noise_bound, min_inlier_num, max_iter_num);
+    }
+    // cregistration.hpp:664-666 (the reference declares one overload)
+    int coarse_reg_teaser(const typename pcl::PointCloud<PointT>::Ptr &target_pts, const typename pcl::PointCloud<PointT>::Ptr &source_pts,
+                          Eigen::Matrix4d &tran_mat, float noise_bound = 0.2, int min_inlier_num = 8) {
+        return b200::coarse_reg_teaser<PointT>(target_pts, source_pts, tran_mat, noise_bound, min_inlier_num);
     }
     // cregistration.hpp:945-947. The device runs the DIRECT7 neighbourhood; KDTREE (use_direct_search = false) is the
     // reference member. A template on the guess type, so that the class compiles against a reference build that does

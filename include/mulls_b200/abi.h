@@ -38,6 +38,7 @@
  *                               cfilter.hpp:470-549
  *   mulls_ncc_correspondences <- lo::CRegistration<PointT>::find_feature_correspondence_ncc, cregistration.hpp:409-601
  *   mulls_coarse_reg_ransac  <- lo::CRegistration<PointT>::coarse_reg_ransac, cregistration.hpp:604-661
+ *   mulls_coarse_reg_teaser  <- lo::CRegistration<PointT>::coarse_reg_teaser, cregistration.hpp:664-759
  *   mulls_non_max_suppress   <- lo::CFilter<PointT>::non_max_suppress(cloud_in_out, non_max_radius), cfilter.hpp:1183-1240
  *   mulls_omp_ndt            <- lo::CRegistration<PointT>::omp_ndt with use_direct_search (DIRECT7), cregistration.hpp:945-1021
  *   mulls_omp_ndt_kdtree     <- lo::CRegistration<PointT>::omp_ndt without use_direct_search (KDTREE), cregistration.hpp:945-1021
@@ -579,6 +580,48 @@ int mulls_ncc_correspondences(mulls_ctx *ctx, mulls_cloud_view target_kpts, mull
 int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_cloud_view source_pts, float noise_bound,
                             int min_inlier_num, int max_iter_num, double tran_mat[16] /* row-major, written only when status >= 0 */,
                             int *status, int *n_inliers, int *n_hypotheses);
+
+/* lo::CRegistration<PointT>::coarse_reg_teaser(target_pts, source_pts, tran_mat, noise_bound, min_inlier_num),
+ * cregistration.hpp:664-759: the coarse transform of the global registration with --teaser_on / the default
+ * --teaser_based_global_registration_on (test/mulls_reg.cpp:170-186, test/mulls_slam.cpp:532-559): TEASER++'s
+ * RobustRegistrationSolver over the correspondences i <-> i with cbar2 = 1, fixed scale, GNC-TLS rotation (100
+ * iterations, factor 1.4, cost threshold 0.005) and the maximum clique. Stateless like mulls_coarse_reg_ransac: the
+ * batch resident on the context and its grid are left alone. 48-byte rows; only x y z are read, widened to double.
+ * Readings of TEASER++ as published (teaser_core.cuh T1-T9 state them in full; none is confirmed against a checkout):
+ *   - T1/T2 a pair i < j of correspondences is an edge of the consistency graph when the lengths of its source and
+ *     target TIMs (v_j - v_i) differ by at most 2 * noise_bound, each sqrt((x^2 + y^2) + z^2) in double; NaN: no edge
+ *   - T3 a maximum clique of that graph (PMC_EXACT), ascending; a clique of at most one vertex is an invalid solution
+ *   - T4-T6 GNC-TLS over the chain TIMs of the clique with the noise bound 2 * noise_bound; the rotation inliers are the
+ *     chain TIMs with weight >= 0.5, and their count is what min_inlier_num is compared with
+ *   - T7 the translation per axis by TLS adaptive voting over the clique's correspondences, ranges noise_bound
+ *   - T8 every sum in one fixed order (Eigen's depends on the machine), so the last bits can differ from a TEASER++ build
+ *   - T9 among several maximum cliques, the lexicographically smallest ascending index list (PMC leaves the choice to
+ *     its threads); equal voting boundaries in ascending signed key order
+ * Outputs: *status is -1 when the clouds differ in size or N <= 3 (the reference's refusals: not an error, nothing
+ * else written), when the solution is invalid or when the rotation-inlier count is below min_inlier_num; else 1 when
+ * the count is >= 2 * min_inlier_num and 0 otherwise (the comparisons are against size_t, so a negative min_inlier_num
+ * always gives -1). tran_mat (row-major) is written only when *status >= 0. info (may be NULL) reports the graph's
+ * edge count, its largest core number, the clique size, the rotation-inlier count, the GNC iterations (svdRot calls)
+ * and the number of search launches.
+ * A NULL tran_mat or status, or NULL rows with n > 0: MULLS_E_ARG. N above MULLS_TEASER_MAX_CORR or the context's
+ * max_tgt_pts: MULLS_E_CAPACITY. The clique search runs in launches in which each warp processes at most 2^18 64-bit
+ * words of the pruned graph; after MULLS_TEASER_SEARCH_LAUNCHES launches without an answer (about 30 s at most on an
+ * H100, sized to cover graphs one CPU thread solves in that time) it stops with MULLS_E_CAPACITY: a pathological graph ends with an error, never with a different clique. (TEASER++
+ * would keep searching for up to PMC's time limit of 3 600 s.) The context stays usable after any of these. */
+#define MULLS_TEASER_MAX_CORR 32768                    /* correspondences: 128 MiB of adjacency */
+#define MULLS_TEASER_SEARCH_LAUNCHES 4096              /* the clique search's budget */
+typedef struct mulls_teaser_info {
+    int64_t n_edges;      /* edges of the consistency graph */
+    int max_core;         /* its largest core number (the clique has at most max_core + 1 vertices) */
+    int clique_size;      /* the maximum clique's size */
+    int rotation_inliers; /* the count compared with min_inlier_num */
+    int gnc_iterations;   /* svdRot calls of the GNC-TLS loop */
+    int search_launches;  /* launches of the clique search */
+    int pad;
+} mulls_teaser_info;
+int mulls_coarse_reg_teaser(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_cloud_view source_pts, float noise_bound,
+                            int min_inlier_num, double tran_mat[16] /* row-major, written only when status >= 0 */,
+                            int *status, mulls_teaser_info *info);
 
 /* lo::CFilter<PointT>::non_max_suppress(cloud_in_out, non_max_radius, kd_tree_already_built = false), cfilter.hpp:1183-1240:
  * the keypoint suppression in front of the NCC matching (test/mulls_reg.cpp:145-149, test/mulls_slam.cpp:462). Stateless

@@ -77,6 +77,12 @@ class IcpTrace(C.Structure):
     ]
 
 
+class TeaserInfo(C.Structure):
+    """mulls_teaser_info"""
+    _fields_ = [("n_edges", C.c_int64), ("max_core", C.c_int), ("clique_size", C.c_int), ("rotation_inliers", C.c_int),
+                ("gnc_iterations", C.c_int), ("search_launches", C.c_int), ("pad", C.c_int)]
+
+
 class RunStats(C.Structure):
     _fields_ = [
         ("kernel_launches", C.c_uint64),
@@ -345,6 +351,7 @@ EXPORTED_SYMBOLS = (
     "mulls_motion_compensation",
     "mulls_ncc_correspondences",
     "mulls_coarse_reg_ransac",
+    "mulls_coarse_reg_teaser",
     "mulls_non_max_suppress",
     "mulls_omp_ndt",
     "mulls_omp_ndt_kdtree",
@@ -431,6 +438,9 @@ def load_library() -> C.CDLL:
     lib.mulls_ncc_correspondences.restype = C.c_int
     lib.mulls_ncc_correspondences.argtypes = [vp, CloudView, CloudView, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32),
                                               C.POINTER(C.c_int32), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int)]
+    lib.mulls_coarse_reg_teaser.restype = C.c_int
+    lib.mulls_coarse_reg_teaser.argtypes = [vp, CloudView, CloudView, C.c_float, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int),
+                                            C.POINTER(TeaserInfo)]
     lib.mulls_coarse_reg_ransac.restype = C.c_int
     lib.mulls_coarse_reg_ransac.argtypes = [vp, CloudView, CloudView, C.c_float, C.c_int, C.c_int, C.POINTER(C.c_double),
                                             C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]

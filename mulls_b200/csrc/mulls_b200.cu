@@ -33,6 +33,7 @@
 #include "kernels_rawscan.cuh"
 #include "kernels_ncc.cuh"
 #include "kernels_ransac.cuh"
+#include "kernels_teaser.cuh"
 #include "kernels_ndt.cuh"
 #include "kernels_gicp.cuh"
 #include "kernels_gicp_pcl.cuh"
@@ -179,6 +180,8 @@ struct mulls_ctx {
     Scratch ndt_kd_buf;          // NDT with KDTREE: the per-point neighbour lists, grown to the longest list seen
     Scratch gicp_buf;            // GICP: clouds, covariances, voxel keys and sort scratch, voxels, tile sums, distances
     Scratch gicp_pcl_buf;        // point-wise GICP: clouds, covariances, correspondences, tile sums, distances
+    Scratch tm_buf;              // TEASER++: correspondences, graph, core numbers, GNC and voting state
+    Scratch tm_srch_buf;         // TEASER++: the pruned graph and the clique search's stacks
     void *rc_host = nullptr;     // pinned: two chunks of sample triples and their counts
     // the local map whose clouds the target slices of pair 0 currently index (set by mulls_icp_run_to_map, cleared
     // by any other upload): what block1->tree_* are to MapManager::map_based_dynamic_close_removal
@@ -1979,6 +1982,224 @@ int mulls_coarse_reg_ransac(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_c
         return ransac_impl(ctx, target_pts, source_pts, noise_bound, min_inlier_num, max_iter_num, tran_mat, status, n_inliers,
                            n_hypotheses, launches);
     });
+}
+
+// ================================================================================================
+// TEASER++ coarse registration (CRegistration::coarse_reg_teaser, cregistration.hpp:664-759): teaser_core.cuh,
+// kernels_teaser.cuh. Stateless like the RANSAC: the resident batch and its grid are left alone.
+// The graph, its core numbers and a greedy clique come first. Vertices whose core number is below the greedy size
+// minus one cannot be in a maximum clique and are dropped. Unless the greedy clique already meets the core bound, a
+// kTmMax search finds the clique number; a kTmLex search then finds the lexicographically smallest clique of that
+// size. Both run in launches of at most kTmLaunchWords words per warp, the host relaunching until the search is done.
+// ================================================================================================
+static constexpr int kTmHindexBatch = 4;                           // h-index steps between two looks at the flag
+static constexpr unsigned long long kTmLaunchWords = 1ull << 18;   // search work per warp and launch
+static constexpr int kTmMaxSlots = 2048;                           // warps of one search launch, at most
+static constexpr size_t kTmStackBytes = (size_t)256 << 20;         // the stacks of all slots together, at most
+static constexpr size_t kTmKeepBytes = (size_t)64 << 20;           // search scratch a context keeps after a call, at most
+
+static int teaser_impl(mulls_ctx *ctx, mulls_cloud_view tv, mulls_cloud_view sv, float noise_bound, int min_inlier_num,
+                       double *tran_mat, int *status, mulls_teaser_info *info_out, uint64_t &launches) {
+    if (!tran_mat || !status || (tv.n && !tv.aos48) || (sv.n && !sv.aos48)) return MULLS_E_ARG;
+    const char *fn = "mulls_coarse_reg_teaser";
+    mulls_teaser_info info{};
+    const size_t N = tv.n;
+    if (sv.n != N || N <= 3) { // cregistration.hpp:675-685
+        *status = -1;
+        if (info_out) *info_out = info;
+        return MULLS_OK;
+    }
+    if (N > (size_t)MULLS_TEASER_MAX_CORR) {
+        ctx->err = std::string(fn) + ": " + std::to_string(N) + " correspondences exceed MULLS_TEASER_MAX_CORR (" +
+                   std::to_string(MULLS_TEASER_MAX_CORR) + ")";
+        return MULLS_E_CAPACITY;
+    }
+    int rc;
+    if ((rc = check_capacity(ctx, N, fn)) != MULLS_OK) return rc;
+    const int n = (int)N, W = (int)ceil_div(N, 64);
+    const double nb = (double)noise_bound;
+    int padded = 1;
+    while (padded < 2 * n) padded <<= 1;
+    cudaStream_t st = ctx->stream;
+    // ---- the graph, the core numbers, the greedy clique ----
+    double *d_p6, *d_tims, *d_w, *d_r, *d_R, *d_x3, *d_t;
+    uint64_t *d_adj, *d_cand;
+    int *d_core, *d_small, *d_clique, *d_gout;
+    unsigned long long *d_edges;
+    uint8_t *d_mask;
+    TmBound *d_bnd;
+    ScratchLayout L;
+    L.take(d_p6, 6 * N), L.take(d_adj, N * W), L.take(d_core, N), L.take(d_small, 2), L.take(d_edges, 1), L.take(d_cand, W);
+    L.take(d_clique, N), L.take(d_tims, 6 * N), L.take(d_w, N), L.take(d_r, N), L.take(d_mask, N), L.take(d_R, 9);
+    L.take(d_gout, 2), L.take(d_x3, 3 * N), L.take(d_bnd, 3 * (size_t)padded), L.take(d_t, 3);
+    if ((rc = L.grow(ctx, ctx->tm_buf)) != MULLS_OK) return rc;
+    std::vector<double> p6(6 * N); // solve(src, dst): source x y z, target x y z, widened
+    for (size_t i = 0; i < N; ++i)
+        for (int c = 0; c < 3; ++c) p6[6 * i + c] = (double)sv.aos48[12 * i + c], p6[6 * i + 3 + c] = (double)tv.aos48[12 * i + c];
+    CK(cudaMemcpyAsync(d_p6, p6.data(), 6 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(d_core, 0, N * sizeof(int), st));
+    CK(cudaMemsetAsync(d_edges, 0, sizeof(unsigned long long), st));
+    k_tm_graph<<<(unsigned)ceil_div(N * W, kTmGraphBlock), kTmGraphBlock, 0, st>>>(d_p6, n, W, 2.0 * nb, d_adj, d_core, d_edges);
+    ++launches;
+    const unsigned hb = (unsigned)ceil_div(N, kTmWarpsPerBlock);
+    for (;;) { // h-index steps from the degrees until one changes nothing
+        for (int b = 0; b < kTmHindexBatch; ++b) {
+            if (b == kTmHindexBatch - 1) CK(cudaMemsetAsync(d_small, 0, sizeof(int), st));
+            k_tm_hindex<<<hb, 32 * kTmWarpsPerBlock, 0, st>>>(d_adj, n, W, d_core, d_small);
+            ++launches;
+        }
+        int changed = 0;
+        CK(cudaMemcpyAsync(&changed, d_small, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (!changed) break;
+    }
+    k_tm_greedy<<<1, kTmGreedyBlock, 0, st>>>(d_adj, n, W, d_core, d_cand, d_small + 1);
+    ++launches;
+    std::vector<int> core(N);
+    int lb = 0;
+    unsigned long long edges2 = 0;
+    CK(cudaMemcpyAsync(core.data(), d_core, N * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&lb, d_small + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&edges2, d_edges, sizeof(edges2), cudaMemcpyDeviceToHost, st));
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    info.n_edges = (int64_t)(edges2 / 2);
+    for (int c : core) info.max_core = std::max(info.max_core, c);
+    const int ub = info.max_core + 1;
+    int omega = lb;
+    std::vector<int> clique;
+    if (lb >= 2) { // an edge exists
+        // ---- the pruned graph and the search ----
+        std::vector<int> map, map_core, rcore;
+        for (int i = 0; i < n; ++i)
+            if (core[i] >= lb - 1) map.push_back(i);
+        map_core = map; // kTmMax: ascending core number, then index
+        std::stable_sort(map_core.begin(), map_core.end(), [&](int a, int b) { return core[a] < core[b]; });
+        for (int v : map_core) rcore.push_back(core[v]);
+        const int n2 = (int)map.size(), W2 = (int)ceil_div((size_t)n2, 64), levels = ub + 1;
+        const size_t per_slot = (size_t)levels * (W2 * sizeof(uint64_t) + sizeof(int) + sizeof(TmLevel) + kTmOrder * sizeof(int2));
+        size_t slots = std::min<size_t>({(size_t)kTmMaxSlots, ceil_div((size_t)n2, kTmWarpsPerBlock) * kTmWarpsPerBlock,
+                                         std::max<size_t>(kTmStackBytes / per_slot, 1)});
+        slots = ceil_div(slots, kTmWarpsPerBlock) * kTmWarpsPerBlock;
+        int *d_map, *d_rcore;
+        TmSearchArgs S{};
+        ScratchLayout L2;
+        L2.take(d_map, n2), L2.take(d_rcore, n2), L2.take(S.stack, slots * levels * W2), L2.take(S.path, slots * levels), L2.take(S.slots, slots);
+        L2.take(S.lvl, slots * levels), L2.take(S.ring, slots * levels * kTmOrder);
+        L2.take(S.ctl, 1);
+        uint64_t *d_adj2;
+        L2.take(d_adj2, (size_t)n2 * W2);
+        if ((rc = L2.grow(ctx, ctx->tm_srch_buf)) != MULLS_OK) return rc;
+        // the pruned graph with its vertices in the order `m`
+        auto compact = [&](const std::vector<int> &m) -> int {
+            CK(cudaMemcpyAsync(d_map, m.data(), n2 * sizeof(int), cudaMemcpyHostToDevice, st));
+            k_tm_compact<<<(unsigned)ceil_div((size_t)n2 * W2, kTmGraphBlock), kTmGraphBlock, 0, st>>>(d_adj, W, d_map, n2, W2, d_adj2);
+            ++launches;
+            return MULLS_OK;
+        };
+        CK(cudaMemcpyAsync(d_rcore, rcore.data(), n2 * sizeof(int), cudaMemcpyHostToDevice, st));
+        S.adj = d_adj2, S.core = d_rcore, S.n = n2, S.W = W2, S.levels = levels, S.ub = ub, S.launch_words = kTmLaunchWords;
+        TmCtl h{};
+        auto search = [&](int mode, int target, int best0) -> int {
+            TmCtl c0{};
+            c0.best = best0;
+            c0.found = ~0ull;
+            CK(cudaMemcpyAsync(S.ctl, &c0, sizeof(c0), cudaMemcpyHostToDevice, st));
+            CK(cudaMemsetAsync(S.slots, 0xff, slots * sizeof(TmSlot), st)); // task -1: none
+            S.mode = mode, S.target = target;
+            unsigned long long work_seen = 0;
+            for (;;) {
+                CK(cudaMemsetAsync(&S.ctl->active, 0, sizeof(int), st));
+                const unsigned nb = (unsigned)(slots / kTmWarpsPerBlock), nt = 32 * kTmWarpsPerBlock;
+                if (W2 <= 32) k_tm_search<1><<<nb, nt, 0, st>>>(S);
+                else if (W2 <= 64) k_tm_search<2><<<nb, nt, 0, st>>>(S);
+                else if (W2 <= 128) k_tm_search<4><<<nb, nt, 0, st>>>(S);
+                else if (W2 <= 256) k_tm_search<8><<<nb, nt, 0, st>>>(S);
+                else k_tm_search<16><<<nb, nt, 0, st>>>(S);
+                ++launches, ++info.search_launches;
+                CK(cudaMemcpyAsync(&h, S.ctl, sizeof(h), cudaMemcpyDeviceToHost, st));
+                CK(cudaGetLastError());
+                CK(cudaStreamSynchronize(st));
+                const bool stop = mode == kTmLex ? h.found != ~0ull : h.best >= ub;
+                if (h.active == 0 && (stop || h.next_task >= n2)) break;
+                if (info.search_launches >= MULLS_TEASER_SEARCH_LAUNCHES) {
+                    ctx->err = std::string(fn) + ": the maximum-clique search used MULLS_TEASER_SEARCH_LAUNCHES launches (" +
+                               std::to_string(n2) + " vertices after pruning, clique bound " + std::to_string(ub) +
+                               (mode == kTmMax ? ", proving the clique number; best so far " + std::to_string(h.best)
+                                               : ", finding the smallest clique of " + std::to_string(target)) + ")";
+                    return MULLS_E_CAPACITY;
+                }
+                if (h.work == work_seen) { // every launch takes a root or expands a node
+                    ctx->err = std::string(fn) + ": a search launch made no progress";
+                    return MULLS_E_CUDA;
+                }
+                work_seen = h.work;
+            }
+            return MULLS_OK;
+        };
+        if (lb < ub) {
+            if ((rc = compact(map_core)) != MULLS_OK || (rc = search(kTmMax, 0, lb)) != MULLS_OK) return rc;
+            omega = h.best;
+        }
+        if ((rc = compact(map)) != MULLS_OK || (rc = search(kTmLex, omega, 0)) != MULLS_OK) return rc;
+        if (h.found == ~0ull) {
+            ctx->err = std::string(fn) + ": no clique of the size the search found";
+            return MULLS_E_CUDA;
+        }
+        std::vector<int> path(omega);
+        CK(cudaMemcpyAsync(path.data(), S.path + (size_t)(h.found & 0xffffffffu) * levels, omega * sizeof(int),
+                           cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        for (int v : path) clique.push_back(map[v]);
+    }
+    info.clique_size = omega;
+    const bool valid = omega >= 2; // T3: a clique of at most one vertex
+    double R[9], t[3];
+    if (valid) {
+        // ---- GNC-TLS and the voting ----
+        const int M = omega;
+        CK(cudaMemcpyAsync(d_clique, clique.data(), M * sizeof(int), cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(d_gout, 0, 2 * sizeof(int), st));
+        TmGncArgs G{d_p6, d_clique, M, nb, d_tims, d_w, d_r, d_mask, d_R, d_gout};
+        k_tm_gnc<<<1, kTmLanes, 0, st>>>(G);
+        int pm = 1;
+        while (pm < 2 * M) pm <<= 1;
+        k_tm_vote<<<3, kTmVoteBlock, 0, st>>>(d_p6, d_clique, M, d_R, nb, d_x3, d_bnd, pm, d_t);
+        launches += 2;
+        int gout[2];
+        CK(cudaMemcpyAsync(gout, d_gout, sizeof(gout), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(R, d_R, sizeof(R), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(t, d_t, sizeof(t), cudaMemcpyDeviceToHost, st));
+        CK(cudaGetLastError());
+        CK(cudaStreamSynchronize(st));
+        info.gnc_iterations = gout[0];
+        info.rotation_inliers = gout[1];
+    }
+    // inliers.size() >= min_inlier_num: int against size_t, so a negative minimum is never reached
+    const size_t cnt = (size_t)info.rotation_inliers;
+    const size_t lo = (size_t)(int64_t)min_inlier_num, hi = (size_t)(int64_t)(int32_t)((uint32_t)min_inlier_num * 2u);
+    int stat = -1;
+    if (valid && cnt >= lo) {
+        stat = cnt >= hi ? 1 : 0;
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) tran_mat[4 * r + c] = R[3 * r + c];
+            tran_mat[4 * r + 3] = t[r];
+        }
+        tran_mat[12] = tran_mat[13] = tran_mat[14] = 0.0;
+        tran_mat[15] = 1.0;
+    }
+    *status = stat;
+    if (info_out) *info_out = info;
+    return MULLS_OK;
+}
+int mulls_coarse_reg_teaser(mulls_ctx *ctx, mulls_cloud_view target_pts, mulls_cloud_view source_pts, float noise_bound,
+                            int min_inlier_num, double tran_mat[16], int *status, mulls_teaser_info *info) {
+    const int rc = front_call(ctx, [&](uint64_t &launches) {
+        return teaser_impl(ctx, target_pts, source_pts, noise_bound, min_inlier_num, tran_mat, status, info, launches);
+    });
+    // a hard graph can take hundreds of MiB of search stacks: do not keep them on the context (the stream has drained)
+    if (ctx && ctx->tm_srch_buf.bytes > kTmKeepBytes) ctx->tm_srch_buf.release();
+    return rc;
 }
 
 // ================================================================================================

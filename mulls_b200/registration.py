@@ -399,6 +399,22 @@ class Context:
                                                      C.byref(nh)))
         return st.value, buf.reshape(4, 4), ni.value, nh.value
 
+    def coarse_reg_teaser(self, target_pts: np.ndarray, source_pts: np.ndarray, noise_bound: float = 0.2,
+                          min_inlier_num: int = 8, tran_mat=None):
+        """CRegistration::coarse_reg_teaser (cregistration.hpp:664-759) on the GPU over the correspondences i <-> i.
+        Returns (status, tran_mat, info): status 1 (reliable), 0 (need check) or -1 (failed); tran_mat is a (4, 4)
+        float64 copy of the given one (identity when None), replaced by the estimate when status >= 0; info a dict of
+        mulls_teaser_info (n_edges, max_core, clique_size, rotation_inliers, gnc_iterations, search_launches). The
+        resident batch is untouched."""
+        t, s = abi.as_aos48(target_pts), abi.as_aos48(source_pts)
+        T = np.array(np.eye(4) if tran_mat is None else tran_mat, np.float64).reshape(4, 4).copy()
+        buf = np.ascontiguousarray(T.ravel())
+        st, info = C.c_int(0), abi.TeaserInfo()
+        self._check(self.lib.mulls_coarse_reg_teaser(self.handle, abi.cloud_view(t), abi.cloud_view(s), float(noise_bound),
+                                                     int(min_inlier_num), buf.ctypes.data_as(C.POINTER(C.c_double)),
+                                                     C.byref(st), C.byref(info)))
+        return st.value, buf.reshape(4, 4), {k: getattr(info, k) for k, _ in abi.TeaserInfo._fields_ if k != "pad"}
+
     def omp_ndt(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, ndt_resolution: float = 1.0,
                 use_direct_search: bool = True, initial_guess=None, apply_intersection_filter: bool = True,
                 fitness_score_thre: float = 10.0, trace_cap: int = 0):
@@ -713,6 +729,13 @@ class CRegistration:
         """lo::CRegistration::coarse_reg_ransac (cregistration.hpp:604-661): returns (status, tran_mat). tran_mat is the
         given (4, 4) matrix (identity when None), replaced by the estimate when status >= 0 and left as it was on -1."""
         status, T, _, _ = self._ctx.coarse_reg_ransac(target_pts, source_pts, noise_bound, min_inlier_num, max_iter_num, tran_mat)
+        return status, T
+
+    def coarse_reg_teaser(self, target_pts: np.ndarray, source_pts: np.ndarray, tran_mat=None, noise_bound: float = 0.2,
+                          min_inlier_num: int = 8):
+        """lo::CRegistration::coarse_reg_teaser (cregistration.hpp:664-759): returns (status, tran_mat). tran_mat is the
+        given (4, 4) matrix (identity when None), replaced by the estimate when status >= 0 and left as it was on -1."""
+        status, T, _ = self._ctx.coarse_reg_teaser(target_pts, source_pts, noise_bound, min_inlier_num, tran_mat)
         return status, T
 
     def omp_ndt(self, target: np.ndarray, source: np.ndarray, target_bound, source_bound, ndt_resolution: float = 1.0,
